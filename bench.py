@@ -3,8 +3,10 @@
 merge path (BASELINE.json config #2: 1e6 particles x 128-dim summaries per GPU, fp64), plus the
 north-star multi-GPU metric (SMC-ABC on MA2, N = 1e6, strong scaling) as the `smc_ma2` block.
 
-    python bench.py --gpus N --steps K --warmup W            # our arm (CUDA, sm_100a)
+    python bench.py --gpus N --steps K --warmup W            # our arm (CUDA, sm_90a)
+    python bench.py ... --dump-outputs DIR                   # + the last timed step's outputs
     python bench.py --impl reference --gpus N ...            # CPU arm: the UNMODIFIED reference
+                                                             # (needs ELFI_REFERENCE_ROOT)
 
 One "step" = one batch through the hot path exactly as `Rejection(d, batch_size=1e6)` runs it
 (SURVEY.md section 8d, config 2; elfi/model/utils.py:37-52, samplers.py:140-237):
@@ -20,7 +22,12 @@ rows (d, t1, t2) merged into the best-n state.  Inputs are the survey's config-2
               with HOST inputs: every step copies its 1.024 GB batch from pinned host memory to
               the device; the result (best-n rows) is read back to the host at the end.
 `roofline`  : algorithmic bytes (B*D*8 read + B*8 written) / CUDA-event time of the distance
-              kernel alone, against MEASURED_PEAKS.json's HBM copy bandwidth.
+              kernel alone, against MEASURED_PEAKS.json's HBM copy bandwidth when that file is
+              present, else against the H100 SXM data sheet's 3.35 TB/s.
+`--dump-outputs DIR`: after the timed steps, what the last one handed back -- its distances,
+              its accepted row indices and the best-n rows (d, t1, t2) of the timed steps -- as
+              DIR/<name>.npy (float64, 8.4 MB in all; rank 0).  The inputs are seeded, so two
+              builds can be compared output for output.
 `smc_ma2`   : SMC-ABC on MA2 in throughput mode, N = 1e6 particles x 5 populations, STRONG scaling
               over the ranks with the per-generation NCCL all-gather; preceded (N > 1) by an
               assert that the rank-sharded run equals the single-rank run bit for bit.
@@ -46,9 +53,7 @@ D = 128
 ACCEPT_Q = 0.01
 N_SAMPLES = 10_000
 WORKLOAD = 'rejection_dist_thr_merge_B1e6_D128_f64'
-# dram__bytes_read.sum + dram__bytes_write.sum of the distance kernel at this shape, from the
-# committed ncu --set full capture (1.024039 GB + 11.09 MB); algorithmic bytes are 1.032 GB
-NCU_DRAM_BYTES_PER_LAUNCH = 1.0351e9
+H100_DATASHEET_HBM_GBS = 3350.0      # H100 SXM data sheet, HBM3; a bound, never a measurement
 SMC = dict(population=1_000_000, populations=5, quantile=0.5, batch=125_000, seed=1)
 
 
@@ -57,7 +62,7 @@ def peaks():
     if os.path.exists(path):
         with open(path) as f:
             return float(json.load(f)['hbm_gbs']), 'measured'
-    return 6650.0, 'fallback'
+    return H100_DATASHEET_HBM_GBS, 'H100 SXM data sheet'
 
 
 def make_inputs(rank, pinned=False):
@@ -85,7 +90,7 @@ def config_dict(world, thr):
             'accept_quantile': ACCEPT_Q, 'threshold': thr, 'n_samples': N_SAMPLES,
             'inputs': 'S = RandomState(0).randn(1e6, 128) (rank r > 0: seed 1000 + r), '
                       'obs = RandomState(1).randn(1, 128), threshold = np.quantile(d, 0.01)',
-            'l2_policy': 'input (1.02 GB) larger than L2 (126 MB)',
+            'l2_policy': 'input (1.02 GB) larger than L2 (50 MB)',
             'parallelism': 'rows sharded x{}'.format(world)}
 
 
@@ -160,7 +165,7 @@ def dist_env():
 
 # ------------------------------------------------------------------------------ reference arm
 def run_reference(args):
-    """The unmodified reference (baseline/_ref mirror of /root/reference/elfi through
+    """The unmodified reference (the elfi-dev/elfi checkout named by ELFI_REFERENCE_ROOT, through
     oracle/ref_shim.py) on the host cores: its Distance operation on all cores + its
     Rejection.update merge, pipelined like its own batch loop (oracle/ref_arm.py)."""
     rank, local, world = dist_env()
@@ -239,18 +244,18 @@ def run_reference(args):
                 'd2h_bytes_per_step': 0},
         'reference_detail': extras,
     }
-    if not args.brief:      # lets our arm quote the reference's MA2 pipeline rate of the same box
-        try:
-            with open(os.path.join(ROOT, 'gpurun_out', 'bench_reference_last.json'), 'w') as f:
-                json.dump(line, f)
-        except OSError:
-            pass
     print(json.dumps(line), flush=True)
 
 
 def cpu_baseline_subprocess():
     """Rank 0, N = 1: the reference arm as a bounded subprocess (a fresh process: its worker pool
     is forked before anything touches CUDA)."""
+    sys.path.insert(0, os.path.join(ROOT, 'oracle'))
+    import ref_shim
+    if not ref_shim.reference_available():
+        return {'value': None, 'unit': 'accepted particles/s', 'cores': os.cpu_count(),
+                'kind': 'reference', 'sample': 'not run: ELFI_REFERENCE_ROOT names no elfi-dev/elfi '
+                                               'checkout'}
     try:
         out = subprocess.run([sys.executable, os.path.abspath(__file__), '--impl', 'reference',
                               '--steps', '5', '--warmup', '1', '--brief'],
@@ -553,6 +558,14 @@ def run_ours(args):
     barrier()
     ms_total = e0.elapsed_time(e1)
     assert dropped == 0 and count == args.steps * int(n_acc.item())
+    if args.dump_outputs and rank == 0:
+        n_last = int(n_acc.item())
+        dump = {'distances': d.cpu().numpy(),
+                'accepted_index': idx[:n_last].cpu().numpy().astype(np.float64),
+                'best_rows': best.cpu().numpy()}
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in dump.items():
+            np.save(os.path.join(args.dump_outputs, name + '.npy'), arr)
     # dominant kernel alone (distance + mask), per launch, CUDA events on the launch stream
     kev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
            for _ in range(args.steps)]
@@ -646,17 +659,6 @@ def run_ours(args):
            'ms_per_batch': api_dt / api_batches * 1e3, 'runs_s': [round(t, 4) for t in api_times],
            'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': int(api_res.n_samples) * 3 * 8,
            'posterior_mean_t1': api_mean}
-    ref_path = os.path.join(ROOT, 'gpurun_out', 'bench_reference_last.json')
-    if os.path.exists(ref_path):
-        try:
-            with open(ref_path) as f:
-                ref_api = json.load(f)['reference_detail'].get('ma2_rejection_api')
-            if ref_api and 'simulated_per_s' in ref_api:
-                api['reference_arm_same_box'] = ref_api
-                api['vs_reference_arm'] = api['simulated_particles_per_s'] / \
-                    ref_api['simulated_per_s']
-        except Exception:
-            pass
 
     del S, d, idx, cand
     torch.cuda.empty_cache()
@@ -696,13 +698,10 @@ def run_ours(args):
                             'lives in pinned host memory: H2D of the batch, distance, merge; '
                             'PCIe-bound'},
             'roofline': {'bound': 'hbm', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s',
-                         'frac': achieved / peak, 'traffic': NCU_DRAM_BYTES_PER_LAUNCH,
-                         'traffic_source': 'profiles/r1_dist_first_ncu_full.md (dram__bytes_read + '
-                                           'dram__bytes_write of one ncu --set full capture)',
-                         'peak_source': how,
+                         'frac': achieved / peak, 'peak_source': how,
                          'kernel': 'rowstream_kernel<EuclidConsumer>',
                          'kernel_ms': kernel_ms, 'algorithmic_bytes': alg_bytes,
-                         'frac_of_nominal_8TBs': achieved / 8000.0},
+                         'frac_of_datasheet': achieved / H100_DATASHEET_HBM_GBS},
             'api_throughput_mode': api,
             'smc_ma2': smc,
         }
@@ -723,15 +722,17 @@ def main():
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--brief', action='store_true',
                     help='reference arm: only the headline step (used for cpu_baseline)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step to DIR/<name>.npy')
     args = ap.parse_args()
-    os.makedirs(os.path.join(ROOT, 'gpurun_out'), exist_ok=True)
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
     # make sure the in-tree CUDA library and the oracle are built (no-op when up to date); with
     # torchrun only local rank 0 builds, the others wait for the files
     import __graft_entry__ as entry
     if int(os.environ.get('LOCAL_RANK', '0')) == 0:
         entry.build_cuda()
         entry.build_oracle()
-        entry.build_reference()
     else:
         t_wait = time.time() + 600
         while not os.path.exists(entry.LIB) and time.time() < t_wait:

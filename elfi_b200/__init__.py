@@ -1,4 +1,4 @@
-"""elfi_b200 -- B200-native (sm_100a) implementation of ELFI's data-parallel hot path.
+"""elfi_b200 -- H100-native (sm_90a) implementation of ELFI's data-parallel hot path.
 
 The package mirrors the operator / sampler API of elfi-dev/elfi for the batched
 summary -> distance -> threshold/top-n selection -> SMC weight path and the BOLFI GP

@@ -1,7 +1,7 @@
 """ctypes binding of libelfi_b200.so (the C ABI declared in include/elfi_b200.h).
 
 There is no CPU fallback: if the shared library is missing or a call fails, an exception is
-raised.  Build it with ``python -c "import __graft_entry__ as g; g.build()"`` (nvcc, sm_100a).
+raised.  Build it with ``python -c "import __graft_entry__ as g; g.build()"`` (nvcc, sm_90a).
 """
 import ctypes
 import os

@@ -1,6 +1,6 @@
 """BOLFI on the device: GP surrogate, LCBSC acquisition, Bayesian optimisation loop.
 
-Mirrors (file:line in /root/reference):
+Mirrors (file:line in elfi-dev/elfi):
   GPyRegression          elfi/methods/bo/gpy_regression.py:15-364   (duck type used by acquisition
                          and posterior code: input_dim, bounds, parameter_names, X, Y, noise,
                          n_evidence, is_sampling, predict, predict_mean, predictive_gradients,

@@ -1,4 +1,4 @@
-// common.cuh -- shared plumbing for the elfi_b200 CUDA library (sm_100a only).
+// common.cuh -- shared plumbing for the elfi_b200 CUDA library (sm_90a only).
 //
 // Error model of the C ABI: every entry point returns 0 on success and a negative
 // code on failure; the message is kept per host thread and read back with

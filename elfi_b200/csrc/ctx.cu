@@ -77,8 +77,8 @@ int elfi_b200_ctx_create(int device, elfi_b200_ctx** out) {
     ELFI_CUDA_OK(cudaSetDevice(device));
     cudaDeviceProp prop;
     ELFI_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        elfi::set_error("ctx_create: device %d is sm_%d%d; this library is built for sm_100a only",
+    if (prop.major != 9 || prop.minor != 0) {
+        elfi::set_error("ctx_create: device %d is sm_%d%d; this library is built for sm_90a only",
                         device, prop.major, prop.minor);
         return ELFI_B200_ERR_UNSUPPORTED;
     }

@@ -8,8 +8,9 @@
 //
 // Algorithmic traffic per particle: D*8 bytes read + K*8 bytes written (+ 1 bit of mask).
 // Roofline: HBM.  The fp64 pipe does 3 (unweighted) or 4 (weighted) issue slots per element,
-// ~20 % of the memory time at D=128 on B200, so the kernel is bandwidth bound as long as
-// the TMA pipeline keeps >= ~45 KiB in flight per SM (see rowstream.cuh).
+// under 10 % of the memory time at D=128 on an H100 SXM (data-sheet rates: 34 TFLOP/s fp64,
+// 3.35 TB/s), so the kernel is bandwidth bound as long as the TMA pipeline keeps enough rows in
+// flight per SM (see rowstream.cuh).
 #include <cstdlib>
 
 #include "rowstream.cuh"
@@ -283,7 +284,7 @@ struct NestedMomentsConsumer : NestedConsumer<KMAX> {
 // out[0*D + j] = mean_j, out[1*D + j] = M2_j from the per-warp shifted power sums.
 // Block (32 columns, 32 slices): slice y adds the warps y, y + 32, ... of its column, the slices
 // are then added in order -- a fixed summation tree, ~nwarps / 32 dependent loads per thread
-// (a single thread per column walking all ~1200 warps cost 0.15 ms of pure latency).
+// (a single thread per column walking all ~1000 warps is a chain of dependent loads).
 __global__ void __launch_bounds__(1024)
 colmoments_flush_kernel(const double* __restrict__ S, const double* __restrict__ partial,
                         int64_t nwarps, int64_t B, int64_t D, double* __restrict__ out) {
@@ -309,9 +310,8 @@ colmoments_flush_kernel(const double* __restrict__ S, const double* __restrict__
 
 // Warps per CTA of the fused kernel: 12 when the ring still gets >= 3 slots next to the per-warp
 // accumulators (two warps per scheduler leave the fp64 pipe half idle: long dependent chains of
-// K + 2 accumulators per lane), else 8.  Measured at 5e5 x 256: K = 2 0.232 -> 0.214 ms, K = 6
-// 0.297 -> 0.279 ms; 16 warps (128 registers, 2-slot ring) gives the 8-warp time back, and the
-// plain nested kernels do not gain from either.  ELFI_B200_FUSED_WARPS=8 restores 8 (KMAX <= 8).
+// K + 2 accumulators per lane), else 8; 16 warps (128 registers, 2-slot ring) gives the
+// 8-warp time back, and the plain nested kernels do not gain from either.  ELFI_B200_FUSED_WARPS=8 restores 8 (KMAX <= 8).
 template <int KMAX>
 static int fused_moments_warps(elfi_b200_ctx* ctx, int64_t Dp, int64_t K) {
     int warps = 12;

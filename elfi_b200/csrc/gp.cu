@@ -8,8 +8,8 @@
 //        acquisition.py:296-301)
 //
 // Precision: the north_star asks for 1e-5 relative agreement of posterior mean / variance in
-// fp64; Ky has condition numbers ~1e6, so the factorisation stays in fp64.  tcgen05.mma has no
-// f64 kind, so the tensor-core path for this work is the DMMA instruction
+// fp64; Ky has condition numbers ~1e6, so the factorisation stays in fp64.  wgmma has no f64
+// kind, so the tensor-core path for this work is the DMMA instruction
 // mma.sync.aligned.m8n8k4.f64 (one NT GEMM kernel below does every O(n^3) / O(n^2 m) product:
 // the trailing updates of the blocked Cholesky, the recursive triangular inverse and the
 // n^2 m / 2 variance product  V = K* W^T).
@@ -65,16 +65,15 @@ struct GemmArgs {
 
 // C = alpha * A * B^T + beta * C on the fp64 tensor path.  CTA tile BM x BN x 16, WARPS_M x WARPS_N
 // warps, each a (BM / WARPS_M) x (BN / WARPS_N) tile of 8x8 DMMA tiles; 3-stage cp.async ring with
-// ONE block barrier per 16-wide slab (round 1: double buffering with two barriers, during which
-// the tensor pipe idled: ncu showed `wait` / `math_pipe_throttle` stalls at 58 % of the DMMA
-// peak); batch = grid.z.  Two instances:
+// ONE block barrier per 16-wide slab (double buffering with two barriers left the tensor pipe
+// idle at the barriers); batch = grid.z.  Two instances:
 //   128 x 128, 2 x 4 warps  -- the n^2 m / 2 prediction product and the large trailing updates;
 //    64 x  64, 2 x 2 warps  -- products with fewer than ~100 large tiles (the next-block-column
 //                              update of every Cholesky panel: 128 x 64 x 64 useful per CTA in a
 //                              128 x 128 tile; the levels of the recursive inverse: at most 64
-//                              large tiles on 148 SMs): four times the CTAs, three CTAs per SM.
-// (mma.m16n8k16.f64 is no alternative: ptxas lowers it to eight DMMA.8 on sm_100a,
-// profiles/r2_dmma_m16n8k16_sass.md.)
+//                              large tiles on 132 SMs): four times the CTAs, three CTAs per SM.
+// (On sm_90a ptxas emits a native DMMA.16x8x16 for mma.m16n8k16.f64; whether that shape beats
+// m8n8k4 here is not measured -- it also changes the order of the fp64 accumulation.)
 template <int BM, int BN, int WARPS_M, int WARPS_N, int BK>
 struct GemmCfg {
     static constexpr int THREADS = 32 * WARPS_M * WARPS_N;
@@ -277,8 +276,8 @@ static int launch_gemm(const GemmArgs& g, int64_t batch, cudaStream_t stream) {
     int64_t tiles = ((g.M + GM_BM - 1) / GM_BM) * ((g.N + GM_BN - 1) / GM_BN) * batch;
     if (g.mode == 1) tiles = tiles / 2 + 1;
     if (g.mode != 2 && tiles < small_below) return launch_gemm_cfg<64, 64, 2, 2, 16>(g, batch, stream);
-    // 32-wide slabs halve the block barriers of the large tile (221 KB of shared memory, 230
-    // registers): the 1e5 x 2000 grid prediction 16.40 -> 15.96 ms.  ELFI_B200_GEMM_BK32=0: 16.
+    // 32-wide slabs halve the block barriers of the large tile (221 KB of shared memory, within
+    // the 227 KB a block may opt in to; 230 registers).  ELFI_B200_GEMM_BK32=0: 16.
     static const bool wide_slab = [] {
         const char* v = getenv("ELFI_B200_GEMM_BK32");
         return !(v != nullptr && v[0] == '0');
@@ -372,8 +371,8 @@ potrf_diag_panel_kernel(double* __restrict__ A, int64_t lda, int64_t k, int64_t 
         // columns c = 2 cc + q of row r.  Per column j: the pivot owner publishes sqrt(a_jj), the
         // owners of column j scale it and publish it, everyone applies the rank-1 update from
         // the published column -- two block barriers per column and only the column itself goes
-        // through shared memory (the all-in-shared-memory version spent ~40 us per block in
-        // barrier + shared-memory latency; this one ~10 us).  j is a compile-time constant in
+        // through shared memory (the all-in-shared-memory version spent most of its time in
+        // barrier + shared-memory latency).  j is a compile-time constant in
         // the unrolled loop, so every register index is static.
         __shared__ double colj[GP_NB];
         __shared__ double piv_inv;
@@ -523,11 +522,11 @@ predict_rows_sq_kernel(const double* __restrict__ Ks, int64_t ld, int64_t mrows,
 // ---- K13: gradients / whitening for a few query points -----------------------------------------
 // Acquisition optimisers, NUTS chains and rank-b factor updates ask for t = W k_q, u = W^T t at a
 // handful of points per call.  Round 1 gave every point its own CTA, which walks the whole 16 MB
-// triangle of W with 8 warps: ~0.5 ms per triangular product however few points there are --
-// 1.0 ms per lock-step round of a 10-start LCBSC minimisation, the inner loop of BOLFI.fit.  The
+// triangle of W with 8 warps however few points there are -- twice per lock-step round of a
+// 10-start LCBSC minimisation, the inner loop of BOLFI.fit.  The
 // products are matrix-vector shaped: spread the ROWS of W over the grid instead (8 rows per CTA,
 // one per warp), keep the <= 16 right-hand sides of a chunk in shared memory, and W is read once
-// per chunk at L2 speed (m = 10, n = 2000: 1.01 -> 0.078 ms; W stays L2 resident between calls).
+// per chunk at L2 speed (W, 32 MB at n = 2000, fits the 50 MB L2 between calls).
 //   kx_j = s2 exp(f r2_j); t = W (kx + b); u = W^T t = Ky^-1 (kx + b);
 //   mean = (kx + b) . alpha ; var = s2 + b - |t|^2 ; grad_mu_d = sum_j dk_jd alpha_j ;
 //   grad_var_d = -2 sum_j dk_jd u_j with dk_jd = 2 f (x_d - X_jd) kx_j     (gpy_regression.py:211-218)

@@ -23,7 +23,8 @@
 //     byte count, so the expect_tx value is a constant 4096.
 //
 // Bytes in flight per SM = WARPS * (NS-1) * 4 KiB (160 KiB at WARPS=8, NS=6): several times
-// the ~45 KiB Little's-law requirement for 6.5 TB/s at ~1 us, so HBM latency is covered
+// the ~25 KiB per SM that Little's law asks for 3.35 TB/s (H100 SXM data sheet) at ~1 us of
+// latency over 132 SMs, so HBM latency is covered
 // without relying on occupancy.  Grid = one persistent CTA per SM; tiles are dealt
 // round-robin to the global warp index.
 #pragma once

@@ -514,7 +514,7 @@ rowsort_kernel(const double* __restrict__ X, int64_t ldX, int64_t B, int n, int 
 // consecutive elements L*KPL .. L*KPL + KPL-1, so compare-exchange distances j < KPL stay inside
 // a thread and j >= KPL are one shuffle per key with lane L ^ (j / KPL): no shared memory, no
 // bank conflicts, no __syncwarp between stages (the shared-memory network above spends its time
-// there: 6.9 ms for 1e6 x 256).  A lane's elements are contiguous in memory: 16-byte loads and
+// there).  A lane's elements are contiguous in memory: 16-byte loads and
 // stores when the row is aligned and entirely inside [0, n).
 __device__ __forceinline__ uint64_t shfl_xor_u64(uint64_t v, int m) {
     uint32_t lo = uint32_t(v), hi = uint32_t(v >> 32);

@@ -118,7 +118,7 @@ __device__ __forceinline__ void ma2_leaf_products(LeafSum& l1, LeafSum& l2, cons
 // products of the benchmark model): eight running sums per lag (leafsum.cuh) instead of the general
 // PairwiseStream tree with its per-level stack -- the kernel drops from 255 registers to well under
 // half, i.e. more than two resident blocks per SM for a kernel whose Box-Muller chains need the
-// latency hiding (0.79 ms for 1e6 x 100 at 8 warps per SM against ~0.3 ms of fp64-pipe time).
+// latency hiding (the kernel is latency bound, not fp64-pipe bound).
 template <bool WRITE_X, bool SUMMARIES, bool LEAF>
 __global__ void __launch_bounds__(128)
 sim_ma2_kernel(const double* __restrict__ t1, const double* __restrict__ t2, int64_t B, int n_obs,
@@ -303,7 +303,7 @@ __device__ __forceinline__ void leaf_feed8(LeafSum& s, int k0, const double (&t)
 // LEAF: n_obs <= 128, the row sums are single leaves of NumPy's pairwise sum (fewer registers, more
 // resident blocks; keeping the draws in registers to generate them only once was tried and is
 // slower -- 180 registers, two blocks per SM: the Box-Muller chains need the occupancy more than
-// they need the halved work: 0.715 against 0.562 ms for 1e6 x 50).
+// they need the halved work).
 template <bool WRITE_Y, bool LEAF>
 __global__ void __launch_bounds__(128)
 sim_gauss_kernel(const double* __restrict__ mu, const double* __restrict__ sigma, int64_t B, int n_obs,

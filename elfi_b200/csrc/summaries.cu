@@ -164,7 +164,7 @@ struct MeanVarConsumer {
 // and the box logic is AutocovBoxes / MeanVarBoxes, which also compile for the host.
 //   Sum = LeafSum   every reduced run has <= 128 terms, so NumPy's tree is one leaf and the state
 //                   is 8 accumulators per sum: same results as the consumers above at a fraction
-//                   of the integer bookkeeping (profiles/r1_summ_instruction_mix.md).  Default.
+//                   of the integer bookkeeping.  Default.
 //   Sum = TreeSum   longer rows, same front end; default for rows of more than 128 terms since its
 //                   device timing (ELFI_B200_SUMM_TERMWISE=0 falls back to the TermGrouper
 //                   consumers).
@@ -250,8 +250,8 @@ struct MeanVarRegsConsumer {
 
 // Contiguous rows whose pitch is an odd multiple of 16 bytes (n = 2 mod 4; the Gaussian model
 // has n = 50: 400-byte rows).  Through the 2-D tensor map such a matrix costs ceil(n/16) boxes
-// per 32 rows, the last one nearly empty (n = 50: 4 boxes for 3.125 boxes of data -- the
-// kernel ran at 0.6 of the HBM peak against 0.8 at n = 64), and no box row is line aligned.
+// per 32 rows, the last one nearly empty (n = 50: 4 boxes for 3.125 boxes of data), and no box
+// row is line aligned.
 // Here a tile is what it is in memory: 32 rows = ONE contiguous run of 32 * 8n bytes, fetched
 // by one 1-D bulk copy into the warp's ring slot.  No swizzle is needed: lane l reads 16-byte
 // chunk c of its row at l * 8n + 16c, and with 8n / 16 odd the eight lanes of a quarter-warp
@@ -380,9 +380,8 @@ static int rowgroup_launch(elfi_b200_ctx* ctx, const double* X, int64_t B, int64
 
 typedef TreeSum<RS_PW_DEPTH> RowTreeSum;
 
-// Rows of 129..7688 terms: the term-wise TreeSum front end is the default since it was timed on
-// the device (autocov(1,2) 4e5 x 256: 0.152 ms = 0.83 of the HBM peak against 0.225 ms = 0.56 for
-// the TermGrouper consumers; mean/var 0.183 against 0.350 ms; profiles/r2_kernels.md).
+// Rows of 129..7688 terms: the term-wise TreeSum front end is the default (it was faster on the
+// device than the TermGrouper consumers for both autocov and mean/var).
 // ELFI_B200_SUMM_TERMWISE=0 selects the round-1 consumers.
 static bool summaries_termwise() {
     static const bool on = [] {

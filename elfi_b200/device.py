@@ -16,7 +16,7 @@ _contexts = {}
 def require_cuda():
     if not torch.cuda.is_available():
         raise _lib.ElfiB200Error(
-            "elfi_b200 needs a CUDA device (B200, sm_100a); none is visible and there is no "
+            "elfi_b200 needs a CUDA device (H100, sm_90a); none is visible and there is no "
             "CPU fallback.")
 
 

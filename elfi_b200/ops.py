@@ -389,8 +389,8 @@ class CandidateBuffer:
     def bind_batch(self, S, obs, thresholds, d_out, acc_idx, n_acc, extras, w=None):
         """A zero-argument callable running ONE threshold-mode batch -- distances of S + acceptance
         + append of the accepted rows [d | extras] to this buffer -- as a single library call
-        (elfi_b200_rejection_batch_f64) with every argument marshalled once: ~10 us of host time
-        per batch, so that a busy host cannot starve a 0.17 ms kernel.  All tensors are device
+        (elfi_b200_rejection_batch_f64) with every argument marshalled once: microseconds of host
+        time per batch, so that a busy host cannot starve a sub-millisecond kernel.  All tensors are device
         tensors the caller keeps alive; `thresholds` is a host sequence or a device tensor."""
         S = _matrix(S)
         B, D = S.shape
@@ -501,7 +501,8 @@ def gm_logpdf(x, means, cov=1, weights=None, validate=True, mixed=False):
     x (N, p) and means (M, p) may be host or device arrays; returns a device tensor (N,).
     ``validate=False`` skips the two synchronising weight checks of normalize_weights
     (utils.py:80-88) for weights the caller produced itself.  ``mixed=True`` takes 2^f from the
-    fp32 special-function unit (term error <= 2e-7 instead of 2e-9, 1.3x faster): the throughput
+    fp32 special-function unit (term error <= 2e-7 instead of 2e-9, fewer fp64 instructions
+    per term): the throughput
     mode's choice, where parity with the reference is statistical."""
     means = _matrix(means)
     M, p = means.shape

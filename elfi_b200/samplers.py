@@ -1,6 +1,6 @@
 """Rejection / SMC-ABC samplers with the population arithmetic on the device.
 
-Host control flow mirrors the reference (file:line in /root/reference):
+Host control flow mirrors the reference (file:line in elfi-dev/elfi):
   ParameterInference.infer/iterate      elfi/methods/inference/parameter_inference.py:226-305
   Rejection                             elfi/methods/inference/samplers.py:57-317
   SMC                                   elfi/methods/inference/samplers.py:320-559
@@ -494,8 +494,8 @@ class Rejection(Sampler):
             # quantile / n_sim mode: every row of the batch is a candidate, as in the reference
             # (samplers.py:219-221).  Pruning with the buffer's current n-th distance would shrink
             # the merge sort, but the accepted COUNT then sizes the merge and costs one host round
-            # trip per batch (0.4 ms of a 1.5 ms throughput-mode batch, against 0.1 ms more sort
-            # work: the radix passes are latency bound at these sizes); without it nothing in this
+            # trip per batch (more than the extra sort work costs: the radix passes are latency
+            # bound at these sizes); without it nothing in this
             # mode waits for the device until the result is extracted.
             return None
         return {self.discrepancy_name: np.atleast_1d(np.asarray(thr, dtype=np.float64))}

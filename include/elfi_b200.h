@@ -1,5 +1,5 @@
 /*
- * elfi_b200.h -- C ABI of libelfi_b200.so: the B200 (sm_100a) implementation of ELFI's
+ * elfi_b200.h -- C ABI of libelfi_b200.so: the H100 (sm_90a) implementation of ELFI's
  * data-parallel sampler / BOLFI hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  ELFI is pure Python: the binding a
@@ -44,7 +44,7 @@ typedef struct elfi_b200_ctx elfi_b200_ctx;
 int elfi_b200_version(void);
 const char* elfi_b200_last_error(void);
 
-/* Creates the context of CUDA device `device` (must be compute capability 10.x). */
+/* Creates the context of CUDA device `device` (must be compute capability 9.0). */
 int elfi_b200_ctx_create(int device, elfi_b200_ctx** out);
 int elfi_b200_ctx_destroy(elfi_b200_ctx* ctx);
 /* Number of SMs of the context's device (grid sizing is a multiple of this). */
@@ -269,8 +269,8 @@ int elfi_b200_wquantile_f64(elfi_b200_ctx* ctx, const double* x, const double* w
  *   Tolerance: <= 1e-8 relative on q (range-reduced exp with a degree-6 minimax polynomial, max
  *   term error 1.9e-9; fp64 accumulation).
  * elfi_b200_gm_logpdf_mixed_f64: the same density with 2^f taken from the special-function unit in
- *   fp32 (range reduction and accumulation stay fp64): 1.3x faster, term error <= 2e-7 (measured
- *   2.4e-8 on the density of a 1e6-component mixture) -- used where parity with the reference is
+ *   fp32 (range reduction and accumulation stay fp64): fewer fp64 instructions per term, term
+ *   error <= 2e-7 -- used where parity with the reference is
  *   statistical anyway (throughput mode: device RNG), 50x inside the 1e-5 tolerance on SMC weights.
  *
  * elfi_b200_smc_weights_f64: w_i = exp(logprior_i - logq_i) (samplers.py:514).

@@ -1,5 +1,5 @@
 """Reference-side binding of libelfi_b200.so: the module a maintainer of elfi-dev/elfi would add
-(e.g. as ``elfi/b200_ops.py``) to run the hot path of an UNMODIFIED ELFI installation on a B200.
+(e.g. as ``elfi/b200_ops.py``) to run the hot path of an UNMODIFIED ELFI installation on an H100.
 
 It uses nothing but ctypes + the C ABI of include/elfi_b200.h (torch only allocates the device
 buffers and supplies the stream) and plugs into the reference through its own extension points:

@@ -6,7 +6,7 @@
  * (elfi_b200/) never does and has no CPU fallback.
  *
  * Every function names the reference call site it restates (paths relative to
- * /root/reference).  The arithmetic that lives in third-party code (SciPy cdist,
+ * elfi-dev/elfi).  The arithmetic that lives in third-party code (SciPy cdist,
  * NumPy pairwise reductions) is restated from the published algorithm and pinned
  * bit-for-bit against the installed scipy 1.18.1 / numpy 2.3.5 by
  * tests/test_oracle.py (those packages are what the reference itself calls).

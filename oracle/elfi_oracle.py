@@ -5,7 +5,7 @@ TEST INFRASTRUCTURE ONLY -- not part of the product.  Only ``tests/``,
 legs may import this module.  ``elfi_b200`` never does: the product path has no CPU
 fallback and fails loudly when the CUDA library is missing.
 
-Each function restates one reference function (paths relative to /root/reference) and
+Each function restates one reference function (paths relative to the root of elfi-dev/elfi) and
 is pinned against (i) the reference itself, imported with oracle/ref_shim.py when the
 golden fixtures under tests/golden/ were generated, and (ii) the installed SciPy/NumPy
 that the reference calls (tests/test_oracle.py).

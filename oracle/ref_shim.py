@@ -1,9 +1,10 @@
-"""Import the UNMODIFIED reference (elfi-dev/elfi): from /root/reference in the build container,
-else from the mirror baseline/_ref/ that __graft_entry__.build_reference() makes for the GPU box.
+"""Import the UNMODIFIED reference (elfi-dev/elfi) from the source checkout named by the
+environment variable ELFI_REFERENCE_ROOT (the directory that contains its `elfi` package).
 
 TEST / BASELINE INFRASTRUCTURE ONLY.  Used by tests/golden/gen_golden*.py to produce the
 committed golden fixtures, by the reference-driven plugin tests and by ``bench.py --impl
-reference`` (the CPU arm); never imported by the product (`elfi_b200/`).
+reference`` (the CPU arm); never imported by the product (`elfi_b200/`).  Without the variable
+those tests skip and the CPU arm is not run.
 
 The reference needs packages that are absent here (matplotlib, GPy, arviz, numdifftools,
 ipyparallel, dask, toolz) and uses NumPy-1 aliases; none of them touch the sampler hot
@@ -17,12 +18,12 @@ import numpy as np
 
 import os
 
-_MIRROR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'baseline', '_ref')
-REFERENCE_ROOT = '/root/reference' if os.path.isdir('/root/reference/elfi') else _MIRROR
+REFERENCE_ROOT = os.path.abspath(os.environ.get('ELFI_REFERENCE_ROOT') or os.devnull)
 
 
 def reference_available():
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, 'elfi'))
+    return 'ELFI_REFERENCE_ROOT' in os.environ and \
+        os.path.isdir(os.path.join(REFERENCE_ROOT, 'elfi'))
 
 
 def import_reference():

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Per-kernel device timings at the BASELINE shapes (CUDA events, warm, inputs > L2 or noted).
-Writes gpurun_out/kernels.json; summarised into profiles/ by hand.  Not the headline bench."""
+Writes bench_out/kernels.json.  Not the headline bench."""
 import ctypes
 import json
 import os
@@ -181,8 +181,8 @@ def main():
     except Exception as exc:   # keep the timings gathered so far
         out.append(dict(name='new-kernel section failed', error=repr(exc)))
         print(json.dumps(out[-1]), flush=True)
-    os.makedirs(os.path.join(ROOT, 'gpurun_out'), exist_ok=True)
-    with open(os.path.join(ROOT, 'gpurun_out', 'kernels.json'), 'w') as f:
+    os.makedirs(os.path.join(ROOT, 'bench_out'), exist_ok=True)
+    with open(os.path.join(ROOT, 'bench_out', 'kernels.json'), 'w') as f:
         json.dump(out, f, indent=1)
 
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Round-2 kernel timings (CUDA events around batches of back-to-back launches, so the per-call
 Python overhead overlaps with the previous kernel; median of the batches).  One JSON line per
-kernel + gpurun_out/r2_kernels[_TAG].json.  Variants selected by environment variables are
+kernel + bench_out/r2_kernels[_TAG].json.  Variants selected by environment variables are
 static per process: run the script once per variant (TAG names the output)."""
 import json
 import os
@@ -113,8 +113,8 @@ for N in (125_000, 1_000_000):
     out.append(e)
     print(json.dumps(e), flush=True)
     if N == 125_000:      # kept for an accuracy comparison between ELFI_B200_GM_MODE variants
-        np.save(os.path.join(ROOT, 'gpurun_out', 'gm_logq_{}.npy'.format(TAG)),
+        np.save(os.path.join(ROOT, 'bench_out', 'gm_logq_{}.npy'.format(TAG)),
                 ops.gm_logpdf(xs, means, cov, w, validate=False).cpu().numpy())
 
-with open(os.path.join(ROOT, 'gpurun_out', 'r2_kernels_{}.json'.format(TAG)), 'w') as f:
+with open(os.path.join(ROOT, 'bench_out', 'r2_kernels_{}.json'.format(TAG)), 'w') as f:
     json.dump(out, f, indent=1)

@@ -1,5 +1,5 @@
 """One short GPU call: summary-kernel parity tests, then CUDA-event timings of the two
-row-stream summary kernels on the benchmark shapes.  Writes gpurun_out/leaf_check.json."""
+row-stream summary kernels on the benchmark shapes.  Writes bench_out/leaf_check.json."""
 import json
 import os
 import sys
@@ -8,7 +8,7 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-os.makedirs(os.path.join(ROOT, 'gpurun_out'), exist_ok=True)
+os.makedirs(os.path.join(ROOT, 'bench_out'), exist_ok=True)
 rc = pytest.main(['-x', '-q', '-m', 'gpu', os.path.join(ROOT, 'tests', 'test_summaries_gpu.py'),
                   os.path.join(ROOT, 'tests', 'test_model_gpu.py')])
 res = {'pytest_rc': int(rc)}
@@ -44,6 +44,6 @@ ms = timed(lambda: ops.autocov(z, lags=(1, 2)))
 res['autocov_tree_4e5x256_ms'] = ms
 res['autocov_tree_GBps'] = z.numel() * 8 / ms / 1e6
 print(json.dumps(res))
-with open(os.path.join(ROOT, 'gpurun_out', 'leaf_check.json'), 'w') as f:
+with open(os.path.join(ROOT, 'bench_out', 'leaf_check.json'), 'w') as f:
     json.dump(res, f, indent=1)
 sys.exit(int(rc))

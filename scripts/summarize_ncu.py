@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Summarise ncu output brought back in gpurun_out/ into small tracked files under profiles/.
+"""Summarise ncu output under bench_out/ into small markdown files under bench_out/.
 
-    python scripts/summarize_ncu.py <tag> [--rep gpurun_out/prof.ncu-rep] [--launches gpurun_out/launches.csv]
+    python scripts/summarize_ncu.py <tag> [--rep bench_out/prof.ncu-rep] [--launches bench_out/launches.csv]
 """
 import argparse
 import csv
@@ -38,13 +38,13 @@ def main():
     ap.add_argument('--rep', default=None)
     ap.add_argument('--launches', default=None)
     args = ap.parse_args()
-    os.makedirs('profiles', exist_ok=True)
+    os.makedirs('bench_out', exist_ok=True)
     if args.rep:
         raw = subprocess.run(['ncu', '-i', args.rep, '--page', 'raw', '--csv'],
                              capture_output=True, text=True).stdout
         rows = list(csv.reader(io.StringIO(raw)))
         hdr, units = rows[0], rows[1]
-        out = os.path.join('profiles', args.tag + '_ncu_full.md')
+        out = os.path.join('bench_out', args.tag + '_ncu_full.md')
         with open(out, 'w') as f:
             f.write('# ncu --set full capture: {}\n\n'.format(args.tag))
             f.write('source: `{}` (per launch; ncu serialises and replays, so compare shares, '
@@ -75,7 +75,7 @@ def main():
             a[0] += 1
             a[1] += v
         total = sum(a[1] for a in agg.values()) or 1.0
-        out = os.path.join('profiles', args.tag + '_launches.md')
+        out = os.path.join('bench_out', args.tag + '_launches.md')
         with open(out, 'w') as f:
             f.write('# ncu launch list: {}\n\n'.format(args.tag))
             f.write('`ncu --metrics gpu__time_duration.sum --clock-control none` (cold-cache, '

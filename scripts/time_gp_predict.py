@@ -14,7 +14,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-OUT = os.path.join(ROOT, 'gpurun_out')
+OUT = os.path.join(ROOT, 'bench_out')
 
 
 def child(tag):

@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100)')
     config.addinivalue_line('markers', 'first_device_run: written after the last GPU session; '
                                        'ordered after the device-verified tests')
 

@@ -1,6 +1,7 @@
-"""Generate the golden fixtures from the UNMODIFIED reference (/root/reference).
+"""Generate the golden fixtures from the UNMODIFIED reference (elfi-dev/elfi, imported through
+oracle/ref_shim.py from the checkout named by ELFI_REFERENCE_ROOT).
 
-Run in the build container only (the reference is not present on the GPU box):
+Run where a checkout of the reference is at hand (ELFI_REFERENCE_ROOT):
 
     python tests/golden/gen_golden.py
 

@@ -1,6 +1,7 @@
-"""Golden fixtures for the BOLFI sampling path, from the UNMODIFIED reference (/root/reference).
+"""Golden fixtures for the BOLFI sampling path, from the UNMODIFIED reference (elfi-dev/elfi,
+the checkout named by ELFI_REFERENCE_ROOT).
 
-    python tests/golden/gen_golden_bolfi.py          (build container only)
+    ELFI_REFERENCE_ROOT=<checkout> python tests/golden/gen_golden_bolfi.py
 
 * mcmc.npz            -- elfi.methods.mcmc.nuts / metropolis chains on analytic targets and the
                          ESS / R-hat of those chains (mcmc.py is pure NumPy).
@@ -136,7 +137,7 @@ def main():
     # generated in PyStan with Stan's ESS and split R-hat)
     import importlib.util
     spec = importlib.util.spec_from_file_location(
-        'ref_test_mcmc', '/root/reference/tests/unit/test_mcmc.py')
+        'ref_test_mcmc', os.path.join(os.environ['ELFI_REFERENCE_ROOT'], 'tests', 'unit', 'test_mcmc.py'))
     ref_test = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(ref_test)
     out['stan_chains'] = np.asarray(ref_test.chains_Stan)

