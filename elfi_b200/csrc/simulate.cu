@@ -12,35 +12,16 @@
 //                                 rejection of draws outside the prior support)
 // The random numbers are a pure function of (seed, stream, row, index): the simulator can be
 // replayed (e.g. to materialise X for a test) and any sharding of rows gives the same particles.
+// oracle/streams.py replays every kernel's counter layout in NumPy; tests/test_streams_gpu.py
+// compares the kernels with it element by element.
 #include <cstdlib>
 
 #include "gnkmath.cuh"
 #include "leafsum.cuh"
 #include "pairwise.cuh"
+#include "philox.cuh"
 
 namespace elfi {
-
-struct Philox {
-    uint32_t key0, key1;
-    __device__ __forceinline__ Philox(uint64_t seed) : key0(uint32_t(seed)), key1(uint32_t(seed >> 32)) {}
-    __device__ __forceinline__ uint4 operator()(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3) const {
-        uint32_t k0 = key0, k1 = key1;
-#pragma unroll
-        for (int r = 0; r < 10; ++r) {
-            const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-            const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-            const uint32_t n0 = hi1 ^ c1 ^ k0, n2 = hi0 ^ c3 ^ k1;
-            c0 = n0; c1 = lo1; c2 = n2; c3 = lo0;
-            k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-        }
-        return make_uint4(c0, c1, c2, c3);
-    }
-};
-
-__device__ __forceinline__ double u01(uint32_t a, uint32_t b) {   // (0, 1], 53 bits
-    const uint64_t v = (uint64_t(a) << 21) ^ uint64_t(b >> 11);
-    return (double(v & ((uint64_t(1) << 53) - 1)) + 1.0) * (1.0 / 9007199254740992.0);
-}
 
 // two standard normals from one Philox block (Box-Muller)
 __device__ __forceinline__ void normal2(const uint4& r, double& n0, double& n1) {
@@ -261,8 +242,12 @@ __global__ void gm_rvs_kernel(const double* __restrict__ means, int64_t ldm, con
 
 // ---- Gaussian noise model (elfi/examples/gauss.py) --------------------------------------------------
 // priors of get_model(): mu ~ U(mu_lo, mu_lo + mu_w); sigma ~ truncnorm(a, b) (standard normal
-// truncated to [a, b], scipy convention with loc 0, scale 1).
-struct GaussPrior { double mu_lo, mu_w, a, b, cdf_a, cdf_w; };
+// truncated to [a, b], scipy convention with loc 0, scale 1).  sigma is drawn by inverse-CDF
+// sampling of [lo, hi] = [a, b] with the result multiplied by sign = 1 or, when a > 0, of the
+// mirror image [-b, -a] with sign = -1: in the upper tail Phi(a) rounds to 1 (a >~ 8.3) and
+// Phi(b) - Phi(a) loses every digit, while Phi(-a) and Phi(-b) stay accurate.
+// cdf_lo = Phi(lo), cdf_w = Phi(hi) - Phi(lo) (the mass of the truncation).
+struct GaussPrior { double mu_lo, mu_w, a, b, lo, hi, sign, cdf_lo, cdf_w; };
 
 __global__ void prior_gauss_kernel(int64_t B, uint64_t seed, uint64_t offset, GaussPrior g,
                                    double* __restrict__ mu, double* __restrict__ sigma) {
@@ -273,8 +258,8 @@ __global__ void prior_gauss_kernel(int64_t B, uint64_t seed, uint64_t offset, Ga
     const uint4 r = ph(uint32_t(row), uint32_t(row >> 32), 0u, 0x47415553u);
     const double u = u01(r.x, r.y), v = u01(r.z, r.w);
     mu[i] = g.mu_lo + g.mu_w * u;
-    double sgm = normcdfinv(g.cdf_a + v * g.cdf_w);     // inverse-CDF sampling of the truncation
-    sigma[i] = fmin(fmax(sgm, g.a), g.b);
+    double sgm = normcdfinv(g.cdf_lo + v * g.cdf_w);    // inverse-CDF sampling of the truncation
+    sigma[i] = g.sign * fmin(fmax(sgm, g.lo), g.hi);
 }
 
 __global__ void logprior_gauss_kernel(const double* __restrict__ x, int64_t ld, int64_t B, GaussPrior g,
@@ -414,30 +399,74 @@ __global__ void logprior_box_kernel(const double* __restrict__ x, int64_t ld, in
     out[i] = inside ? box.logdens : -INFINITY;
 }
 
-// inclusive scan of w / sum(w) (single block; N up to a few million is fine: one pass each)
+// Inclusive running sum of the (unnormalised) weights, w == NULL: all ones; single block, N up to
+// a few million.  A tile is 1024 threads x GM_CDF_PER_THREAD consecutive weights: each thread adds
+// its weights sequentially, the thread totals are scanned (warp shuffles, then the warp totals left
+// to right) into each thread's base, and the running sums from that base are capped below by a
+// running maximum of the threads' last values.  The table is therefore nondecreasing, which the
+// binary search of gm_rvs_kernel needs: a plain tree scan adds in a different order for
+// neighbouring entries, and after a zero weight an entry can round one ulp below its predecessor,
+// so that the search skips the right component or lands on a zero-weight one.  Only additions in
+// a fixed order and maxima: the table is a deterministic function of the weights
+// (oracle/streams.py gm_cdf replays it bit for bit).
+constexpr int GM_CDF_PER_THREAD = 8;
+
 __global__ void __launch_bounds__(1024)
 cumsum_kernel(const double* __restrict__ w, int64_t n, double* __restrict__ out) {
-    __shared__ double ws[32];
+    constexpr int K = GM_CDF_PER_THREAD;
+    __shared__ double wsum[32], wmax[32];
     __shared__ double carry_s;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     if (tid == 0) carry_s = 0.0;
     __syncthreads();
-    for (int64_t base = 0; base < n; base += 1024) {
-        const int64_t i = base + tid;
-        const double v = i < n ? (w ? w[i] : 1.0) : 0.0;
-        double incl = v;
+    for (int64_t base = 0; base < n; base += 1024 * K) {
+        const int64_t i0 = base + int64_t(tid) * K;
+        double v[K];
+#pragma unroll
+        for (int j = 0; j < K; ++j) v[j] = i0 + j < n ? (w ? w[i0 + j] : 1.0) : 0.0;
+        double tot = v[0];
+#pragma unroll
+        for (int j = 1; j < K; ++j) tot += v[j];
+        double incl = tot;
         for (int o = 1; o < 32; o <<= 1) {
             const double t = __shfl_up_sync(0xffffffffu, incl, o);
             if (lane >= o) incl += t;
         }
-        if (lane == 31) ws[wid] = incl;
+        double excl = __shfl_up_sync(0xffffffffu, incl, 1);
+        if (lane == 0) excl = 0.0;
+        if (lane == 31) wsum[wid] = incl;
         __syncthreads();
         double woff = 0.0;
-        for (int k = 0; k < wid; ++k) woff += ws[k];
+        for (int k = 0; k < wid; ++k) woff += wsum[k];
         const double carry = carry_s;
-        if (i < n) out[i] = carry + woff + incl;
+        double run = carry + (woff + excl);
+        double r[K];
+        bool seen = false;                     // a nonzero weight among this thread's so far
+#pragma unroll
+        for (int j = 0; j < K; ++j) {
+            run += v[j];
+            seen = seen || v[j] != 0.0;
+            r[j] = seen ? run : -INFINITY;
+        }
+        // exclusive running maximum of the threads' last values, starting at the carry.  A
+        // thread's leading zero weights take that maximum, which is exactly the entry before
+        // them: a zero weight never gets a share of the table, not even one ulp.
+        double m = r[K - 1];
+        for (int o = 1; o < 32; o <<= 1) {
+            const double t = __shfl_up_sync(0xffffffffu, m, o);
+            if (lane >= o) m = fmax(m, t);
+        }
+        double pm = __shfl_up_sync(0xffffffffu, m, 1);
+        if (lane == 0) pm = carry;
+        if (lane == 31) wmax[wid] = m;
         __syncthreads();
-        if (tid == 1023) carry_s = carry + woff + incl;
+        pm = fmax(pm, carry);
+        for (int k = 0; k < wid; ++k) pm = fmax(pm, wmax[k]);
+#pragma unroll
+        for (int j = 0; j < K; ++j)
+            if (i0 + j < n) out[i0 + j] = fmax(r[j], pm);
+        __syncthreads();                       // carry_s, wsum and wmax have been read
+        if (tid == 1023) carry_s = fmax(r[K - 1], pm);
         __syncthreads();
     }
 }
@@ -551,8 +580,12 @@ int elfi_b200_gm_rvs_f64(elfi_b200_ctx* ctx, const double* means, int64_t ldm, c
 static elfi::GaussPrior make_gauss_prior(const double* prm) {
     elfi::GaussPrior g;
     g.mu_lo = prm[0]; g.mu_w = prm[1]; g.a = prm[2]; g.b = prm[3];
-    g.cdf_a = 0.5 * erfc(-g.a * 0.7071067811865476);
-    g.cdf_w = 0.5 * erfc(-g.b * 0.7071067811865476) - g.cdf_a;
+    const bool mirror = g.a > 0.0;
+    g.lo = mirror ? -g.b : g.a;
+    g.hi = mirror ? -g.a : g.b;
+    g.sign = mirror ? -1.0 : 1.0;
+    g.cdf_lo = 0.5 * erfc(-g.lo * 0.7071067811865476);
+    g.cdf_w = 0.5 * erfc(-g.hi * 0.7071067811865476) - g.cdf_lo;
     return g;
 }
 

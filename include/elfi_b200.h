@@ -365,10 +365,14 @@ int elfi_b200_probe_fp64_f64(elfi_b200_ctx* ctx, double* tflops_host);
  *   elfi_b200_gm_rvs_f64        GMDistribution.rvs (elfi/methods/utils.py:200-261): component by
  *                               weight, + MVN(0, Sigma) with Sigma = L L^T (Lchol_host, p <= 4),
  *                               redrawn until inside the support (0 = none, 1 = MA2 prior support,
- *                               2 = box: box_host = [lo_0..lo_{p-1}, hi_0..hi_{p-1}])
+ *                               2 = box: box_host = [lo_0..lo_{p-1}, hi_0..hi_{p-1}]).  At most
+ *                               1000 draws per row: when all of them fall outside the support,
+ *                               the 1000th draw is returned as it is (outside the support)
  *   elfi_b200_gm_cdf_f64        inclusive running sum of the (unnormalised) component weights, the
  *                               table np.random.choice(p=weights) builds on every call
- *                               (utils.py:239); one per population, reused by every batch of it
+ *                               (utils.py:239); one per population, reused by every batch of it.
+ *                               Nondecreasing whatever the weights (>= 0), so a zero-weight
+ *                               component is never drawn; deterministic
  *   elfi_b200_gm_rvs_cdf_f64    gm_rvs with that table (`cumw`, device, N) instead of the weights
  */
 int elfi_b200_prior_ma2_f64(elfi_b200_ctx* ctx, int64_t B, uint64_t seed, uint64_t offset,
