@@ -14,5 +14,6 @@ from .model import (AdaptiveDistance, Constant, Discrepancy, Distance, ElfiModel
 from .samplers import (SMC, AdaptiveDistanceSMC, AdaptiveThresholdSMC,  # noqa: F401
                        DensityRatioEstimation, GMDistribution, ModelPrior, Rejection)
 from .store import OutputPool  # noqa: F401
+from .priors import DeviceModelPrior  # noqa: F401
 from .bo import (BOLFI, LCBSC, BayesianOptimization, BolfiPosterior, GPyRegression,  # noqa: F401
                  ExpIntVar, MaxVar, RandMaxVar, UniformAcquisition)

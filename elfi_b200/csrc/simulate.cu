@@ -16,22 +16,14 @@
 // compares the kernels with it element by element.
 #include <cstdlib>
 
+#include "boxmuller.cuh"
 #include "gnkmath.cuh"
 #include "leafsum.cuh"
 #include "pairwise.cuh"
 #include "philox.cuh"
+#include "priors.cuh"
 
 namespace elfi {
-
-// two standard normals from one Philox block (Box-Muller)
-__device__ __forceinline__ void normal2(const uint4& r, double& n0, double& n1) {
-    const double u = u01(r.x, r.y), v = u01(r.z, r.w);
-    const double rad = sqrt(-2.0 * log(u));
-    double s, c;
-    sincospi(2.0 * v, &s, &c);
-    n0 = rad * c;
-    n1 = rad * s;
-}
 
 // ---- MA2 prior ------------------------------------------------------------------------------
 // mode 0: joint draw (t1, t2); mode 1: t1 only; mode 2: t2 given the t1 passed in.
@@ -200,7 +192,8 @@ sim_ma2_kernel(const double* __restrict__ t1, const double* __restrict__ t2, int
 
 // ---- Gaussian-mixture proposals ------------------------------------------------------------------
 // cumw: inclusive cumulative sum of the normalised weights (N); Lc: lower Cholesky factor of the
-// shared covariance (p x p, row-major, p <= 4).  support: 0 none, 1 MA2 prior support.
+// shared covariance (p x p, row-major, p <= 4).  support: 0 none, 1 MA2 prior support, 2 box.
+// Support 3 and p > 4 go to gm_rvs_wide_kernel below; this kernel is the p <= 4 path as it was.
 struct BoxSupport { double lo[4], hi[4]; };
 struct LowerFactor4 { double v[16]; };   // row-major p x p (p <= 4), passed by value
 
@@ -238,6 +231,69 @@ __global__ void gm_rvs_kernel(const double* __restrict__ means, int64_t ldm, con
         if (ok) break;
     }
     for (int a = 0; a < p; ++a) out[i * ldo + a] = x[a];
+}
+
+// The same proposals for p <= 16 and for support 3, "prior": a draw is kept iff the joint log
+// density of the prior table (priors.cuh) is finite, the rule of GMDistribution.rvs
+// (x[np.isfinite(prior_logpdf(x))], utils.py:200-261).  Trial t uses blocks 4t .. 4t + 2 of
+// SALT_GM_RVS exactly as gm_rvs_kernel does (component uniform, z_0 z_1, z_2 z_3), so for p <= 4
+// the two kernels draw the same particles; z_{4+2k}, z_{5+2k} come from block 8t + k of
+// SALT_GM_RVS_WIDE (k = 0 .. 5).  The factor is packed: row a of L starts at a (a + 1) / 2.
+constexpr uint32_t SALT_GM_RVS = 0x474d5256u, SALT_GM_RVS_WIDE = 0x474d5258u;
+struct PackedLower16 { double v[PRIOR_MAX_PARAMS * (PRIOR_MAX_PARAMS + 1) / 2]; };
+struct BoxSupport16 { double lo[PRIOR_MAX_PARAMS], hi[PRIOR_MAX_PARAMS]; };
+
+// PMAX (4, 8 or 16) >= p: the loops are unrolled over PMAX so that x[] and z[] stay in registers.
+template <int PMAX>
+__global__ void __launch_bounds__(128)
+gm_rvs_wide_kernel(const double* __restrict__ means, int64_t ldm, const double* __restrict__ cumw,
+                   int64_t N, int p, const PackedLower16 Lc, int64_t B, uint64_t seed,
+                   uint64_t offset, int support, const BoxSupport16 box, const PriorTable prior,
+                   double* __restrict__ out, int64_t ldo) {
+    const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= B) return;
+    const Philox ph(seed);
+    const uint64_t row = offset + uint64_t(i);
+    const uint32_t r0 = uint32_t(row), r1 = uint32_t(row >> 32);
+    const double total = cumw[N - 1];
+    double x[PMAX];
+    for (uint32_t trial = 0; trial < 1000u; ++trial) {
+        const uint4 r = ph(r0, r1, trial * 4u, SALT_GM_RVS);
+        const double u = u01(r.x, r.y) * total;
+        int64_t lo = 0, hi = N - 1;               // first index with cumw >= u
+        while (lo < hi) {
+            const int64_t mid = (lo + hi) >> 1;
+            if (cumw[mid] < u) lo = mid + 1; else hi = mid;
+        }
+        double z[PMAX];
+        normal2(ph(r0, r1, trial * 4u + 1u, SALT_GM_RVS), z[0], z[1]);
+        if (p > 2) normal2(ph(r0, r1, trial * 4u + 2u, SALT_GM_RVS), z[2], z[3]);
+#pragma unroll
+        for (int k = 0; k < (PMAX - 4) / 2; ++k)
+            if (4 + 2 * k < p) normal2(ph(r0, r1, trial * 8u + uint32_t(k), SALT_GM_RVS_WIDE),
+                                       z[4 + 2 * k], z[5 + 2 * k]);
+#pragma unroll
+        for (int a = 0; a < PMAX; ++a) {
+            if (a < p) {
+                double s = means[lo * ldm + a];
+#pragma unroll
+                for (int b = 0; b <= a; ++b) s = fma(Lc.v[a * (a + 1) / 2 + b], z[b], s);
+                x[a] = s;
+            }
+        }
+        bool ok = true;
+        if (support == 2) {
+#pragma unroll
+            for (int a = 0; a < PMAX; ++a)
+                if (a < p) ok = ok && x[a] >= box.lo[a] && x[a] <= box.hi[a];
+        } else if (support == 3) {
+            ok = isfinite(prior_joint_logpdf<PMAX>(prior.e, x, p));
+        }
+        if (ok) break;
+    }
+#pragma unroll
+    for (int a = 0; a < PMAX; ++a)
+        if (a < p) out[i * ldo + a] = x[a];
 }
 
 // ---- Gaussian noise model (elfi/examples/gauss.py) --------------------------------------------------
@@ -541,9 +597,43 @@ int elfi_b200_gm_rvs_cdf_f64(elfi_b200_ctx* ctx, const double* means, int64_t ld
                              int64_t ldo, void* stream_) {
     using namespace elfi;
     ELFI_REQUIRE(ctx && means && cumw && Lchol_host && (B == 0 || out), "gm_rvs: NULL argument");
-    ELFI_REQUIRE(N >= 1 && p >= 1 && p <= 4 && ldm >= p && ldo >= p, "gm_rvs: bad shape (p <= 4)");
-    ELFI_REQUIRE(support == 0 || (support == 1 && p == 2) || (support == 2 && box_host),
+    ELFI_REQUIRE(N >= 1 && p >= 1 && p <= PRIOR_MAX_PARAMS && ldm >= p && ldo >= p,
+                 "gm_rvs: bad shape (p <= 16)");
+    ELFI_REQUIRE(support == 0 || (support == 1 && p == 2) || ((support == 2 || support == 3) && box_host),
                  "gm_rvs: unknown support %d", support);
+    if (support == 3 || p > 4) {
+        // the wide kernel: support 3 (the prior table travels in box_host) or p > 4
+        PriorTable prior;
+        memset(&prior, 0, sizeof(prior));
+        if (support == 3) {
+            for (int a = 0; a < p; ++a) {
+                char why[160];
+                ELFI_REQUIRE(prior_entry_from_spec(box_host + PRIOR_SPEC_WORDS * a, &prior.e[a], why,
+                                                   sizeof(why)),
+                             "gm_rvs: prior parameter %d: %s", a, why);
+            }
+        }
+        BoxSupport16 box16;
+        memset(&box16, 0, sizeof(box16));
+        if (support == 2)
+            for (int a = 0; a < p; ++a) { box16.lo[a] = box_host[a]; box16.hi[a] = box_host[p + a]; }
+        if (B == 0) return ELFI_B200_OK;
+        cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+        ELFI_CUDA_OK(cudaSetDevice(ctx->device));
+        PackedLower16 Lp;
+        memset(&Lp, 0, sizeof(Lp));
+        for (int a = 0; a < p; ++a)
+            for (int b = 0; b <= a; ++b) Lp.v[a * (a + 1) / 2 + b] = Lchol_host[a * p + b];
+#define ELFI_GM_RVS_WIDE(PMAX)                                                                   \
+        gm_rvs_wide_kernel<PMAX><<<unsigned((B + 127) / 128), 128, 0, stream>>>(                  \
+            means, ldm, cumw, N, int(p), Lp, B, seed, offset, support, box16, prior, out, ldo)
+        if (p <= 4) ELFI_GM_RVS_WIDE(4);
+        else if (p <= 8) ELFI_GM_RVS_WIDE(8);
+        else ELFI_GM_RVS_WIDE(16);
+#undef ELFI_GM_RVS_WIDE
+        ELFI_CUDA_OK(cudaGetLastError());
+        return ELFI_B200_OK;
+    }
     BoxSupport box;
     memset(&box, 0, sizeof(box));
     if (support == 2)

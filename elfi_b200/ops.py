@@ -589,10 +589,12 @@ def gm_cdf(weights, n=None):
     return cumw
 
 
-def gm_rvs(means, cov, weights, size, seed, offset=0, support=0, box=None, cdf=None):
-    """GMDistribution.rvs on the device (elfi/methods/utils.py:200-261); support=1 keeps only
-    draws inside the MA2 prior support, support=2 inside ``box`` = (lo (p,), hi (p,)) (redrawn per
-    particle).  ``cdf`` = :func:`gm_cdf` of the weights (then ``weights`` is not read)."""
+def gm_rvs(means, cov, weights, size, seed, offset=0, support=0, box=None, cdf=None, prior=None):
+    """GMDistribution.rvs on the device (elfi/methods/utils.py:200-261) for p <= 16; support=1
+    keeps only draws inside the MA2 prior support, support=2 inside ``box`` = (lo (p,), hi (p,)),
+    support=3 where the joint log density of ``prior`` (a (p, 5) table of :func:`prior_logpdf`) is
+    finite (redrawn per particle).  ``cdf`` = :func:`gm_cdf` of the weights (then ``weights`` is
+    not read)."""
     means = _matrix(means)
     N, p = means.shape
     cov = np.atleast_2d(np.asarray(cov, dtype=np.float64))
@@ -603,6 +605,11 @@ def gm_rvs(means, cov, weights, size, seed, offset=0, support=0, box=None, cdf=N
     if support == 2:
         boxarr = np.ascontiguousarray(np.concatenate([np.asarray(box[0], dtype=np.float64),
                                                       np.asarray(box[1], dtype=np.float64)]))
+    elif support == 3:
+        boxarr = _prior_table(prior)
+        if boxarr.shape[0] != p:
+            raise ValueError('the prior table has {} parameters, the mixture {}'.format(
+                boxarr.shape[0], p))
     out = dev.empty((size, p))
     if cdf is None:
         cdf = gm_cdf(weights, N)
@@ -611,6 +618,73 @@ def gm_rvs(means, cov, weights, size, seed, offset=0, support=0, box=None, cdf=N
     _lib.call('elfi_b200_gm_rvs_cdf_f64', dev.context(), dev.ptr(means), _ld(means), dev.ptr(cdf), N,
               p, dev.ptr(L), size, int(seed), int(offset), int(support), dev.ptr(boxarr),
               dev.ptr(out), p, dev.stream_ptr())
+    return out
+
+
+# stock scipy.stats priors: a parameter is [kind, p0, p1, p2, p3], scipy's positional parameters
+# with loc and scale filled in (include/elfi_b200.h; elfi_b200.priors builds them from a model)
+PRIOR_KINDS = ('uniform', 'norm', 'truncnorm', 'expon', 'gamma', 'beta')
+PRIOR_SHAPES = {'uniform': (), 'norm': (), 'truncnorm': ('a', 'b'), 'expon': (), 'gamma': ('a',),
+                'beta': ('a', 'b')}
+MAX_PRIOR_PARAMS = 16
+PRIOR_SPEC_WORDS = 5
+
+
+def _prior_spec_error(spec):
+    """Why a [kind, p0, p1, p2, p3] row is invalid (the library's checks), or None."""
+    k = spec[0]
+    if k not in range(len(PRIOR_KINDS)):
+        return 'unknown kind {!r} (supported: {})'.format(k, ', '.join(PRIOR_KINDS))
+    name = PRIOR_KINDS[int(k)]
+    ns = len(PRIOR_SHAPES[name])
+    shapes, loc, scale = spec[1:1 + ns], spec[1 + ns], spec[2 + ns]
+    if not (np.isfinite(loc) and np.isfinite(scale) and scale > 0):
+        return 'loc must be finite and scale finite and > 0 (loc {}, scale {})'.format(loc, scale)
+    if name == 'truncnorm' and not shapes[0] < shapes[1]:
+        return 'truncnorm needs a < b (a {}, b {})'.format(*shapes)
+    if name in ('gamma', 'beta') and not all(np.isfinite(s) and s > 0 for s in shapes):
+        return '{} needs finite shape parameters > 0 ({})'.format(name, ', '.join(
+            '{} {}'.format(n, s) for n, s in zip(PRIOR_SHAPES[name], shapes)))
+    return None
+
+
+def _prior_table(specs):
+    t = np.ascontiguousarray(np.atleast_2d(np.asarray(specs, dtype=np.float64)))
+    if t.ndim != 2 or t.shape[1] != 5 or not 1 <= t.shape[0] <= MAX_PRIOR_PARAMS:
+        raise ValueError('a prior table is (p, 5) with 1 <= p <= {}, got shape {}'.format(
+            MAX_PRIOR_PARAMS, np.shape(specs)))
+    for i, row in enumerate(t):
+        why = _prior_spec_error(row)
+        if why:
+            raise ValueError('prior parameter {}: {}'.format(i, why))
+    return t
+
+
+def prior_rvs(spec, size, seed, offset=0):
+    """``size`` draws of one stock prior on the device: spec = [kind, p0, p1, p2, p3]
+    (PRIOR_KINDS, scipy's positional parameters).  Row i is a pure function of (seed, offset + i).
+    Returns a device tensor (size,)."""
+    t = _prior_table(spec)
+    if t.shape[0] != 1:
+        raise ValueError('prior_rvs draws one parameter; got {} specs'.format(t.shape[0]))
+    out = dev.empty((int(size),))
+    _lib.call('elfi_b200_prior_rvs_f64', dev.context(), dev.ptr(t), int(size), int(seed), int(offset),
+              dev.ptr(out), dev.stream_ptr())
+    return out
+
+
+def prior_logpdf(params, specs):
+    """Joint log density of independent stock priors at the rows of params (B, p): the sum, left
+    to right, of scipy.stats.<kind>.logpdf per column; -inf outside the support.  specs (p, 5).
+    Returns a device tensor (B,)."""
+    t = _prior_table(specs)
+    x = _matrix(params)
+    if x.shape[1] != t.shape[0]:
+        raise ValueError('params have {} columns, the prior table {} rows'.format(x.shape[1],
+                                                                                 t.shape[0]))
+    out = dev.empty((x.shape[0],))
+    _lib.call('elfi_b200_prior_logpdf_f64', dev.context(), dev.ptr(x), _ld(x), x.shape[0],
+              t.shape[0], dev.ptr(t), dev.ptr(out), dev.stream_ptr())
     return out
 
 

@@ -1,0 +1,162 @@
+"""Device priors and SMC proposals for any model whose priors are stock scipy.stats distributions.
+
+``DeviceModelPrior(model)`` checks that every parameter of the model is an independent Prior of a
+supported kind (uniform, norm, truncnorm, expon, gamma, beta; also ELFI's shorthands 'normal',
+'exponential', 'unif' and the scipy distribution objects) with constant scalar parameters, and
+then offers the throughput mode's two device paths for it:
+
+* ``.model``: a copy of the model whose priors draw on the device (ops.prior_rvs, keyed by the
+  batch's random state like the bundled examples' device priors); their pdf / logpdf are scipy's,
+  so the host ModelPrior of the copy is unchanged;
+* the ``device_proposal`` protocol of SMC / AdaptiveDistanceSMC / AdaptiveThresholdSMC:
+  ``rvs`` = the mixture proposal redrawn until the joint prior log density is finite
+  (ops.gm_rvs support 3, the rule of GMDistribution.rvs), ``logpdf`` = ops.prior_logpdf.
+
+    dp = elfi_b200.DeviceModelPrior(m)
+    elfi_b200.SMC(dp.model['d'], device_proposal=dp, batch_size=..., seed=...)
+
+Conditional priors (a parameter that is another node), vector priors (``size=``) and other
+distributions are rejected with a ValueError naming the node.
+"""
+from functools import partial
+
+import numpy as np
+import scipy.stats as ss
+
+from . import model as em
+from . import ops
+
+SUPPORTED = ops.PRIOR_KINDS
+
+
+def _key(random_state):
+    from .examples.gauss import _key as key
+    return key(random_state)
+
+
+def _kind_of(distribution):
+    """(kind name or None, description) of a Prior's distribution attribute."""
+    if isinstance(distribution, str):
+        name = distribution.lower()
+        name = em._SCIPY_SHORTHAND.get(name, name)
+        return (name if name in SUPPORTED else None), "'{}'".format(distribution)
+    if isinstance(distribution, DevicePriorDistribution):
+        return distribution.kind, distribution.kind
+    for name in SUPPORTED:
+        if distribution is getattr(ss, name):
+            return name, 'scipy.stats.' + name
+    if isinstance(distribution, ss.rv_continuous) or isinstance(distribution, ss.rv_discrete):
+        return None, 'scipy.stats.' + str(getattr(distribution, 'name', distribution))
+    return None, 'custom distribution {}'.format(getattr(distribution, '__name__', distribution))
+
+
+def prior_spec(kind, params):
+    """[kind index, p0, p1, p2, p3] of scipy's positional parameters, loc 0 and scale 1 by
+    default (as in scipy)."""
+    shapes = ops.PRIOR_SHAPES[kind]
+    params = [float(v) for v in params]
+    ns = len(shapes)
+    if len(params) < ns or len(params) > ns + 2:
+        raise ValueError('{} takes {} positional parameters ({}), got {}'.format(
+            kind, 'from {} to {}'.format(ns, ns + 2) if ns else 'at most 2',
+            ', '.join(shapes + ('loc', 'scale')), len(params)))
+    full = params + [0.0, 1.0][len(params) - ns:]
+    spec = [float(SUPPORTED.index(kind))] + full
+    return spec + [0.0] * (ops.PRIOR_SPEC_WORDS - len(spec))
+
+
+class DevicePriorDistribution:
+    """A stock prior that draws on the device: ``rvs`` returns a device tensor from
+    ops.prior_rvs keyed by the batch's random state; ``pdf`` / ``logpdf`` are scipy's."""
+
+    def __init__(self, kind):
+        self.kind = kind
+        self.scipy = getattr(ss, kind)
+        self.__name__ = 'device_' + kind
+
+    def rvs(self, *params, size=1, random_state=None):
+        n = int(np.prod(size))
+        return ops.prior_rvs(prior_spec(self.kind, params), n, _key(random_state))
+
+    def pdf(self, x, *params):
+        return self.scipy.pdf(x, *params)
+
+    def logpdf(self, x, *params):
+        return self.scipy.logpdf(x, *params)
+
+
+def _node_spec(model, name):
+    rec = model.record(name)
+    if not issubclass(rec.cls, em.RandomVariable):
+        raise ValueError("parameter '{}' is not a Prior ({})".format(name, rec.cls.__name__))
+    if rec.attrs.get('size') is not None:
+        raise ValueError("prior '{}' is a vector prior (size={}); only scalar priors run on the "
+                         "device".format(name, rec.attrs['size']))
+    kind, what = _kind_of(rec.attrs['distribution'])
+    if kind is None:
+        raise ValueError("prior '{}': {} is not supported on the device (supported: {})".format(
+            name, what, ', '.join(SUPPORTED)))
+    values = []
+    for i, parent in enumerate(rec.inputs):
+        prec = model.record(parent)
+        if not issubclass(prec.cls, em.Constant):
+            raise ValueError("prior '{}': parameter {} depends on node '{}'; only priors with "
+                             "constant parameters run on the device".format(name, i, parent))
+        v = prec.constant
+        if np.ndim(v) != 0 or not np.isreal(v):
+            raise ValueError("prior '{}': parameter {} is not a real scalar ({!r})".format(
+                name, i, v))
+        values.append(float(np.real(v)))
+    try:
+        spec = prior_spec(kind, values)
+    except ValueError as e:
+        raise ValueError("prior '{}': {}".format(name, e)) from None
+    why = ops._prior_spec_error(np.asarray(spec))
+    if why:
+        raise ValueError("prior '{}': {}".format(name, why))
+    return kind, spec
+
+
+def _device_copy(model, kinds):
+    """The model with each named Prior drawing on the device (same name, parents, observed)."""
+    twin = model.copy()
+    for name, kind in kinds.items():
+        rec = twin.record(name)
+        dist = DevicePriorDistribution(kind)
+        new = rec.twin()
+        new.attrs = dict(rec.attrs, distribution=dist)
+        new.op = partial(em._draw, distribution=dist, size=None)
+        twin._records[name] = new
+    return twin
+
+
+class DeviceModelPrior:
+    """Joint prior of a model with stock scipy.stats priors, on the device (see the module
+    docstring).  ``parameter_names`` are the model's (sorted) parameter names; ``specs`` is the
+    (p, 5) table handed to the kernels."""
+
+    def __init__(self, model):
+        names = list(model.parameter_names)
+        if not names:
+            raise ValueError('the model has no parameters')
+        if len(names) > ops.MAX_PRIOR_PARAMS:
+            raise ValueError('{} parameters; the device priors take at most {}'.format(
+                len(names), ops.MAX_PRIOR_PARAMS))
+        kinds, specs = {}, []
+        for name in names:
+            kind, spec = _node_spec(model, name)
+            kinds[name] = kind
+            specs.append(spec)
+        self.parameter_names = names
+        self.kinds = [kinds[n] for n in names]
+        self.specs = np.asarray(specs, dtype=np.float64)
+        self.model = _device_copy(model, kinds)
+
+    def rvs(self, means, cov, weights, size, key, cdf=None):
+        """Mixture proposals (GMDistribution.rvs) redrawn until the joint prior density is
+        positive; a (size, p) device tensor."""
+        return ops.gm_rvs(means, cov, weights, size, seed=key, support=3, prior=self.specs, cdf=cdf)
+
+    def logpdf(self, params):
+        """Joint prior log density of the rows of params (B, p); a device tensor (B,)."""
+        return ops.prior_logpdf(params, self.specs)

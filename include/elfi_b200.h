@@ -363,11 +363,16 @@ int elfi_b200_probe_fp64_f64(elfi_b200_ctx* ctx, double* tflops_host);
  *                               the lag-1 / lag-2 autocovariances S (B, 2) (ma2.py:40-59, NumPy
  *                               pairwise order) so that X never has to touch HBM
  *   elfi_b200_gm_rvs_f64        GMDistribution.rvs (elfi/methods/utils.py:200-261): component by
- *                               weight, + MVN(0, Sigma) with Sigma = L L^T (Lchol_host, p <= 4),
- *                               redrawn until inside the support (0 = none, 1 = MA2 prior support,
- *                               2 = box: box_host = [lo_0..lo_{p-1}, hi_0..hi_{p-1}]).  At most
- *                               1000 draws per row: when all of them fall outside the support,
- *                               the 1000th draw is returned as it is (outside the support)
+ *                               weight, + MVN(0, Sigma) with Sigma = L L^T (Lchol_host, p <= 16),
+ *                               redrawn until inside the support (0 = none, 1 = MA2 prior support
+ *                               (p = 2), 2 = box: box_host = [lo_0..lo_{p-1}, hi_0..hi_{p-1}],
+ *                               3 = prior: box_host = the 5p-word prior table of
+ *                               elfi_b200_prior_logpdf_f64, a draw is kept iff its joint log
+ *                               density is finite).  At most 1000 draws per row: when all of them
+ *                               fall outside the support, the 1000th draw is returned as it is
+ *                               (outside the support).  For p <= 4 with supports 0-2 the streams
+ *                               are those of earlier versions; support 3 uses the same blocks, and
+ *                               z_4 .. z_15 come from a stream of their own
  *   elfi_b200_gm_cdf_f64        inclusive running sum of the (unnormalised) component weights, the
  *                               table np.random.choice(p=weights) builds on every call
  *                               (utils.py:239); one per population, reused by every batch of it.
@@ -392,6 +397,31 @@ int elfi_b200_gm_rvs_cdf_f64(elfi_b200_ctx* ctx, const double* means, int64_t ld
                              int64_t N, int64_t p, const double* Lchol_host, int64_t B, uint64_t seed,
                              uint64_t offset, int32_t support, const double* box_host, double* out,
                              int64_t ldo, void* stream);
+
+/* Stock scipy.stats priors (uniform, norm, truncnorm, expon, gamma, beta) on the device: the
+ * throughput-mode fast path of ModelPrior for independent priors with constant parameters.
+ * A parameter is five doubles [kind, p0, p1, p2, p3] with scipy's positional parameters, loc and
+ * scale filled in: 0 uniform (loc, scale), 1 norm (loc, scale), 2 truncnorm (a, b, loc, scale),
+ * 3 expon (loc, scale), 4 gamma (a, loc, scale), 5 beta (a, b, loc, scale); unused words ignored.
+ * Invalid parameters (scale <= 0, truncnorm a >= b, gamma a <= 0, beta a or b <= 0, an unknown
+ * kind, non-finite values) return ELFI_B200_ERR_ARG with a message naming the parameter index.
+ *   elfi_b200_prior_rvs_f64     B draws of ONE parameter (spec_host: 5 words) into out (B,);
+ *                               row i is a pure function of (seed, offset + i).  Uniform, norm,
+ *                               truncnorm (inverse CDF, mirrored in the upper tail) and expon take
+ *                               one Philox block per row; gamma and beta use Marsaglia-Tsang
+ *                               (stream layout in elfi_b200/csrc/prior.cu) with at most 64 trials
+ *                               per gamma component.  If all 64 are rejected (probability below
+ *                               1e-80 for every valid shape) the component's value is
+ *                               d = a - 1/3 (a >= 1) or a + 2/3 (a < 1), a point of the support
+ *   elfi_b200_prior_logpdf_f64  joint log density of p <= 16 independent parameters at the rows of
+ *                               x (B, p; leading dimension ldx): the sum, left to right, of
+ *                               scipy.stats.<kind>.logpdf, -inf outside the closed support and
+ *                               scipy's values on its edges (spec_host: 5p words)
+ */
+int elfi_b200_prior_rvs_f64(elfi_b200_ctx* ctx, const double* spec_host, int64_t B, uint64_t seed,
+                            uint64_t offset, double* out, void* stream);
+int elfi_b200_prior_logpdf_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int64_t B, int64_t p,
+                               const double* spec_host, double* out, void* stream);
 
 /* Gaussian noise model of elfi/examples/gauss.py (1-d case): priors mu ~ U(prm[0], prm[0]+prm[1]),
  * sigma ~ truncnorm(prm[2], prm[3]) (gauss.py:118-126); simulator y = mu + sigma z (gauss.py:11-35)
