@@ -79,6 +79,13 @@ SIGNATURES = {
     'elfi_b200_sim_gnk_f64': [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_dbl, c_i64, c_i64, c_u64, c_u64,
                               c_ptr, c_i64, c_ptr],
     'elfi_b200_logprior_box_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
+    'elfi_b200_gnk_summaries_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, ctypes.c_int32,
+                                    c_ptr, c_ptr, c_i64, c_ptr],
+    'elfi_b200_sim_gnk_summaries_f64': [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_dbl, c_i64, c_i64, c_u64,
+                                        c_u64, ctypes.c_int32, c_ptr, c_ptr, c_i64, c_ptr],
+    'elfi_b200_sim_bignk_f64': [c_ptr, c_ptr, c_i64, c_dbl, c_i64, c_i64, c_u64, c_u64, c_ptr, c_i64,
+                                ctypes.c_int32, c_ptr, c_ptr, c_i64, c_ptr],
+    'elfi_b200_euclidean_multiss_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     'elfi_b200_prior_rvs_f64': [c_ptr, c_ptr, c_i64, c_u64, c_u64, c_ptr, c_ptr],
     'elfi_b200_prior_logpdf_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     'elfi_b200_gp_padded_size': [c_i64],

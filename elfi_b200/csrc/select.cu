@@ -12,6 +12,7 @@
 // distances) degenerate to a copy.
 #include <cstdlib>
 
+#include "bitonic.cuh"
 #include "eqweight.h"
 #include "pairwise.cuh"
 
@@ -19,17 +20,6 @@ namespace elfi {
 
 constexpr int SORT_CHUNK = 1024;   // keys per warp sub-chunk
 constexpr int SORT_WARPS = 8;      // warps per block
-
-__device__ __forceinline__ uint64_t key_to_u64(double d) {
-    if (d != d) return ~uint64_t(0);                 // NaN sorts last
-    uint64_t u = static_cast<uint64_t>(__double_as_longlong(d));
-    return (u >> 63) ? ~u : (u | (uint64_t(1) << 63));
-}
-__device__ __forceinline__ double u64_to_key(uint64_t u) {
-    if (u == ~uint64_t(0)) return __longlong_as_double(0x7ff8000000000000LL);
-    u = (u >> 63) ? (u & ~(uint64_t(1) << 63)) : ~u;
-    return __longlong_as_double(static_cast<long long>(u));
-}
 
 // keys -> u64, vals -> iota, and the 8 x 256 global digit histograms in one read.
 __global__ void __launch_bounds__(256)
@@ -493,70 +483,15 @@ rowsort_kernel(const double* __restrict__ X, int64_t ldX, int64_t B, int n, int 
     for (int64_t row = int64_t(blockIdx.x) * 8 + warp; row < B; row += int64_t(gridDim.x) * 8) {
         for (int i = lane; i < npow2; i += 32) sk[i] = i < n ? key_to_u64(X[row * ldX + i]) : ~uint64_t(0);
         __syncwarp();
-        for (int k = 2; k <= npow2; k <<= 1) {
-            for (int j = k >> 1; j > 0; j >>= 1) {
-                for (int t = lane; t < (npow2 >> 1); t += 32) {
-                    const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
-                    const int l = i | j;
-                    const bool up = (i & k) == 0;
-                    const uint64_t a = sk[i], b = sk[l];
-                    if ((a > b) == up) { sk[i] = b; sk[l] = a; }
-                }
-                __syncwarp();
-            }
-        }
+        bitonic_in_shared(sk, npow2, lane);
         for (int i = lane; i < n; i += 32) out[row * ld_out + i] = u64_to_key(sk[i]);
         __syncwarp();
     }
 }
 
-// Rows of up to 512 keys: the same network with the keys in REGISTERS.  Lane L holds the KPL
-// consecutive elements L*KPL .. L*KPL + KPL-1, so compare-exchange distances j < KPL stay inside
-// a thread and j >= KPL are one shuffle per key with lane L ^ (j / KPL): no shared memory, no
-// bank conflicts, no __syncwarp between stages (the shared-memory network above spends its time
-// there).  A lane's elements are contiguous in memory: 16-byte loads and
-// stores when the row is aligned and entirely inside [0, n).
-__device__ __forceinline__ uint64_t shfl_xor_u64(uint64_t v, int m) {
-    uint32_t lo = uint32_t(v), hi = uint32_t(v >> 32);
-    asm volatile("shfl.sync.bfly.b32 %0, %0, %2, 0x1f, 0xffffffff;\n\t"
-                 "shfl.sync.bfly.b32 %1, %1, %2, 0x1f, 0xffffffff;"
-                 : "+r"(lo), "+r"(hi) : "r"(m));
-    return (uint64_t(hi) << 32) | lo;
-}
-
-template <int KPL>
-__device__ __forceinline__ void bitonic_in_registers(uint64_t (&key)[KPL], int lane) {
-    constexpr int N = KPL * 32;
-#pragma unroll
-    for (int k = 2; k <= N; k <<= 1) {
-        // sort direction of the k-block the element sits in: bit k of i = L*KPL + r
-        const bool lane_up = (k >= N) ? true : ((lane & (k >= KPL ? k / KPL : 1)) == 0);
-#pragma unroll
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            if (j >= KPL) {
-                const int m = j / KPL;
-                const bool keep_min = ((lane & m) == 0) == lane_up;
-#pragma unroll
-                for (int r = 0; r < KPL; ++r) {
-                    const uint64_t o = shfl_xor_u64(key[r], m);
-                    key[r] = ((o < key[r]) == keep_min) ? o : key[r];
-                }
-            } else {
-#pragma unroll
-                for (int r = 0; r < KPL; ++r) {
-                    if ((r & j) == 0) {
-                        const bool up = (k < KPL) ? ((r & k) == 0) : lane_up;
-                        const uint64_t a = key[r], b = key[r | j];
-                        const bool sw = (a > b) == up;
-                        key[r] = sw ? b : a;
-                        key[r | j] = sw ? a : b;
-                    }
-                }
-            }
-        }
-    }
-}
-
+// Rows of up to 512 keys: the register network of bitonic.cuh.  A lane's elements are
+// contiguous in memory: 16-byte loads and stores when the row is aligned and entirely inside
+// [0, n).
 template <int KPL>
 __global__ void __launch_bounds__(256)
 rowsort_regs_kernel(const double* __restrict__ X, int64_t ldX, int64_t B, int n_,

@@ -1,5 +1,9 @@
 """Univariate g-and-k model (mirror of elfi/examples/gnk.py) + the 2-d order-statistic variant that
-BASELINE config #5 needs (AdaptiveDistance over a (B, n_obs) summary matrix)."""
+BASELINE config #5 needs (AdaptiveDistance over a (B, n_obs) summary matrix).
+
+ss_robust, ss_octile and euclidean_multiss take host arrays (the reference's NumPy code), device
+tensors (the kernels of gnkstats.cu) and the lazy output of the throughput-mode simulators (the
+summaries are computed in the simulator kernel); all three forms give the same bits."""
 from functools import partial
 
 import numpy as np
@@ -36,11 +40,68 @@ def ss_sorted(y):
 
 
 def euclidean_multiss(*simulated, observed):
-    """gnk.py:115-142 (host callable over 3-d summaries)."""
+    """gnk.py:115-142 over 3-d summaries (B, K, 1); device summaries give a device (B,) result."""
+    if dev.is_device_array(simulated[0]):
+        return ops.euclidean_multiss(simulated[0], observed[0])
     pts_sim = dev.to_host(simulated[0])
     pts_obs = dev.to_host(observed[0])
     d_ss_merged = np.sum((pts_sim - pts_obs)**2., axis=1)
     return np.sqrt(np.sum(d_ss_merged, axis=1))
+
+
+def _lazy_summaries(y, kind):
+    """(B, width * d, 1) summaries of lazy simulator output or device data; None for host data."""
+    if isinstance(y, LazyGNKData):
+        return y.summaries(kind)[:, :, None]
+    if dev.is_device_array(y):
+        return ops.gnk_summaries(y, kind)[:, :, None]
+    return None
+
+
+def ss_robust(y):
+    """Robust summary of Drovandi & Pettitt (2011), gnk.py:164-188: (B, 4 d, 1) for y (B, n_obs, d),
+    [A_1..A_d, B_1..B_d, g_1..g_d, k_1..k_d]."""
+    s = _lazy_summaries(y, 'ss_robust')
+    if s is not None:
+        return s
+    ss = np.hstack((_get_ss_A(y), _get_ss_B(y), _get_ss_g(y), _get_ss_k(y)))
+    return ss[:, :, np.newaxis]
+
+
+def ss_octile(y):
+    """Octile summary, gnk.py:191-213: (B, 7 d, 1) for y (B, n_obs, d), [E1_1..E1_d, .., E7_d]."""
+    s = _lazy_summaries(y, 'ss_octile')
+    if s is not None:
+        return s
+    octiles = np.linspace(12.5, 87.5, 7)
+    E1, E2, E3, E4, E5, E6, E7 = np.percentile(y, octiles, axis=1)
+    return np.hstack((E1, E2, E3, E4, E5, E6, E7))[:, :, np.newaxis]
+
+
+def _get_ss_A(y):
+    """gnk.py:216-219: the median."""
+    return np.percentile(y, 50, axis=1)
+
+
+def _get_ss_B(y):
+    """gnk.py:222-234: the interquartile range, eps where it is 0 (it divides ss_g and ss_k)."""
+    L1, L3 = np.percentile(y, [25, 75], axis=1)
+    ss_B = (L3 - L1).ravel()
+    idxs_zero = np.where(ss_B == 0)[0]
+    ss_B[idxs_zero] += np.finfo(float).eps
+    return ss_B.reshape(y.shape[0], y.shape[-1])
+
+
+def _get_ss_g(y):
+    """gnk.py:237-241: skewness."""
+    L1, L2, L3 = np.percentile(y, [25, 50, 75], axis=1)
+    return np.divide(L3 + L1 - 2 * L2, _get_ss_B(y))
+
+
+def _get_ss_k(y):
+    """gnk.py:244-248: kurtosis."""
+    E1, E3, E5, E7 = np.percentile(y, [12.5, 37.5, 62.5, 87.5], axis=1)
+    return np.divide(E7 - E5 + E3 - E1, _get_ss_B(y))
 
 
 def _base(n_obs, true_params, seed):
@@ -103,16 +164,76 @@ class DeviceProposal:
         return ops.logprior_box(params, self.lo, self.width)
 
 
-def get_device_model(n_obs=256, true_params=None, seed=None):
-    """Config #5 in throughput mode: uniform(0, 10) priors drawn on the device, `gnk_device`,
-    row-sorted order statistics and AdaptiveDistance.  Returns (model, DeviceProposal)."""
+class LazyGNKData:
+    """Output of :func:`gnk_device_lazy`: the robust / octile summaries are computed in the
+    simulator kernel (n_obs <= 512), so the (B, n_obs) data is only written when asked for
+    (for n_obs > 512 the summaries are taken from the written data).  Subclasses replace
+    _fused and materialize."""
+
+    def __init__(self, A, B, g, k, c, n_obs, key):
+        self.params, self.c, self.n_obs, self.key = (A, B, g, k), c, n_obs, key
+        self.shape = (int(A.numel()), n_obs, 1)
+        self.ndim = 3
+        self._S = {}
+
+    def __len__(self):
+        return self.shape[0]
+
+    def summaries(self, kind):
+        """(B, width) summaries of kind 'ss_robust' or 'ss_octile'."""
+        if kind not in self._S:
+            self._S[kind] = self._fused(kind) if self.n_obs <= ops.GNK_FUSED_MAX else \
+                ops.gnk_summaries(self.materialize(), kind)
+        return self._S[kind]
+
+    def _fused(self, kind):
+        return ops.sim_gnk_summaries(*self.params, n_obs=self.n_obs, seed=self.key, c=self.c,
+                                     kind=kind)
+
+    def materialize(self):
+        """The simulated data, (B, n_obs, 1) on the device."""
+        return ops.sim_gnk(*self.params, n_obs=self.n_obs, seed=self.key, c=self.c)[:, :, None]
+
+
+def gnk_device_lazy(A, B, g, k, c=0.8, n_obs=50, batch_size=1, random_state=None):
+    """Device twin of GNK whose robust / octile summaries are fused into the simulator."""
+    from .gauss import _key
+
+    def as_dev(v):
+        if dev.is_device_array(v):
+            return v.reshape(-1)
+        return dev.to_device(np.broadcast_to(np.asarray(v, dtype=np.float64).reshape(-1),
+                                             (batch_size,)).copy())
+    return LazyGNKData(as_dev(A), as_dev(B), as_dev(g), as_dev(k), c, n_obs, _key(random_state))
+
+
+def get_device_model(n_obs=256, true_params=None, seed=None, summary='ss_sorted'):
+    """The g-and-k task in throughput mode: uniform(0, 10) priors drawn on the device and the
+    simulator on the device.  Returns (model, DeviceProposal).
+
+    summary='ss_sorted': config #5, row-sorted order statistics and AdaptiveDistance.
+    summary='ss_robust' or 'ss_octile': the reference's get_model graph with that summary and
+    euclidean_multiss; the summaries are fused into the simulator (n_obs <= 2048; the data is
+    only written for n_obs > 512).  The observed summaries are computed on the host."""
     from .gauss import _DeviceUniform
+    if summary not in ('ss_sorted', 'ss_robust', 'ss_octile'):
+        raise ValueError("summary must be 'ss_sorted', 'ss_robust' or 'ss_octile', got {!r}".format(
+            summary))
+    if summary != 'ss_sorted' and not 1 <= n_obs <= ops.GNK_SERIES_MAX:
+        raise ValueError('device g-and-k summaries take 1 <= n_obs <= {}, got {}'.format(
+            ops.GNK_SERIES_MAX, n_obs))
     if true_params is None:
         true_params = [3, 1, 2, .5]
     m = em.new_model()
     priors = [em.Prior(_DeviceUniform, 0, 10, model=m, name=n) for n in ('A', 'B', 'g', 'k')]
     y_obs = GNK(*true_params, n_obs=n_obs, random_state=np.random.RandomState(seed))
-    em.Simulator(partial(gnk_device, n_obs=n_obs), *priors, observed=y_obs, name='GNK')
-    s = em.Summary(ss_sorted, m['GNK'], name='ss_sorted')
-    em.AdaptiveDistance(s, name='d')
+    if summary == 'ss_sorted':
+        em.Simulator(partial(gnk_device, n_obs=n_obs), *priors, observed=y_obs, name='GNK')
+        s = em.Summary(ss_sorted, m['GNK'], name='ss_sorted')
+        em.AdaptiveDistance(s, name='d')
+    else:
+        em.Simulator(partial(gnk_device_lazy, n_obs=n_obs), *priors, observed=y_obs, name='GNK')
+        s = em.Summary(ss_robust if summary == 'ss_robust' else ss_octile, m['GNK'], name=summary)
+        em.Discrepancy(euclidean_multiss, s, name='d')
     return m, DeviceProposal()
+

@@ -776,3 +776,131 @@ def rowsort(x):
     _lib.call('elfi_b200_rowsort_f64', dev.context(), dev.ptr(x), _ld(x), B, n, dev.ptr(out), n,
               dev.stream_ptr())
     return out
+
+
+# ---- robust / octile g-and-k summaries (elfi/examples/gnk.py:164-248, bignk.py) ------------------
+GNK_KINDS = {'ss_robust': 0, 'ss_octile': 1}
+GNK_WIDTH = {'ss_robust': 4, 'ss_octile': 7}
+GNK_SERIES_MAX = 2048     # series length of gnk_summaries (the shared-memory sort)
+GNK_FUSED_MAX = 512       # n_obs of the fused simulators (the register sort)
+_GNK_OCTILES = np.linspace(12.5, 87.5, 7)
+
+
+def gnk_picks(n):
+    """Sorted positions and weights of np.percentile(y, [12.5, 25, .., 87.5], method='linear') for
+    a series of length n, computed as numpy/lib/_function_base_impl.py does (_quantile,
+    _get_indexes, _get_gamma): [lo (7), hi (7), t (7)] as a float64 array."""
+    q = np.true_divide(_GNK_OCTILES, 100)
+    vi = (n - 1) * q
+    lo = np.floor(vi)
+    hi = lo + 1
+    above = vi >= n - 1
+    lo[above] = -1
+    hi[above] = -1
+    t = vi - lo
+    lo[lo < 0] = n - 1
+    hi[hi < 0] = n - 1
+    return np.ascontiguousarray(np.concatenate([lo, hi, t]), dtype=np.float64)
+
+
+def _gnk_kind(kind):
+    if kind not in GNK_KINDS:
+        raise ValueError('unknown g-and-k summary {!r} (supported: {})'.format(
+            kind, ', '.join(GNK_KINDS)))
+    return GNK_KINDS[kind]
+
+
+def gnk_summaries(y, kind='ss_robust'):
+    """ss_robust / ss_octile of gnk.py on the device for y (B, n, d) (or (B, n) for d = 1),
+    1 <= n <= 2048, d in {1, 2}: a (B, width * d) tensor laid out as the reference's np.hstack
+    (reshape to (B, width * d, 1) for its shape), bit for bit."""
+    k = _gnk_kind(kind)
+    if not (dev.is_device_array(y) and y.dtype == torch.float64):
+        y = dev.to_device(y)    # device views are read in place (row and observation strides)
+    if y.dim() == 2:
+        y = y[:, :, None]
+    if y.dim() != 3:
+        raise ValueError('expected (batch, n_obs, dim) data, got shape {}'.format(tuple(y.shape)))
+    B, n, d = y.shape
+    if d not in (1, 2):
+        raise ValueError('g-and-k summaries take 1 or 2 dimensions, got {}'.format(d))
+    if not 1 <= n <= GNK_SERIES_MAX:
+        raise ValueError('g-and-k summaries on the device take 1 <= n_obs <= {}, got {}'.format(
+            GNK_SERIES_MAX, n))
+    if y.stride(2) != 1 or y.stride(1) < d:
+        y = y.contiguous()
+    out = dev.empty((B, GNK_WIDTH[kind] * d))
+    _lib.call('elfi_b200_gnk_summaries_f64', dev.context(), dev.ptr(y),
+              y.stride(0) if B > 1 else (n - 1) * y.stride(1) + d, y.stride(1), B, n, d, k,
+              dev.ptr(gnk_picks(n)), dev.ptr(out), out.shape[1], dev.stream_ptr())
+    return out
+
+
+def sim_gnk_summaries(A, B, g, k, n_obs=50, seed=0, offset=0, c=0.8, kind='ss_robust'):
+    """The ss_robust / ss_octile summaries of the rows :func:`sim_gnk` simulates for the same
+    arguments, computed without writing the data: (batch, width), bit for bit equal to
+    gnk_summaries(sim_gnk(...)).  n_obs <= 512."""
+    kd = _gnk_kind(kind)
+    if not 1 <= n_obs <= GNK_FUSED_MAX:
+        raise ValueError('the fused g-and-k summaries take 1 <= n_obs <= {}, got {}'.format(
+            GNK_FUSED_MAX, n_obs))
+    cols = [dev.to_device(v).reshape(-1).contiguous() for v in (A, B, g, k)]
+    n = cols[0].numel()
+    if any(col.numel() != n for col in cols):
+        raise ValueError('A, B, g and k must have the same number of elements')
+    out = dev.empty((n, GNK_WIDTH[kind]))
+    _lib.call('elfi_b200_sim_gnk_summaries_f64', dev.context(), dev.ptr(cols[0]), dev.ptr(cols[1]),
+              dev.ptr(cols[2]), dev.ptr(cols[3]), float(c), n, int(n_obs), int(seed), int(offset), kd,
+              dev.ptr(gnk_picks(n_obs)), dev.ptr(out), out.shape[1], dev.stream_ptr())
+    return out
+
+
+def sim_bignk(params, n_obs=150, seed=0, offset=0, c=0.8, want_data=True, kind=None):
+    """Bivariate g-and-k simulator on the device (elfi/examples/bignk.py:12-108).  params: (batch, 9)
+    columns A1, A2, B1, B2, g1, g2, k1, k2, rho.  Returns (Y (batch, n_obs, 2) or None,
+    S (batch, 2 * width) or None): S = the fused ss_robust / ss_octile summaries when ``kind`` is
+    given (n_obs <= 512), equal to gnk_summaries(Y, kind) bit for bit."""
+    P = _matrix(params)
+    if P.shape[1] != 9:
+        raise ValueError('the bivariate g-and-k model has 9 parameters, got {}'.format(P.shape[1]))
+    if n_obs < 1:
+        raise ValueError('n_obs must be >= 1')
+    kd, S = -1, None
+    if kind is not None:
+        kd = _gnk_kind(kind)
+        if n_obs > GNK_FUSED_MAX:
+            raise ValueError('the fused g-and-k summaries take n_obs <= {}, got {}'.format(
+                GNK_FUSED_MAX, n_obs))
+    B = P.shape[0]
+    Y = dev.empty((B, n_obs, 2)) if want_data else None
+    if kind is not None:
+        S = dev.empty((B, 2 * GNK_WIDTH[kind]))
+    _lib.call('elfi_b200_sim_bignk_f64', dev.context(), dev.ptr(P), _ld(P), float(c), B,
+              int(n_obs), int(seed), int(offset), dev.ptr(Y), 2 * n_obs, kd,
+              dev.ptr(gnk_picks(n_obs)) if kind is not None else None, dev.ptr(S),
+              S.shape[1] if S is not None else 0, dev.stream_ptr())
+    return Y, S
+
+
+def euclidean_multiss(S, obs):
+    """euclidean_multiss of gnk.py:115-142 for device summaries S (B, K) or (B, K, 1) and observed
+    summaries obs (K,) / (1, K, 1), K <= 128: sqrt(sum_j (S[:, j] - obs[j])^2) in NumPy's order,
+    bit for bit.  Returns a device tensor (B,)."""
+    if dev.is_device_array(S) and S.dim() == 3:
+        if S.shape[2] != 1:
+            raise ValueError('euclidean_multiss on the device takes (B, K, 1) summaries')
+        S = S[:, :, 0]
+    S = _matrix(S)
+    B, K = S.shape
+    o = np.ascontiguousarray(np.asarray(dev.to_host(obs) if dev.is_device_array(obs) else obs,
+                                        dtype=np.float64).reshape(-1))
+    if o.size != K:
+        raise ValueError('observed summaries have {} values, simulated {}'.format(o.size, K))
+    if not 1 <= K <= 128:
+        raise ValueError('euclidean_multiss on the device takes 1 <= K <= 128 summaries, got {}'
+                         .format(K))
+    o = dev.to_device(o)
+    out = dev.empty((B,))
+    _lib.call('elfi_b200_euclidean_multiss_f64', dev.context(), dev.ptr(S), _ld(S), B, K,
+              dev.ptr(o), dev.ptr(out), dev.stream_ptr())
+    return out

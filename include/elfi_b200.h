@@ -447,6 +447,41 @@ int elfi_b200_sim_gnk_f64(elfi_b200_ctx* ctx, const double* A, const double* Bs,
 int elfi_b200_logprior_box_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int64_t B, int64_t p,
                                const double* box_host, double* out, void* stream);
 
+/* Robust and octile g-and-k summaries (elfi/examples/gnk.py:164-248), bit for bit.
+ * kind 0 = ss_robust: [L2, ss_B, ss_g, ss_k] per dimension; kind 1 = ss_octile: [E1 .. E7].
+ * The output row is laid out as the reference's np.hstack: value j of dimension a at
+ * out[i * ld_out + j * d + a].  picks_host = lo[7], hi[7], t[7] (doubles) of
+ * np.percentile(.., [12.5, 25, .., 87.5], method='linear') for the series length (ops.gnk_picks):
+ * value = t >= 0.5 ? b - (b - a)(1 - t) : a + (b - a) t with a, b the sorted elements lo, hi.
+ * NaN rules as NumPy's: a NaN in a series makes all its octiles NaN; an infinity at a picked
+ * position with t = 0 gives NaN through (inf - a) * 0; ss_B = 0 becomes eps.
+ * gnk_summaries: series (i, a) of a data matrix is X[i * ld_row + j * ld_obs + a], j < n,
+ *   1 <= n <= 2048, d in {1, 2}.
+ * sim_gnk_summaries: the summaries of the rows elfi_b200_sim_gnk_f64 would simulate, without
+ *   writing them (1 <= n_obs <= 512); equal to sim_gnk followed by gnk_summaries.
+ * sim_bignk: bivariate g-and-k (elfi/examples/bignk.py:12-108).  P[i * ldP + 0..8] = A1, A2, B1, B2,
+ *   g1, g2, k1, k2, rho.  Observation j of row i: Philox block (seed, offset + i, j) gives n0, n1;
+ *   z1 = n0, z2 = rho n0 + sqrt(1 - rho^2) n1, y_a = the g-and-k quantile of (A_a, B_a, g_a, k_a, c)
+ *   at z_a.  |rho| > 1 or NaN gives NaN rows.  Y (B, n_obs, 2) with leading dimension ldY (may be
+ *   NULL); S (B, 2 * width) fused summaries of kind `kind` (may be NULL, needs n_obs <= 512).
+ * euclidean_multiss (gnk.py:115-142) on (B, K, 1) summaries stored as (B, K) with leading dimension
+ *   ldS, K <= 128, obs (K) on the device: out[i] = sqrt(sum_j (S[i, j] - obs[j])^2), summed in
+ *   NumPy's pairwise order. */
+int elfi_b200_gnk_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_row, int64_t ld_obs,
+                                int64_t B, int64_t n, int64_t d, int32_t kind,
+                                const double* picks_host, double* out, int64_t ld_out, void* stream);
+int elfi_b200_sim_gnk_summaries_f64(elfi_b200_ctx* ctx, const double* A, const double* Bs,
+                                    const double* g, const double* k, double c, int64_t B,
+                                    int64_t n_obs, uint64_t seed, uint64_t offset, int32_t kind,
+                                    const double* picks_host, double* out, int64_t ld_out,
+                                    void* stream);
+int elfi_b200_sim_bignk_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, double c, int64_t B,
+                            int64_t n_obs, uint64_t seed, uint64_t offset, double* Y, int64_t ldY,
+                            int32_t kind, const double* picks_host, double* S, int64_t ldS,
+                            void* stream);
+int elfi_b200_euclidean_multiss_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
+                                    int64_t K, const double* obs, double* out, void* stream);
+
 /* ---- KLIEP density-ratio estimation (AdaptiveThresholdSMC) -------------------------------------
  * DensityRatioEstimation.fit + max_ratio (elfi/methods/density_ratio_estimation.py:71-207):
  * basis centres = first n_basis rows of x, A = RBF(x, centres), b = weighted RBF mean over y,
