@@ -86,6 +86,11 @@ SIGNATURES = {
     'elfi_b200_sim_bignk_f64': [c_ptr, c_ptr, c_i64, c_dbl, c_i64, c_i64, c_u64, c_u64, c_ptr, c_i64,
                                 ctypes.c_int32, c_ptr, c_ptr, c_i64, c_ptr],
     'elfi_b200_euclidean_multiss_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
+    'elfi_b200_poisson_f64': [c_ptr, c_ptr, c_i64, c_u64, c_u64, c_ptr, c_ptr],
+    'elfi_b200_sim_ricker_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_dbl, c_u64, c_u64, c_ptr,
+                                 c_i64, c_ptr, c_i64, c_ptr, c_i64, c_ptr],
+    'elfi_b200_count_zeros_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr],
+    'elfi_b200_chi_squared_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     'elfi_b200_prior_rvs_f64': [c_ptr, c_ptr, c_i64, c_u64, c_u64, c_ptr, c_ptr],
     'elfi_b200_prior_logpdf_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     'elfi_b200_gp_padded_size': [c_i64],

@@ -1,2 +1,2 @@
-"""Benchmark models of the hot path (MA2, Gaussian noise, univariate and bivariate g-and-k) on the
-elfi_b200 node API."""
+"""Benchmark models of the hot path (MA2, Gaussian noise, univariate and bivariate g-and-k, Ricker)
+on the elfi_b200 node API."""

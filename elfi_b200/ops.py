@@ -904,3 +904,103 @@ def euclidean_multiss(S, obs):
     _lib.call('elfi_b200_euclidean_multiss_f64', dev.context(), dev.ptr(S), _ld(S), B, K,
               dev.ptr(o), dev.ptr(out), dev.stream_ptr())
     return out
+
+
+# ---- Ricker model (elfi/examples/ricker.py) -------------------------------------------------------
+POISSON_LAM_MAX = 9.223372006484771e18   # NumPy's limit; larger rates give NaN
+RICKER_FUSED_MAX = 128    # n_obs of the fused summaries (one leaf of NumPy's pairwise sum)
+RICKER_NOBS_MAX = 1 << 24
+
+
+def poisson(lam, seed, offset=0):
+    """Poisson(lam) draws on the device, one per element of lam (any shape): element i (in C order)
+    is a pure function of (seed, offset + i).  lam == 0 gives 0; lam < 0, NaN or lam >
+    POISSON_LAM_MAX give NaN (where NumPy raises).  Returns float64 counts shaped like lam."""
+    lam = dev.to_device(lam)
+    flat = lam.reshape(-1).contiguous()
+    out = dev.empty((flat.numel(),))
+    _lib.call('elfi_b200_poisson_f64', dev.context(), dev.ptr(flat), flat.numel(), int(seed),
+              int(offset), dev.ptr(out), dev.stream_ptr())
+    return out.reshape(lam.shape)
+
+
+def _ricker_params(params, stochastic):
+    P = _matrix(params)
+    p = 3 if stochastic else 1
+    if P.shape[1] != p:
+        raise ValueError('the {} Ricker model has {} parameter{}, got {}'.format(
+            'stochastic' if stochastic else 'deterministic', p, 's' if p > 1 else '', P.shape[1]))
+    return P
+
+
+def sim_ricker(params, n_obs=50, seed=0, offset=0, stochastic=True, stock_init=1.0, want_data=False,
+               want_latent=False, want_summaries=True):
+    """Ricker simulator on the device (elfi/examples/ricker.py:11-85).  params: (batch, 3) columns
+    log_rate, std, scale for the stochastic model, (batch, 1) or (batch,) log_rate for the
+    deterministic one.  Row i is a pure function of (seed, offset + i).
+
+    Returns (Y, N, S), each None unless asked for: Y (batch, n_obs) the observed counts (the stock
+    for the deterministic model), N (batch, n_obs) the latent stock, S (batch, 3) =
+    [np.mean(Y), np.var(Y), number of zeros of Y] per row.  For n_obs <= RICKER_FUSED_MAX S is
+    computed in the simulator without writing Y; above, Y is written and summarised
+    (:func:`ricker_summaries`).  Both give the same bits."""
+    if np.ndim(stock_init) != 0:
+        raise ValueError('stock_init must be a scalar on the device, got shape {}'.format(
+            np.shape(stock_init)))
+    if not 1 <= int(n_obs) <= RICKER_NOBS_MAX:
+        raise ValueError('the device Ricker simulator takes 1 <= n_obs <= {}, got {}'.format(
+            RICKER_NOBS_MAX, n_obs))
+    n_obs = int(n_obs)
+    P = _ricker_params(params, stochastic)
+    B = P.shape[0]
+    fused = want_summaries and n_obs <= RICKER_FUSED_MAX
+    Y = dev.empty((B, n_obs)) if want_data or (want_summaries and not fused) else None
+    N = dev.empty((B, n_obs)) if want_latent else None
+    S = dev.empty((B, 3)) if fused else None
+    _lib.call('elfi_b200_sim_ricker_f64', dev.context(), dev.ptr(P), _ld(P), P.shape[1], B, n_obs,
+              float(stock_init), int(seed), int(offset), dev.ptr(Y), n_obs, dev.ptr(N), n_obs,
+              dev.ptr(S), 3, dev.stream_ptr())
+    if want_summaries and not fused:
+        S = ricker_summaries(Y)
+    return (Y if want_data else None), N, S
+
+
+def count_zeros(y, out=None):
+    """num_zeros of elfi/examples/ricker.py:164-167 on the device: the number of zeros of each row
+    of y (B, n), as float64 (B,) (or into the column view ``out``)."""
+    y = _matrix(y)
+    B, n = y.shape
+    if out is None:
+        out = dev.empty((B,))
+    _lib.call('elfi_b200_count_zeros_f64', dev.context(), dev.ptr(y), _ld(y), B, n, dev.ptr(out),
+              out.stride(0), dev.stream_ptr())
+    return out
+
+
+def ricker_summaries(y):
+    """The Ricker summaries [np.mean, np.var, num_zeros] of each row of device data y (B, n): a
+    (B, 3) tensor, bit for bit NumPy's (mean and variance from :func:`meanvar`)."""
+    y = _matrix(y)
+    S = dev.empty((y.shape[0], 3))
+    meanvar(y, out=S[:, :2])
+    count_zeros(y, out=S[:, 2])
+    return S
+
+
+def chi_squared(S, obs):
+    """chi_squared of elfi/examples/ricker.py:147-161 for device summaries S (B, K) and observed
+    summaries obs (K,), K <= 128: sum_j (S[:, j] - obs[j])^2 / obs[j] in NumPy's order, bit for
+    bit (obs[j] = 0 gives NumPy's inf / NaN).  Returns a device tensor (B,)."""
+    S = _matrix(S)
+    B, K = S.shape
+    o = np.ascontiguousarray(np.asarray(dev.to_host(obs) if dev.is_device_array(obs) else obs,
+                                        dtype=np.float64).reshape(-1))
+    if o.size != K:
+        raise ValueError('observed summaries have {} values, simulated {}'.format(o.size, K))
+    if not 1 <= K <= 128:
+        raise ValueError('chi_squared on the device takes 1 <= K <= 128 summaries, got {}'.format(K))
+    o = dev.to_device(o)
+    out = dev.empty((B,))
+    _lib.call('elfi_b200_chi_squared_f64', dev.context(), dev.ptr(S), _ld(S), B, K, dev.ptr(o),
+              dev.ptr(out), dev.stream_ptr())
+    return out

@@ -482,6 +482,37 @@ int elfi_b200_sim_bignk_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, do
 int elfi_b200_euclidean_multiss_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
                                     int64_t K, const double* obs, double* out, void* stream);
 
+/* Ricker model of elfi/examples/ricker.py (throughput mode, statistical parity); stream layout,
+ * algorithms and limits in elfi_b200/csrc/ricker.cu and poisson.cuh.
+ * poisson: out[i] ~ Poisson(lam[i]) (device vectors of n doubles), a pure function of
+ *   (seed, offset + i).  Inversion for lam < 10, PTRS (Hoermann 1993) with a cancellation-free
+ *   log-pmf test above.  lam == 0 gives 0; lam < 0, NaN or lam > 9.223372006484771e18 (NumPy's
+ *   POISSON_LAM_MAX, where NumPy raises) give NaN.  PTRS takes at most 32 trials (each rejected
+ *   with probability below 0.12); if all 32 are rejected the draw is floor(lam).  The inversion
+ *   search stops at 64.  Counts are doubles.
+ * sim_ricker: one row per parameter row P[i * ldP + ..]: n_params 3 = (r, sigma, phi), the
+ *   stochastic model N_t = N_{t-1} exp((r - N_{t-1}) + sigma e_t) from N_{-1} = stock_init and
+ *   Y_t ~ Poisson(phi N_t), t < n_obs; n_params 1 = (r), the deterministic model Y_0 = stock_init,
+ *   Y_t = Y_{t-1} exp(r - Y_{t-1}) (N = Y).  1 <= n_obs <= 2^24.  Y (B, n_obs; ldY), N (B, n_obs;
+ *   ldN) and S (B, 3; ldS) may each be NULL.  S = [np.mean(Y), np.var(Y), number of zeros of Y]
+ *   per row, computed in the simulator without writing Y (needs n_obs <= 128); equal bit for bit
+ *   to summary_meanvar and count_zeros of Y.
+ * count_zeros: out[i * ld_out] = the number of entries of row i of X (B, n; ldX) equal to 0, as a
+ *   double (num_zeros of ricker.py).
+ * chi_squared (ricker.py:147-161) on summaries S (B, K; ldS), K <= 128, obs (K) on the device:
+ *   out[i] = sum_j (S[i, j] - obs[j])^2 / obs[j] summed in NumPy's pairwise order; obs[j] = 0
+ *   gives NumPy's inf / NaN terms. */
+int elfi_b200_poisson_f64(elfi_b200_ctx* ctx, const double* lam, int64_t n, uint64_t seed,
+                          uint64_t offset, double* out, void* stream);
+int elfi_b200_sim_ricker_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t n_params,
+                             int64_t B, int64_t n_obs, double stock_init, uint64_t seed,
+                             uint64_t offset, double* Y, int64_t ldY, double* N, int64_t ldN,
+                             double* S, int64_t ldS, void* stream);
+int elfi_b200_count_zeros_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, int64_t B, int64_t n,
+                              double* out, int64_t ld_out, void* stream);
+int elfi_b200_chi_squared_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B, int64_t K,
+                              const double* obs, double* out, void* stream);
+
 /* ---- KLIEP density-ratio estimation (AdaptiveThresholdSMC) -------------------------------------
  * DensityRatioEstimation.fit + max_ratio (elfi/methods/density_ratio_estimation.py:71-207):
  * basis centres = first n_basis rows of x, A = RBF(x, centres), b = weighted RBF mean over y,
