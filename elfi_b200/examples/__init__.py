@@ -1,2 +1,3 @@
-"""Benchmark models of the hot path (MA2, Gaussian noise, univariate and bivariate g-and-k, Ricker)
+"""Benchmark models of the hot path (MA2, Gaussian noise, univariate and bivariate g-and-k, Ricker,
+Lorenz)
 on the elfi_b200 node API."""

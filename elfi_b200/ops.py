@@ -1004,3 +1004,82 @@ def chi_squared(S, obs):
     _lib.call('elfi_b200_chi_squared_f64', dev.context(), dev.ptr(S), _ld(S), B, K, dev.ptr(o),
               dev.ptr(out), dev.stream_ptr())
     return out
+
+
+# ---- Lorenz forecast model (elfi/examples/lorenz.py) ----------------------------------------------
+LORENZ_NOBS_MIN, LORENZ_NOBS_MAX = 4, 128     # variables of the ring on the device
+LORENZ_SUMM_NOBS_MIN = 2     # one variable: NumPy sums over time pairwise, not row by row
+LORENZ_T_MAX = 1 << 26                        # n_timestep of the simulator (the stream's step word)
+LORENZ_SUMM_MAX_TERMS = 30728                 # n_timestep * n_obs of the summaries
+LORENZ_NSUMM = 6
+
+
+def _lorenz_params(params):
+    P = _matrix(params)
+    if P.shape[1] != 2:
+        raise ValueError('the Lorenz model has 2 parameters (theta1, theta2), got a parameter width '
+                         'of {}'.format(P.shape[1]))
+    return P
+
+
+def sim_lorenz(params, n_timestep=160, initial_state=None, f=10., phi=0.984, total_duration=4.,
+               seed=0, offset=0, want_data=False, want_summaries=True):
+    """Stochastic Lorenz 96 forecast model on the device (elfi/examples/lorenz.py:94-163).
+    params: (batch, 2) columns theta1, theta2.  initial_state: the n_obs values of time 0 (default:
+    the reference's 40-value state, examples.lorenz.INITIAL_STATE); 4 <= n_obs <= 128.  Row i is a
+    pure function of (seed, offset + i).  dt = total_duration / n_timestep and
+    sqrt(1 - phi ** 2) are computed as the reference computes them (phi > 1 gives NaN rows).
+
+    Returns (X, S), each None unless asked for: X (batch, n_timestep, n_obs) the trajectories, S
+    (batch, 6) = [Mean, Var, Autocov, Cov, CrosscovPrev, CrosscovNext] per row.  Without want_data
+    the summaries are computed in the simulator and no (batch, n_timestep, n_obs) tensor is
+    allocated; either way S equals :func:`lorenz_summaries` of X bit for bit."""
+    if initial_state is None:
+        from .examples.lorenz import INITIAL_STATE
+        initial_state = INITIAL_STATE
+    init = np.array(initial_state, dtype=np.float64)      # a writable copy for torch
+    if init.ndim != 1:
+        raise ValueError('initial_state must be one vector of n_obs values, got shape {}'.format(
+            init.shape))
+    m = init.size
+    if not LORENZ_NOBS_MIN <= m <= LORENZ_NOBS_MAX:
+        raise ValueError('the device Lorenz simulator takes an initial state of {} <= n_obs <= {} '
+                         'values, got {}'.format(LORENZ_NOBS_MIN, LORENZ_NOBS_MAX, m))
+    n_timestep = int(n_timestep)
+    if not 2 <= n_timestep <= LORENZ_T_MAX:
+        raise ValueError('the device Lorenz simulator takes 2 <= n_timestep <= {}, got {}'.format(
+            LORENZ_T_MAX, n_timestep))
+    if want_summaries and n_timestep * m > LORENZ_SUMM_MAX_TERMS:
+        raise ValueError('the device Lorenz summaries take n_timestep * n_obs <= {}, got {} * {}'
+                         .format(LORENZ_SUMM_MAX_TERMS, n_timestep, m))
+    P = _lorenz_params(params)
+    B = P.shape[0]
+    dt = total_duration / n_timestep
+    with np.errstate(invalid='ignore'):
+        s_phi = float(np.sqrt(1 - pow(phi, 2)))
+    X = dev.empty((B, n_timestep, m)) if want_data else None
+    S = dev.empty((B, LORENZ_NSUMM)) if want_summaries else None
+    _lib.call('elfi_b200_sim_lorenz_f64', dev.context(), dev.ptr(P), _ld(P), B, m, n_timestep,
+              dev.ptr(dev.to_device(init)), float(f), float(phi), s_phi, float(dt), int(seed),
+              int(offset), dev.ptr(X), dev.ptr(S), LORENZ_NSUMM, dev.stream_ptr())
+    return X, S
+
+
+def lorenz_summaries(x):
+    """The six Lorenz summaries [Mean, Var, Autocov, Cov, CrosscovPrev, CrosscovNext]
+    (elfi/examples/lorenz.py:231-320) of device data x (B, n_timestep, n_obs), any strides: a
+    (B, 6) tensor, bit for bit NumPy's on the C-contiguous array.  2 <= n_timestep,
+    2 <= n_obs <= 128, n_timestep * n_obs <= LORENZ_SUMM_MAX_TERMS."""
+    x = dev.to_device(x) if not (dev.is_device_array(x) and x.dtype == torch.float64) else x
+    if x.dim() != 3:
+        raise ValueError('lorenz_summaries takes (batch, n_timestep, n_obs) data, got shape {}'
+                         .format(tuple(x.shape)))
+    B, T, m = x.shape
+    if not LORENZ_SUMM_NOBS_MIN <= m <= LORENZ_NOBS_MAX or T < 2 or T * m > LORENZ_SUMM_MAX_TERMS:
+        raise ValueError('lorenz_summaries takes {} <= n_obs <= {}, 2 <= n_timestep and n_timestep * '
+                         'n_obs <= {}, got n_timestep {}, n_obs {}'.format(
+                             LORENZ_SUMM_NOBS_MIN, LORENZ_NOBS_MAX, LORENZ_SUMM_MAX_TERMS, T, m))
+    S = dev.empty((B, LORENZ_NSUMM))
+    _lib.call('elfi_b200_lorenz_summaries_f64', dev.context(), dev.ptr(x), x.stride(0), x.stride(1),
+              x.stride(2), B, T, m, dev.ptr(S), LORENZ_NSUMM, dev.stream_ptr())
+    return S

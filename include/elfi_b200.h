@@ -513,6 +513,31 @@ int elfi_b200_count_zeros_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, 
 int elfi_b200_chi_squared_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B, int64_t K,
                               const double* obs, double* out, void* stream);
 
+/* Lorenz forecast model of elfi/examples/lorenz.py (throughput mode, statistical parity); stream
+ * layout, lane layout and arithmetic in elfi_b200/csrc/lorenz.cu and lorenz.cuh.
+ * sim_lorenz: row i has parameters (theta1, theta2) = P[i * ldP], P[i * ldP + 1] (ldP >= 2) and
+ *   starts from init (n_obs doubles on the device); for s = 1 .. n_timestep - 1 it draws e (n_obs
+ *   normals, a pure function of (seed, offset + i, s, k): Box-Muller normal (k & 1) of Philox block
+ *   (s << 6) | (k >> 1)), sets eta = phi * eta + e * s_phi and takes one RK4 step of length dt.
+ *   s_phi = sqrt(1 - phi^2) and dt = total_duration / n_timestep are computed by the caller
+ *   (phi > 1 gives NaN rows, as in the reference).  4 <= n_obs <= 128, 2 <= n_timestep <= 2^26.
+ *   X (B, n_timestep, n_obs), C-contiguous, may be NULL; S (B, 6; ldS >= 6) may be NULL and needs
+ *   n_timestep * n_obs <= 30728.  With S and without X the summaries are computed in the simulator
+ *   from a per-warp scratch slab (up to 512 MiB of the context's scratch, independent of B); with
+ *   both, X is written and summarised.  Either way S equals lorenz_summaries of X bit for bit.
+ * lorenz_summaries: S[i * ldS + 0..5] = [Mean, Var, Autocov, Cov, CrosscovPrev, CrosscovNext]
+ *   (lorenz.py:231-320) of the row X[i * ld_row + t * ld_t + k * ld_k] (n_timestep, n_obs), bit for
+ *   bit NumPy's on a C-contiguous array; 2 <= n_obs <= 128 (with one variable NumPy sums over time
+ *   pairwise), n_timestep >= 2,
+ *   n_timestep * n_obs <= 30728.  NaN and inf propagate as in NumPy. */
+int elfi_b200_sim_lorenz_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
+                             int64_t n_obs, int64_t n_timestep, const double* init, double f,
+                             double phi, double s_phi, double dt, uint64_t seed, uint64_t offset,
+                             double* X, double* S, int64_t ldS, void* stream);
+int elfi_b200_lorenz_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_row,
+                                   int64_t ld_t, int64_t ld_k, int64_t B, int64_t n_timestep,
+                                   int64_t n_obs, double* S, int64_t ldS, void* stream);
+
 /* ---- KLIEP density-ratio estimation (AdaptiveThresholdSMC) -------------------------------------
  * DensityRatioEstimation.fit + max_ratio (elfi/methods/density_ratio_estimation.py:71-207):
  * basis centres = first n_basis rows of x, A = RBF(x, centres), b = weighted RBF mean over y,
