@@ -318,6 +318,9 @@ gp_cov_kernel(const double* __restrict__ Aq, int64_t lda, int64_t na, const doub
 
 // ---- K11: blocked Cholesky (right-looking, panel width 64) ------------------------------------
 // Factor the diagonal block A[k:k+64, k:k+64] in place (lower); info != 0 on a bad pivot.
+// A bad pivot turns every later pivot into NaN (the padding's too, through 0 * NaN in the panel
+// solves), so both pivot kernels record info only while it is still 0: columns are visited in
+// order and panels are serialised on the caller's stream, so the FIRST bad pivot is reported.
 __global__ void __launch_bounds__(256)
 potrf_diag_kernel(double* __restrict__ A, int64_t lda, int64_t k, int* __restrict__ info) {
     __shared__ double s[GP_NB][GP_NB + 1];
@@ -331,7 +334,7 @@ potrf_diag_kernel(double* __restrict__ A, int64_t lda, int64_t k, int* __restric
     for (int j = 0; j < GP_NB; ++j) {
         if (tid == 0) {
             const double d = s[j][j];
-            if (!(d > 0.0)) atomicExch(info, int(k + j + 1));
+            if (!(d > 0.0)) atomicCAS(info, 0, int(k + j + 1));
             s[j][j] = sqrt(d);
         }
         __syncthreads();
@@ -387,7 +390,7 @@ potrf_diag_panel_kernel(double* __restrict__ A, int64_t lda, int64_t k, int64_t 
             // on the critical path of all 64 steps (and of the 64 steps of the panel solve below)
             if (r == j && q == (j & 1)) {
                 const double d = a[j >> 1];
-                if (!(d > 0.0) && blockIdx.x == 0) atomicExch(info, int(k + j + 1));
+                if (!(d > 0.0) && blockIdx.x == 0) atomicCAS(info, 0, int(k + j + 1));
                 const double inv = rsqrt(d);
                 a[j >> 1] = d * inv;
                 piv_inv = inv;
@@ -928,6 +931,7 @@ int elfi_b200_gp_predict_grad_f64(elfi_b200_ctx* ctx, const double* Xq, int64_t 
     using namespace elfi;
     ELFI_REQUIRE(ctx && Xq && X && W && U && alpha, "gp_predict_grad: NULL argument");
     ELFI_REQUIRE(m >= 0 && n >= 1 && p >= 1 && ldq >= p && ldX >= p, "gp_predict_grad: bad shape");
+    ELFI_REQUIRE(n_pad == elfi_b200_gp_padded_size(n), "gp_predict_grad: bad n_pad");
     if (m == 0) return ELFI_B200_OK;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     ELFI_CUDA_OK(cudaSetDevice(ctx->device));

@@ -301,8 +301,12 @@ int elfi_b200_smc_weights_f64(elfi_b200_ctx* ctx, const double* logprior, const 
  *
  * Factor storage (caller-allocated, n_pad x n_pad row-major, n_pad = elfi_b200_gp_padded_size(n)):
  *   L lower Cholesky factor (padded with the identity), W = L^-1, U = W^T;  alpha = Ky^-1 y (n).
- * noise_var must already include any jitter (GPy adds 1e-8).  info (device int32) is 0 on
- * success or 1 + the index of the first non-positive pivot.
+ * As in LAPACK's potrf, only the lower triangle of L[0:n, 0:n] is the factor: its strict upper
+ * triangle is workspace and holds unspecified values.  The padding rows and columns of L, W and U
+ * hold the identity (exact zeros off the diagonal), and W (U) has exact zeros above (below) the
+ * diagonal.  noise_var must already include any jitter (GPy adds 1e-8).  info (device int32) is
+ * 0 on success or 1 + the index of the first non-positive (or NaN) pivot; L, W, U and alpha are
+ * then unspecified.
  * gp_predict: mean/var/acq may each be NULL; var = k** - |W k|^2 + noise_add; acq = mean -
  * sqrt(beta * (noiseless var)).  Queries are processed in chunks through context scratch.
  */

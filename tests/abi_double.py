@@ -324,89 +324,127 @@ def kliep_fit_f64(ctx, x, ldx, Nx, y, ldy, Ny, p, wx, wy, sigma, n_basis, epsilo
     out[1] = -1.0   # the oracle does not count steps
 
 
-# ---- BOLFI surrogate: SciPy restatement of the factor layout the header documents ----------
-def _gp_factors(L, n, n_pad):
-    import scipy.linalg as sl
-    Lp = np.eye(n_pad)
-    Lp[:n, :n] = L
-    Wp = sl.solve_triangular(Lp, np.eye(n_pad), lower=True)
-    return Lp, Wp
+# ---- BOLFI surrogate: SciPy restatement of the factor layout and the W-based arithmetic the
+# header documents (var = k** - |W k|^2, T = W k, out = W^T T) ---------------------------------
+def _gp_padded(n):
+    return ((int(n) + 127) // 128) * 128
+
+
+def _gp_kernel(A, B, kernel_var, lengthscale, bias_var):
+    """k(A[i], B[j]) with r2 summed over coordinate differences, as gp.cu evaluates it (the
+    expanded |a|^2 + |b|^2 - 2 a.b loses short distances to cancellation)."""
+    r2 = np.zeros((len(A), len(B)))
+    for d in range(A.shape[1]):
+        diff = A[:, d, None] - B[None, :, d]
+        r2 += diff * diff
+    return kernel_var * np.exp(r2 * (-0.5 / lengthscale ** 2)) + bias_var
 
 
 def gp_fit_f64(ctx, X, ldX, y, n, p, kernel_var, lengthscale, bias_var, noise_var, L, W, U, n_pad,
                alpha, info, stream):
+    import scipy.linalg as sl
+    _require(n >= 1 and p >= 1 and ldX >= p, 'gp_fit: bad shape')
+    _require(n_pad == _gp_padded(n), 'gp_fit: n_pad must be {}'.format(_gp_padded(n)))
     Xm = np.ascontiguousarray(_mat(X, n, p, ldX))
     yv = _vec(y, n).copy()
     info_v = _vec(info, 1, np.int32)
-    K = o.gp_gram(Xm, kernel_var, lengthscale, bias_var) + noise_var * np.eye(n)
-    try:
-        Lc = np.linalg.cholesky(K)
-    except np.linalg.LinAlgError:
-        info_v[0] = 1            # "1 + index of the first bad pivot": any non-zero value raises
+    K = _gp_kernel(Xm, Xm, kernel_var, lengthscale, bias_var) + noise_var * np.eye(n)
+    Lc, bad = sl.lapack.dpotrf(K, lower=1, clean=1)
+    _require(bad >= 0, 'gp_fit: dpotrf argument error')
+    # 1 + the index of the first non-positive pivot; some dpotrf builds do not flag NaN pivots,
+    # which leave NaN on the diagonal
+    nan_piv = np.flatnonzero(np.isnan(np.diagonal(Lc)[:bad - 1 if bad else n]))
+    if nan_piv.size:
+        bad = int(nan_piv[0]) + 1
+    info_v[0] = bad
+    if bad:
         return
-    info_v[0] = 0
-    import scipy.linalg as sl
-    Lp, Wp = _gp_factors(Lc, n, n_pad)
+    Lp = np.eye(n_pad)
+    Lp[:n, :n] = Lc
+    Wp = sl.solve_triangular(Lp, np.eye(n_pad), lower=True)
     _mat(L, n_pad, n_pad)[:] = Lp
     _mat(W, n_pad, n_pad)[:] = Wp
     _mat(U, n_pad, n_pad)[:] = Wp.T
     _vec(alpha, n)[:] = sl.cho_solve((Lc, True), yv)
 
 
-def _gp_state(X, ldX, n, p, W, n_pad, alpha):
+def _gp_query(Xq, ldq, m, X, ldX, n, p, W, n_pad, kernel_var, lengthscale, bias_var):
+    """(k = k(Xq, X) (m, n), W[:n, :n]) for the entry points that take a fitted W."""
+    _require(m >= 0 and n >= 1 and p >= 1 and ldq >= p and ldX >= p, 'gp: bad shape')
+    _require(n_pad == _gp_padded(n), 'gp: bad n_pad')
     Xm = np.ascontiguousarray(_mat(X, n, p, ldX))
-    Wn = _mat(W, n_pad, n_pad)[:n, :n]
-    return Xm, np.linalg.inv(Wn), _vec(alpha, n).copy()[:, None]
+    xq = np.ascontiguousarray(_mat(Xq, m, p, ldq))
+    return _gp_kernel(xq, Xm, kernel_var, lengthscale, bias_var), np.array(_mat(W, n_pad, n_pad)[:n, :n])
 
 
 def gp_predict_f64(ctx, Xq, ldq, m, X, ldX, n, p, W, n_pad, alpha, kernel_var, lengthscale,
                    bias_var, noise_add, beta, mean, var, acq, stream):
-    Xm, Lc, al = _gp_state(X, ldX, n, p, W, n_pad, alpha)
-    xq = np.ascontiguousarray(_mat(Xq, m, p, ldq))
-    mu, v = o.gp_predict(xq, Xm, Lc, al, kernel_var, lengthscale, bias_var)
-    mu, v = mu.ravel(), v.ravel()
+    k, Wn = _gp_query(Xq, ldq, m, X, ldX, n, p, W, n_pad, kernel_var, lengthscale, bias_var)
+    if m == 0:
+        return
+    t = k.dot(Wn.T)
+    mu = k.dot(_vec(alpha, n))
+    v = (kernel_var + bias_var) - np.sum(t * t, axis=1)
     if _addr(mean):
         _vec(mean, m)[:] = mu
     if _addr(var):
         _vec(var, m)[:] = v + noise_add
     if _addr(acq):
-        _vec(acq, m)[:] = o.lcbsc(mu, v, beta)
+        with np.errstate(invalid='ignore'):
+            _vec(acq, m)[:] = o.lcbsc(mu, v, beta)
 
 
 def gp_predict_grad_f64(ctx, Xq, ldq, m, X, ldX, n, p, W, U, n_pad, alpha, kernel_var,
                         lengthscale, bias_var, mean, var, grad_mean, grad_var, stream):
-    Xm, Lc, al = _gp_state(X, ldX, n, p, W, n_pad, alpha)
-    xq = np.ascontiguousarray(_mat(Xq, m, p, ldq))
-    mu, v = o.gp_predict(xq, Xm, Lc, al, kernel_var, lengthscale, bias_var)
-    gm, gv = o.gp_predictive_gradients(xq, Xm, Lc, al, kernel_var, lengthscale, bias_var)
-    _vec(mean, m)[:] = mu.ravel()
-    _vec(var, m)[:] = v.ravel()
-    _mat(grad_mean, m, p)[:] = gm
-    _mat(grad_var, m, p)[:] = gv
+    """gpy_regression.py:206-218 with Ky^-1 = W^T W: t = W k, u = W^T t,
+    grad_mean_d = sum_j dk_jd alpha_j, grad_var_d = -2 sum_j dk_jd u_j."""
+    k, Wn = _gp_query(Xq, ldq, m, X, ldX, n, p, W, n_pad, kernel_var, lengthscale, bias_var)
+    if m == 0:
+        return
+    xq = _mat(Xq, m, p, ldq)
+    Xm = _mat(X, n, p, ldX)
+    al = _vec(alpha, n)
+    f = -0.5 / lengthscale ** 2
+    t = k.dot(Wn.T)
+    u = t.dot(Wn)
+    dk = 2.0 * f * (xq[:, None, :] - Xm[None, :, :]) * (k - bias_var)[:, :, None]   # (m, n, p)
+    if _addr(mean):
+        _vec(mean, m)[:] = k.dot(al)
+    if _addr(var):
+        _vec(var, m)[:] = (kernel_var + bias_var) - np.sum(t * t, axis=1)
+    if _addr(grad_mean):
+        _mat(grad_mean, m, p)[:] = np.einsum('qjd,j->qd', dk, al)
+    if _addr(grad_var):
+        _mat(grad_var, m, p)[:] = -2.0 * np.einsum('qjd,qj->qd', dk, u)
 
 
 def gp_whiten_f64(ctx, Xq, ldq, m, X, ldX, n, p, W, n_pad, kernel_var, lengthscale, bias_var, T,
                   ldT, stream):
-    Xm = np.ascontiguousarray(_mat(X, n, p, ldX))
-    xq = np.ascontiguousarray(_mat(Xq, m, p, ldq))
-    Wn = _mat(W, n_pad, n_pad)[:n, :n]
-    r2 = np.sum(xq ** 2, 1)[:, None] + np.sum(Xm ** 2, 1)[None, :] - 2. * xq.dot(Xm.T)
-    k = kernel_var * np.exp(np.maximum(r2, 0.0) * (-0.5 / lengthscale ** 2)) + bias_var
-    _mat(T, m, n, ldT)[:] = k.dot(Wn.T)
+    _require(ldT >= n, 'gp_whiten: bad shape')
+    k, Wn = _gp_query(Xq, ldq, m, X, ldX, n, p, W, n_pad, kernel_var, lengthscale, bias_var)
+    if m:
+        _mat(T, m, n, ldT)[:] = k.dot(Wn.T)
 
 
 def gp_apply_wt_f64(ctx, T, ldT, m, U, n_pad, n, out, ldo, stream):
-    Wn = _mat(U, n_pad, n_pad)[:n, :n].T
-    _mat(out, m, n, ldo)[:] = _mat(T, m, n, ldT).dot(Wn)
+    _require(m >= 0 and n >= 1 and ldT >= n and ldo >= n and n_pad >= n, 'gp_apply_wt: bad shape')
+    if m:
+        Un = _mat(U, n_pad, n_pad)[:n, :n]
+        _mat(out, m, n, ldo)[:] = _mat(T, m, n, ldT).dot(Un.T)
 
 
 def gp_cross_cov_f64(ctx, Xa, lda, ma, Ta, ldTa, Xb, ldb, mb, Tb, ldTb, n, p, kernel_var,
                      lengthscale, bias_var, cov, stream):
+    if not (ma and mb):
+        return
     xa = np.ascontiguousarray(_mat(Xa, ma, p, lda))
     xb = np.ascontiguousarray(_mat(Xb, mb, p, ldb))
-    r2 = np.sum(xb ** 2, 1)[:, None] + np.sum(xa ** 2, 1)[None, :] - 2. * xb.dot(xa.T)
-    k = kernel_var * np.exp(np.maximum(r2, 0.0) * (-0.5 / lengthscale ** 2)) + bias_var
-    _mat(cov, mb, ma)[:] = k - _mat(Tb, mb, n, ldTb).dot(_mat(Ta, ma, n, ldTa).T)
+    k = _gp_kernel(xb, xa, kernel_var, lengthscale, bias_var)
+    g = _mat(Tb, mb, n, ldTb).dot(_mat(Ta, ma, n, ldTa).T)
+    if (_addr(Xa), lda, ma, _addr(Ta), ldTa) == (_addr(Xb), ldb, mb, _addr(Tb), ldTb):
+        # one point set: the device computes the same dot product for (a, b) and (b, a)
+        g = np.tril(g) + np.tril(g, -1).T
+    _mat(cov, mb, ma)[:] = k - g
 
 
 def lcbsc_f64(ctx, mean, var, grad_mean, grad_var, m, p, beta, acq, grad_acq, stream):
