@@ -11,11 +11,11 @@ import numpy as np
 import scipy.stats as ss
 import torch
 
-from .. import device as dev
 from .. import model as em
 from .. import ops
 from ..priors import DeviceModelPrior
-from .gnk import LazyGNKData, euclidean_multiss, ss_robust
+from ..throughput import batch_columns, batch_key
+from .gnk import euclidean_multiss, lazy_gnk, ss_robust
 
 PARAMETER_NAMES = ['a1', 'a2', 'b1', 'b2', 'g1', 'g2', 'k1', 'k2', 'rho']
 
@@ -70,36 +70,16 @@ def get_model(n_obs=150, true_params=None, seed=None):
 
 
 # ---------------------------------------------------------------------------- throughput mode
-class LazyBiGNKData(LazyGNKData):
-    """Output of :func:`bignk_device`: P (B, 9) parameters on the device; the summaries are
-    fused into the simulator for n_obs <= 512, materialize() gives the (B, n_obs, 2) data."""
-
-    def __init__(self, P, c, n_obs, key):
-        self.P, self.c, self.n_obs, self.key = P, c, n_obs, key
-        self.shape = (int(P.shape[0]), n_obs, 2)
-        self.ndim = 3
-        self._S = {}
-
-    def _fused(self, kind):
-        return ops.sim_bignk(self.P, self.n_obs, seed=self.key, c=self.c, want_data=False,
-                             kind=kind)[1]
-
-    def materialize(self):
-        return ops.sim_bignk(self.P, self.n_obs, seed=self.key, c=self.c)[0]
-
-
 def bignk_device(A1, A2, B1, B2, g1, g2, k1, k2, rho, c=.8, n_obs=150, batch_size=1,
                  random_state=None):
-    """Device twin of BiGNK (Philox streams, ops.sim_bignk); returns a LazyBiGNKData."""
-    from .gauss import _key
-
-    def as_dev(v):
-        if dev.is_device_array(v):
-            return v.reshape(-1)
-        return dev.to_device(np.broadcast_to(np.asarray(v, dtype=np.float64).reshape(-1),
-                                             (batch_size,)).copy())
-    P = torch.stack([as_dev(v) for v in (A1, A2, B1, B2, g1, g2, k1, k2, rho)], dim=1)
-    return LazyBiGNKData(P, c, n_obs, _key(random_state))
+    """Device twin of BiGNK (Philox streams, ops.sim_bignk) with ss_robust / ss_octile fused into
+    the simulator; returns a LazySimulation of shape (batch_size, n_obs, 2)."""
+    P = torch.stack(batch_columns((A1, A2, B1, B2, g1, g2, k1, k2, rho), batch_size), dim=1)
+    key = batch_key(random_state)
+    return lazy_gnk(
+        (int(P.shape[0]), n_obs, 2),
+        lambda kind: ops.sim_bignk(P, n_obs, seed=key, c=c, want_data=False, kind=kind)[1],
+        lambda: ops.sim_bignk(P, n_obs, seed=key, c=c)[0])
 
 
 def get_device_model(n_obs=150, true_params=None, seed=None):

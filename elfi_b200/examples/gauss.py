@@ -6,6 +6,10 @@ import scipy.stats as ss
 
 from .. import model as em
 from .. import ops
+from ..throughput import LazySimulation, batch_columns, batch_key
+
+# the key draw under its earlier name, which tests/device_prior_cases.py seeds its simulator with
+_key = batch_key
 
 
 def gauss(mu, sigma, n_obs=50, batch_size=1, random_state=None):
@@ -18,78 +22,54 @@ def gauss(mu, sigma, n_obs=50, batch_size=1, random_state=None):
 
 def ss_mean(y):
     """np.mean(y, axis=1) on the device (elfi/examples/gauss.py:142-156)."""
-    return ops.meanvar(y)[:, 0]
+    return y.summaries()[:, 0] if isinstance(y, LazySimulation) else ops.meanvar(y)[:, 0]
 
 
 def ss_var(y):
     """np.var(y, axis=1) on the device (elfi/examples/gauss.py:159-173)."""
-    return ops.meanvar(y)[:, 1]
+    return y.summaries()[:, 1] if isinstance(y, LazySimulation) else ops.meanvar(y)[:, 1]
 
 
-def get_model(n_obs=50, true_params=None, seed_obs=None):
-    """elfi/examples/gauss.py:75-139 (nd_mean=False)."""
-    if true_params is None:
-        true_params = [4, .4]
-    fn_simulator = partial(gauss, n_obs=n_obs)
-    y_obs = fn_simulator(*true_params, n_obs=n_obs, random_state=np.random.RandomState(seed_obs))
-    m = em.new_model()
+def _prior_params(true_params):
+    """[mu_lo, mu_width, a, b] of the priors uniform(mu_lo, mu_width) of mu and truncnorm(a, b) of
+    sigma."""
     eps_prior = 5
-    priors = [em.Prior('uniform', true_params[0] - eps_prior, 2 * eps_prior, model=m, name='mu'),
-              em.Prior('truncnorm', np.amax([.01, true_params[1] - eps_prior]), 2 * eps_prior,
-                       model=m, name='sigma')]
-    em.Simulator(fn_simulator, *priors, observed=y_obs, name='gauss')
+    return [true_params[0] - eps_prior, 2 * eps_prior,
+            np.amax([.01, true_params[1] - eps_prior]), 2 * eps_prior]
+
+
+def _graph(m, uniform, truncnorm, prm, simulator, y_obs):
+    """Priors, simulator, summaries and distance of elfi/examples/gauss.py:75-139."""
+    priors = [em.Prior(uniform, prm[0], prm[1], model=m, name='mu'),
+              em.Prior(truncnorm, prm[2], prm[3], model=m, name='sigma')]
+    em.Simulator(simulator, *priors, observed=y_obs, name='gauss')
     sumstats = [em.Summary(ss_mean, m['gauss'], name='ss_mean'),
                 em.Summary(ss_var, m['gauss'], name='ss_var')]
     em.Distance('euclidean', *sumstats, name='d')
     return m
 
 
+def get_model(n_obs=50, true_params=None, seed_obs=None):
+    """elfi/examples/gauss.py:75-139 (nd_mean=False)."""
+    if true_params is None:
+        true_params = [4, .4]
+    y_obs = gauss(*true_params, n_obs=n_obs, random_state=np.random.RandomState(seed_obs))
+    return _graph(em.new_model(), 'uniform', 'truncnorm', _prior_params(true_params),
+                  partial(gauss, n_obs=n_obs), y_obs)
+
+
 # ---------------------------------------------------------------------------- throughput mode
 # Device-side priors, simulator fused with its mean / variance summaries, and proposals
 # (Philox streams; statistical parity with the host path).  See examples/ma2.py for the design.
-def _key(random_state):
-    random_state = random_state or np.random
-    return int(random_state.randint(2 ** 31 - 1))
-
-
-class LazyGaussData:
-    """Simulator output materialised only on request (summaries come from the same kernel)."""
-
-    def __init__(self, mu, sigma, n_obs, key):
-        self.mu, self.sigma, self.n_obs, self.key = mu, sigma, n_obs, key
-        self.shape = (int(mu.numel()), n_obs)
-        self.ndim = 2
-        self._S = None
-
-    def __len__(self):
-        return self.shape[0]
-
-    def summaries(self):
-        if self._S is None:
-            self._S = ops.sim_gauss(self.mu, self.sigma, self.n_obs, seed=self.key)[1]
-        return self._S
-
-    def materialize(self):
-        return ops.sim_gauss(self.mu, self.sigma, self.n_obs, seed=self.key, want_data=True,
-                             want_summaries=False)[0]
-
-
 def gauss_device(mu, sigma, n_obs=50, batch_size=1, random_state=None):
-    from .. import device as dev
-
-    def as_dev(v):
-        if dev.is_device_array(v):
-            return v.reshape(-1)
-        return dev.to_device(np.broadcast_to(np.asarray(v, dtype=np.float64), (batch_size,)).copy())
-    return LazyGaussData(as_dev(mu), as_dev(sigma), n_obs, _key(random_state))
-
-
-def ss_mean_any(y):
-    return y.summaries()[:, 0] if isinstance(y, LazyGaussData) else ss_mean(y)
-
-
-def ss_var_any(y):
-    return y.summaries()[:, 1] if isinstance(y, LazyGaussData) else ss_var(y)
+    """Device twin of gauss with the mean and variance fused into the simulator; returns a
+    LazySimulation."""
+    mu, sigma = batch_columns((mu, sigma), batch_size)
+    key = batch_key(random_state)
+    return LazySimulation(
+        (int(mu.numel()), n_obs),
+        lambda kind: ops.sim_gauss(mu, sigma, n_obs, seed=key)[1],
+        lambda: ops.sim_gauss(mu, sigma, n_obs, seed=key, want_data=True, want_summaries=False)[0])
 
 
 class DeviceProposal:
@@ -114,7 +94,7 @@ class _DeviceUniform:
     @staticmethod
     def rvs(loc, scale, size=1, random_state=None):
         n = int(np.prod(size))
-        u = ops.prior_gauss(n, _key(random_state), [0.0, 1.0, 0.0, 1.0])[0]
+        u = ops.prior_gauss(n, batch_key(random_state), [0.0, 1.0, 0.0, 1.0])[0]
         return loc + scale * u
 
     pdf = staticmethod(lambda x, loc, scale: ss.uniform.pdf(x, loc, scale))
@@ -127,7 +107,7 @@ class _DeviceTruncnorm:
     @staticmethod
     def rvs(a, b, size=1, random_state=None):
         n = int(np.prod(size))
-        return ops.prior_gauss(n, _key(random_state), [0.0, 1.0, a, b])[1]
+        return ops.prior_gauss(n, batch_key(random_state), [0.0, 1.0, a, b])[1]
 
     pdf = staticmethod(lambda x, a, b: ss.truncnorm.pdf(x, a, b))
     logpdf = staticmethod(lambda x, a, b: ss.truncnorm.logpdf(x, a, b))
@@ -139,14 +119,7 @@ def get_device_model(n_obs=50, true_params=None, seed_obs=None):
     if true_params is None:
         true_params = [4, .4]
     y_obs = gauss(*true_params, n_obs=n_obs, random_state=np.random.RandomState(seed_obs))
-    eps_prior = 5
-    mu_lo, mu_w = true_params[0] - eps_prior, 2 * eps_prior
-    a, b = float(np.amax([.01, true_params[1] - eps_prior])), float(2 * eps_prior)
-    m = em.new_model()
-    priors = [em.Prior(_DeviceUniform, mu_lo, mu_w, model=m, name='mu'),
-              em.Prior(_DeviceTruncnorm, a, b, model=m, name='sigma')]
-    em.Simulator(partial(gauss_device, n_obs=n_obs), *priors, observed=y_obs, name='gauss')
-    sumstats = [em.Summary(ss_mean_any, m['gauss'], name='ss_mean'),
-                em.Summary(ss_var_any, m['gauss'], name='ss_var')]
-    em.Distance('euclidean', *sumstats, name='d')
-    return m, DeviceProposal([mu_lo, mu_w, a, b])
+    prm = _prior_params(true_params)
+    m = _graph(em.new_model(), _DeviceUniform, _DeviceTruncnorm, prm,
+               partial(gauss_device, n_obs=n_obs), y_obs)
+    return m, DeviceProposal(prm)

@@ -12,6 +12,7 @@ import scipy.stats as ss
 from .. import device as dev
 from .. import model as em
 from .. import ops
+from ..throughput import LazySimulation, batch_columns, batch_key
 
 
 def GNK(A, B, g, k, c=0.8, n_obs=50, batch_size=1, random_state=None):
@@ -51,7 +52,7 @@ def euclidean_multiss(*simulated, observed):
 
 def _lazy_summaries(y, kind):
     """(B, width * d, 1) summaries of lazy simulator output or device data; None for host data."""
-    if isinstance(y, LazyGNKData):
+    if isinstance(y, LazySimulation):
         return y.summaries(kind)[:, :, None]
     if dev.is_device_array(y):
         return ops.gnk_summaries(y, kind)[:, :, None]
@@ -136,15 +137,8 @@ def get_adaptive_model(n_obs=256, true_params=None, seed=None):
 # and consumed by the nested-distance kernel; only accepted particles leave the device.
 def gnk_device(A, B, g, k, c=0.8, n_obs=50, batch_size=1, random_state=None):
     """Device twin of GNK: returns a (batch_size, n_obs) CUDA tensor."""
-    from .gauss import _key
-
-    def as_dev(v):
-        if dev.is_device_array(v):
-            return v.reshape(-1)
-        return dev.to_device(np.broadcast_to(np.asarray(v, dtype=np.float64).reshape(-1),
-                                             (batch_size,)).copy())
-    return ops.sim_gnk(as_dev(A), as_dev(B), as_dev(g), as_dev(k), n_obs=n_obs,
-                       seed=_key(random_state), c=c)
+    return ops.sim_gnk(*batch_columns((A, B, g, k), batch_size), n_obs=n_obs,
+                       seed=batch_key(random_state), c=c)
 
 
 class DeviceProposal:
@@ -164,47 +158,26 @@ class DeviceProposal:
         return ops.logprior_box(params, self.lo, self.width)
 
 
-class LazyGNKData:
-    """Output of :func:`gnk_device_lazy`: the robust / octile summaries are computed in the
-    simulator kernel (n_obs <= 512), so the (B, n_obs) data is only written when asked for
-    (for n_obs > 512 the summaries are taken from the written data).  Subclasses replace
-    _fused and materialize."""
-
-    def __init__(self, A, B, g, k, c, n_obs, key):
-        self.params, self.c, self.n_obs, self.key = (A, B, g, k), c, n_obs, key
-        self.shape = (int(A.numel()), n_obs, 1)
-        self.ndim = 3
-        self._S = {}
-
-    def __len__(self):
-        return self.shape[0]
-
-    def summaries(self, kind):
-        """(B, width) summaries of kind 'ss_robust' or 'ss_octile'."""
-        if kind not in self._S:
-            self._S[kind] = self._fused(kind) if self.n_obs <= ops.GNK_FUSED_MAX else \
-                ops.gnk_summaries(self.materialize(), kind)
-        return self._S[kind]
-
-    def _fused(self, kind):
-        return ops.sim_gnk_summaries(*self.params, n_obs=self.n_obs, seed=self.key, c=self.c,
-                                     kind=kind)
-
-    def materialize(self):
-        """The simulated data, (B, n_obs, 1) on the device."""
-        return ops.sim_gnk(*self.params, n_obs=self.n_obs, seed=self.key, c=self.c)[:, :, None]
+def lazy_gnk(shape, fused, materialize):
+    """The LazySimulation of a g-and-k simulator of shape (B, n_obs, d): the robust / octile
+    summaries of a kind are fused(kind) for n_obs <= ops.GNK_FUSED_MAX, else taken from the
+    written data."""
+    def summarise(kind):
+        if shape[1] <= ops.GNK_FUSED_MAX:
+            return fused(kind)
+        return ops.gnk_summaries(materialize(), kind)
+    return LazySimulation(shape, summarise, materialize)
 
 
 def gnk_device_lazy(A, B, g, k, c=0.8, n_obs=50, batch_size=1, random_state=None):
-    """Device twin of GNK whose robust / octile summaries are fused into the simulator."""
-    from .gauss import _key
-
-    def as_dev(v):
-        if dev.is_device_array(v):
-            return v.reshape(-1)
-        return dev.to_device(np.broadcast_to(np.asarray(v, dtype=np.float64).reshape(-1),
-                                             (batch_size,)).copy())
-    return LazyGNKData(as_dev(A), as_dev(B), as_dev(g), as_dev(k), c, n_obs, _key(random_state))
+    """Device twin of GNK whose robust / octile summaries are fused into the simulator; returns a
+    LazySimulation of shape (batch_size, n_obs, 1)."""
+    cols = batch_columns((A, B, g, k), batch_size)
+    key = batch_key(random_state)
+    return lazy_gnk(
+        (int(cols[0].numel()), n_obs, 1),
+        lambda kind: ops.sim_gnk_summaries(*cols, n_obs=n_obs, seed=key, c=c, kind=kind),
+        lambda: ops.sim_gnk(*cols, n_obs=n_obs, seed=key, c=c)[:, :, None])
 
 
 def get_device_model(n_obs=256, true_params=None, seed=None, summary='ss_sorted'):

@@ -22,6 +22,7 @@ from .. import device as dev
 from .. import model as em
 from .. import ops
 from ..priors import DeviceModelPrior
+from ..throughput import LazySimulation, batch_columns, batch_key
 
 # the state at time 0 of the task (lorenz.py:129-139), one value per variable of the ring
 INITIAL_STATE = np.array([
@@ -90,7 +91,7 @@ def forecast_lorenz(theta1=None, theta2=None, f=10., phi=0.984, n_obs=40, n_time
 # ---------------------------------------------------------------------------- summaries
 def _summary(x, col):
     """Column col of the six summaries for lazy simulator output or device data; None for host data."""
-    if isinstance(x, LazyLorenzData):
+    if isinstance(x, LazySimulation):
         return x.summaries()[:, col]
     if dev.is_device_array(x):
         return ops.lorenz_summaries(x)[:, col]
@@ -176,47 +177,18 @@ def get_model(true_params=None, seed_obs=None, initial_state=None, n_obs=40, f=1
 
 
 # ---------------------------------------------------------------------------- throughput mode
-class LazyLorenzData:
-    """Output of :func:`lorenz_device`: P (B, 2) parameters on the device.  The six summaries are
-    computed in the simulator kernel (the (B, n_timestep, n_obs) data is never written);
-    materialize() gives the data."""
-
-    def __init__(self, P, key, sim_kwargs):
-        self.P, self.key, self.sim_kwargs = P, key, sim_kwargs
-        n_obs = len(sim_kwargs['initial_state'])
-        self.shape = (int(P.shape[0]), int(sim_kwargs['n_timestep']), n_obs)
-        self.ndim = 3
-        self._S = None
-
-    def __len__(self):
-        return self.shape[0]
-
-    def summaries(self):
-        """(B, 6) [Mean, Var, Autocov, Cov, CrosscovPrev, CrosscovNext] of the simulated rows."""
-        if self._S is None:
-            self._S = ops.sim_lorenz(self.P, seed=self.key, **self.sim_kwargs)[1]
-        return self._S
-
-    def materialize(self):
-        """The simulated data, (B, n_timestep, n_obs) on the device."""
-        return ops.sim_lorenz(self.P, seed=self.key, want_data=True, want_summaries=False,
-                              **self.sim_kwargs)[0]
-
-
 def lorenz_device(theta1, theta2, initial_state=INITIAL_STATE, n_timestep=160, f=10., phi=0.984,
                   total_duration=4, batch_size=1, random_state=None):
-    """Device twin of forecast_lorenz; returns a LazyLorenzData."""
-    from .gauss import _key
-
-    def as_dev(v):
-        if dev.is_device_array(v):
-            return v.reshape(-1)
-        return dev.to_device(np.broadcast_to(np.asarray(v, dtype=np.float64).reshape(-1),
-                                             (batch_size,)).copy())
-    P = torch.stack([as_dev(theta1), as_dev(theta2)], dim=1)
+    """Device twin of forecast_lorenz; returns a LazySimulation of shape (batch_size, n_timestep,
+    n_obs) whose six summaries are computed in the simulator kernel."""
+    P = torch.stack(batch_columns((theta1, theta2), batch_size), dim=1)
+    key = batch_key(random_state)
     kw = dict(initial_state=initial_state, n_timestep=n_timestep, f=f, phi=phi,
               total_duration=total_duration)
-    return LazyLorenzData(P, _key(random_state), kw)
+    return LazySimulation(
+        (int(P.shape[0]), int(n_timestep), len(initial_state)),
+        lambda kind: ops.sim_lorenz(P, seed=key, **kw)[1],
+        lambda: ops.sim_lorenz(P, seed=key, want_data=True, want_summaries=False, **kw)[0])
 
 
 def get_device_model(true_params=None, seed_obs=None, f=10., phi=0.984, total_duration=4):

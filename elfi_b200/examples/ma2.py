@@ -11,6 +11,7 @@ import scipy.stats as ss
 
 from .. import model as em
 from .. import ops
+from ..throughput import LazySimulation, batch_columns, batch_key
 
 
 def MA2(t1, t2, n_obs=100, batch_size=1, random_state=None):
@@ -24,7 +25,12 @@ def MA2(t1, t2, n_obs=100, batch_size=1, random_state=None):
 
 
 def autocov(x, lag=1):
-    """Autocovariance summary on the device (elfi/examples/ma2.py:40-59); returns (B,)."""
+    """Autocovariance summary on the device (elfi/examples/ma2.py:40-59); returns (B,).  Lags 1 and
+    2 of lazy simulator output come from the simulator kernel, other lags from its data."""
+    if isinstance(x, LazySimulation):
+        if lag in (1, 2):
+            return x.summaries()[:, lag - 1]
+        x = x.materialize()
     x = np.atleast_2d(x) if not hasattr(x, 'is_cuda') else x
     return ops.autocov(x, lags=(lag,))[:, 0]
 
@@ -69,20 +75,27 @@ class CustomPrior2:
             return np.log(cls.pdf(x, t1, a))
 
 
-def get_model(n_obs=100, true_params=None, seed_obs=None):
-    """MA2 inference task (elfi/examples/ma2.py:62-92)."""
-    if true_params is None:
-        true_params = [.6, .2]
-    y = MA2(*true_params, n_obs=n_obs, random_state=np.random.RandomState(seed_obs))
-    sim_fn = partial(MA2, n_obs=n_obs)
-    m = em.ElfiModel()
-    em.Prior(CustomPrior1, 2, model=m, name='t1')
-    em.Prior(CustomPrior2, m['t1'], 1, name='t2')
-    em.Simulator(sim_fn, m['t1'], m['t2'], observed=y, name='MA2')
+def _graph(m, prior1, prior2, simulator, y):
+    """Priors, simulator, summaries and distance of elfi/examples/ma2.py:62-92."""
+    em.Prior(prior1, 2, model=m, name='t1')
+    em.Prior(prior2, m['t1'], 1, name='t2')
+    em.Simulator(simulator, m['t1'], m['t2'], observed=y, name='MA2')
     em.Summary(autocov, m['MA2'], name='S1')
     em.Summary(autocov, m['MA2'], 2, name='S2')
     em.Distance('euclidean', m['S1'], m['S2'], name='d')
     return m
+
+
+def _observed(n_obs, true_params, seed_obs):
+    if true_params is None:
+        true_params = [.6, .2]
+    return MA2(*true_params, n_obs=n_obs, random_state=np.random.RandomState(seed_obs))
+
+
+def get_model(n_obs=100, true_params=None, seed_obs=None):
+    """MA2 inference task (elfi/examples/ma2.py:62-92)."""
+    return _graph(em.ElfiModel(), CustomPrior1, CustomPrior2, partial(MA2, n_obs=n_obs),
+                  _observed(n_obs, true_params, seed_obs))
 
 
 # ---------------------------------------------------------------------------- throughput mode
@@ -91,50 +104,15 @@ def get_model(n_obs=100, true_params=None, seed_obs=None):
 # host RandomState of the reference, not bit-identical; SURVEY.md section 7 "Philox throughput
 # mode").  The per-node key is drawn from the batch's host RandomState, so results stay a
 # deterministic function of (seed, batch_index).
-def _key(random_state):
-    random_state = random_state or np.random
-    return int(random_state.randint(2 ** 31 - 1))
-
-
-class LazyMA2Data:
-    """Simulator output that is only materialised on request: the summaries are computed in the
-    simulator kernel, so the (B, n_obs) data never has to be written to HBM."""
-
-    def __init__(self, t1, t2, n_obs, key):
-        self.t1, self.t2, self.n_obs, self.key = t1, t2, n_obs, key
-        self.shape = (int(t1.numel()), n_obs)
-        self.ndim = 2
-        self._S = None
-
-    def __len__(self):
-        return self.shape[0]
-
-    def summaries(self):
-        if self._S is None:
-            self._S = ops.sim_ma2(self.t1, self.t2, self.n_obs, seed=self.key)[1]
-        return self._S
-
-    def materialize(self):
-        return ops.sim_ma2(self.t1, self.t2, self.n_obs, seed=self.key, want_data=True,
-                           want_summaries=False)[0]
-
-
 def MA2_device(t1, t2, n_obs=100, batch_size=1, random_state=None):
-    from .. import device as dev
-    t1 = dev.to_device(np.broadcast_to(np.asarray(t1, dtype=np.float64), (batch_size,)).copy()
-                       if not dev.is_device_array(t1) else t1).reshape(-1)
-    t2 = dev.to_device(np.broadcast_to(np.asarray(t2, dtype=np.float64), (batch_size,)).copy()
-                       if not dev.is_device_array(t2) else t2).reshape(-1)
-    return LazyMA2Data(t1, t2, n_obs, _key(random_state))
-
-
-def autocov_any(x, lag=1):
-    """autocov for host arrays, device arrays and lazily simulated MA2 data."""
-    if isinstance(x, LazyMA2Data):
-        if lag in (1, 2):
-            return x.summaries()[:, lag - 1]
-        x = x.materialize()
-    return autocov(x, lag)
+    """Device twin of MA2 with autocov lags 1 and 2 fused into the simulator; returns a
+    LazySimulation."""
+    t1, t2 = batch_columns((t1, t2), batch_size)
+    key = batch_key(random_state)
+    return LazySimulation(
+        (int(t1.numel()), n_obs),
+        lambda kind: ops.sim_ma2(t1, t2, n_obs, seed=key)[1],
+        lambda: ops.sim_ma2(t1, t2, n_obs, seed=key, want_data=True, want_summaries=False)[0])
 
 
 class DevicePrior1(CustomPrior1):
@@ -142,14 +120,14 @@ class DevicePrior1(CustomPrior1):
     def rvs(cls, b, size=1, random_state=None):
         assert b == 2, 'device MA2 prior is specialised to b = 2'
         n = int(np.prod(size))
-        return ops.prior_ma2(n, _key(random_state), which='t1')
+        return ops.prior_ma2(n, batch_key(random_state), which='t1')
 
 
 class DevicePrior2(CustomPrior2):
     @classmethod
     def rvs(cls, t1, a, size=1, random_state=None):
         assert a == 1, 'device MA2 prior is specialised to a = 1'
-        return ops.prior_ma2(0, _key(random_state), t1=t1, which='t2')
+        return ops.prior_ma2(0, batch_key(random_state), t1=t1, which='t2')
 
 
 class DeviceProposal:
@@ -170,14 +148,5 @@ class DeviceProposal:
 def get_device_model(n_obs=100, true_params=None, seed_obs=None):
     """MA2 inference task with priors, simulator and summaries on the device (same graph and
     names as get_model).  Pass ``device_proposal=DeviceProposal`` to SMC for device proposals."""
-    if true_params is None:
-        true_params = [.6, .2]
-    y = MA2(*true_params, n_obs=n_obs, random_state=np.random.RandomState(seed_obs))
-    m = em.ElfiModel()
-    em.Prior(DevicePrior1, 2, model=m, name='t1')
-    em.Prior(DevicePrior2, m['t1'], 1, name='t2')
-    em.Simulator(partial(MA2_device, n_obs=n_obs), m['t1'], m['t2'], observed=y, name='MA2')
-    em.Summary(autocov_any, m['MA2'], name='S1')
-    em.Summary(autocov_any, m['MA2'], 2, name='S2')
-    em.Distance('euclidean', m['S1'], m['S2'], name='d')
-    return m
+    return _graph(em.ElfiModel(), DevicePrior1, DevicePrior2, partial(MA2_device, n_obs=n_obs),
+                  _observed(n_obs, true_params, seed_obs))

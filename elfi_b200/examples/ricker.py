@@ -21,6 +21,7 @@ from .. import device as dev
 from .. import model as em
 from .. import ops
 from ..priors import DeviceModelPrior
+from ..throughput import LazySimulation, batch_columns, batch_key
 
 
 def ricker(log_rate, stock_init=1., n_obs=50, batch_size=1, random_state=None):
@@ -58,7 +59,7 @@ def stochastic_ricker(log_rate, std, scale, stock_init=1., n_obs=50, batch_size=
 
 def _summary(y, col):
     """Column col of [mean, var, #0] for lazy simulator output or device data; None for host data."""
-    if isinstance(y, LazyRickerData):
+    if isinstance(y, LazySimulation):
         return y.summaries()[:, col]
     if dev.is_device_array(y):
         return ops.meanvar(y)[:, col] if col < 2 else ops.count_zeros(y)
@@ -137,45 +138,17 @@ def get_model(n_obs=50, true_params=None, seed_obs=None, stochastic=True):
 
 
 # ---------------------------------------------------------------------------- throughput mode
-class LazyRickerData:
-    """Output of :func:`ricker_device`: P (B, 3) or (B, 1) parameters on the device.  The summaries
-    [mean, var, #0] are computed in the simulator kernel for n_obs <= ops.RICKER_FUSED_MAX (the
-    data is never written); materialize() gives the (B, n_obs) data."""
-
-    def __init__(self, P, n_obs, key, stochastic):
-        self.P, self.n_obs, self.key, self.stochastic = P, n_obs, key, stochastic
-        self.shape = (int(P.shape[0]), n_obs)
-        self.ndim = 2
-        self._S = None
-
-    def __len__(self):
-        return self.shape[0]
-
-    def summaries(self):
-        """(B, 3) [mean, var, #0] of the simulated rows."""
-        if self._S is None:
-            self._S = ops.sim_ricker(self.P, self.n_obs, seed=self.key,
-                                     stochastic=self.stochastic)[2]
-        return self._S
-
-    def materialize(self):
-        """The simulated data, (B, n_obs) on the device."""
-        return ops.sim_ricker(self.P, self.n_obs, seed=self.key, stochastic=self.stochastic,
-                              want_data=True, want_summaries=False)[0]
-
-
 def ricker_device(*params, n_obs=50, stochastic=True, batch_size=1, random_state=None):
     """Device twin of stochastic_ricker (params log_rate, std, scale) or, with stochastic=False,
-    of ricker (log_rate); returns a LazyRickerData."""
-    from .gauss import _key
-
-    def as_dev(v):
-        if dev.is_device_array(v):
-            return v.reshape(-1)
-        return dev.to_device(np.broadcast_to(np.asarray(v, dtype=np.float64).reshape(-1),
-                                             (batch_size,)).copy())
-    P = torch.stack([as_dev(v) for v in params], dim=1)
-    return LazyRickerData(P, n_obs, _key(random_state), stochastic)
+    of ricker (log_rate); returns a LazySimulation of shape (batch_size, n_obs) whose summaries
+    are [mean, var, #0], computed in the simulator kernel for n_obs <= ops.RICKER_FUSED_MAX."""
+    P = torch.stack(batch_columns(params, batch_size), dim=1)
+    key = batch_key(random_state)
+    return LazySimulation(
+        (int(P.shape[0]), n_obs),
+        lambda kind: ops.sim_ricker(P, n_obs, seed=key, stochastic=stochastic)[2],
+        lambda: ops.sim_ricker(P, n_obs, seed=key, stochastic=stochastic, want_data=True,
+                               want_summaries=False)[0])
 
 
 def get_device_model(n_obs=50, true_params=None, seed_obs=None, stochastic=True):

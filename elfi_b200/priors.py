@@ -25,13 +25,9 @@ import scipy.stats as ss
 
 from . import model as em
 from . import ops
+from .throughput import batch_key
 
 SUPPORTED = ops.PRIOR_KINDS
-
-
-def _key(random_state):
-    from .examples.gauss import _key as key
-    return key(random_state)
 
 
 def _kind_of(distribution):
@@ -76,7 +72,7 @@ class DevicePriorDistribution:
 
     def rvs(self, *params, size=1, random_state=None):
         n = int(np.prod(size))
-        return ops.prior_rvs(prior_spec(self.kind, params), n, _key(random_state))
+        return ops.prior_rvs(prior_spec(self.kind, params), n, batch_key(random_state))
 
     def pdf(self, x, *params):
         return self.scipy.pdf(x, *params)
