@@ -95,6 +95,10 @@ SIGNATURES = {
                                  c_dbl, c_u64, c_u64, c_ptr, c_ptr, c_i64, c_ptr],
     'elfi_b200_lorenz_summaries_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr,
                                        c_i64, c_ptr],
+    'elfi_b200_sim_toad_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_u64, c_u64, c_ptr, c_i64,
+                               c_ptr, c_i64, c_ptr, c_dbl, c_ptr, c_i64, c_ptr],
+    'elfi_b200_toad_summaries_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
+                                     c_i64, c_ptr, c_dbl, c_ptr, c_i64, c_ptr],
     'elfi_b200_prior_rvs_f64': [c_ptr, c_ptr, c_i64, c_u64, c_u64, c_ptr, c_ptr],
     'elfi_b200_prior_logpdf_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     'elfi_b200_gp_padded_size': [c_i64],

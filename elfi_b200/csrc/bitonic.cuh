@@ -18,21 +18,41 @@ __device__ __forceinline__ double u64_to_key(uint64_t u) {
     return __longlong_as_double(static_cast<long long>(u));
 }
 
-// One warp sorts npow2 (a power of two) keys in shared memory ascending, __syncwarp between
-// stages.  The caller syncs the warp before (keys written) and reads the result after.
-__device__ __forceinline__ void bitonic_in_shared(uint64_t* sk, int npow2, int lane) {
+// The network on npow2 (a power of two) keys in shared memory, ascending: nt threads (this one
+// is t0) share the npow2 / 2 compare-exchanges of a stage, and Sync::wait() separates stages.
+template <class Sync>
+__device__ __forceinline__ void bitonic_network_shared(uint64_t* sk, int npow2, int t0, int nt) {
     for (int k = 2; k <= npow2; k <<= 1) {
         for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int t = lane; t < (npow2 >> 1); t += 32) {
+            for (int t = t0; t < (npow2 >> 1); t += nt) {
                 const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
                 const int l = i | j;
                 const bool up = (i & k) == 0;
                 const uint64_t a = sk[i], b = sk[l];
                 if ((a > b) == up) { sk[i] = b; sk[l] = a; }
             }
-            __syncwarp();
+            Sync::wait();
         }
     }
+}
+
+struct WarpSync {
+    static __device__ __forceinline__ void wait() { __syncwarp(); }
+};
+struct CtaSync {
+    static __device__ __forceinline__ void wait() { __syncthreads(); }
+};
+
+// One warp sorts npow2 (a power of two) keys in shared memory ascending, __syncwarp between
+// stages.  The caller syncs the warp before (keys written) and reads the result after.
+__device__ __forceinline__ void bitonic_in_shared(uint64_t* sk, int npow2, int lane) {
+    bitonic_network_shared<WarpSync>(sk, npow2, lane, 32);
+}
+
+// The same network over the whole CTA, __syncthreads between stages.  Every thread of the block
+// calls it; the caller syncs the block before (keys written) and reads the result after.
+__device__ __forceinline__ void bitonic_in_cta(uint64_t* sk, int npow2) {
+    bitonic_network_shared<CtaSync>(sk, npow2, int(threadIdx.x), int(blockDim.x));
 }
 
 // Rows of up to 512 keys: the same network with the keys in REGISTERS.  Lane L holds the KPL

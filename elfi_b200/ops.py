@@ -1083,3 +1083,94 @@ def lorenz_summaries(x):
     _lib.call('elfi_b200_lorenz_summaries_f64', dev.context(), dev.ptr(x), x.stride(0), x.stride(1),
               x.stride(2), B, T, m, dev.ptr(S), LORENZ_NSUMM, dev.stream_ptr())
     return S
+
+
+# ---- Toad movement model (elfi/examples/toad.py) --------------------------------------------------
+TOAD_DISP_MAX = 4096          # displacements of one lag, n_toads * (n_days - lag), sorted per CTA
+TOAD_LAGS_MAX = 8             # lags of the fused summaries
+TOAD_NP_MAX = 32              # quantile levels
+TOAD_CELLS_MAX = 1 << 31      # n_days * n_toads (the stream's block word)
+
+
+def _toad_p(p):
+    p = np.array(p, dtype=np.float64).reshape(-1)
+    if not 1 <= p.size <= TOAD_NP_MAX:
+        raise ValueError('the toad summaries take 1 <= len(p) <= {} quantile levels, got {}'.format(
+            TOAD_NP_MAX, p.size))
+    if not np.all((p >= 0) & (p <= 1)):
+        raise ValueError('the toad quantile levels p must lie in [0, 1]')
+    return np.ascontiguousarray(p)
+
+
+def _toad_lag(lag, n_days):
+    if int(lag) != lag or not 1 <= lag < n_days:
+        raise ValueError('the toad summaries take an integer lag with 1 <= lag < n_days = {}, got {}'
+                         .format(n_days, lag))
+    return int(lag)
+
+
+def _toad_disp(n_toads, rows):
+    if n_toads * rows > TOAD_DISP_MAX:
+        raise ValueError('the device toad summaries take n_toads * (n_days - lag) <= {} '
+                         'displacements, got {} * {}'.format(TOAD_DISP_MAX, n_toads, rows))
+
+
+def sim_toad(params, n_toads=66, n_days=63, seed=0, offset=0, want_data=False, lags=(1, 2, 4, 8),
+             p=np.linspace(0, 1, 11), thd=10.):
+    """Toad movement simulator on the device (elfi/examples/toad.py:16-70).  params: (batch, 3)
+    columns alpha, gamma, p0.  Row i is a pure function of (seed, offset + i); alpha outside (0, 2]
+    or gamma < 0 (where the reference raises) give rows of NaN.
+
+    Returns (X, S), each None unless asked for: X (batch, n_days, n_toads) the positions (batch
+    first; ``X.permute(1, 2, 0)`` is indexed like the reference's array), S (batch, len(lags) *
+    (len(p) + 1)) the summaries of each lag (:func:`toad_summaries`) side by side; lags=None or ()
+    asks for no summaries.  Without want_data the summaries are computed in the simulator and no
+    (batch, n_days, n_toads) tensor is allocated; either way S equals :func:`toad_summaries` of X bit
+    for bit.  Limits: n_days * n_toads <= TOAD_CELLS_MAX; for the summaries n_toads * (n_days - 1)
+    <= TOAD_DISP_MAX, at most TOAD_LAGS_MAX lags and TOAD_NP_MAX levels."""
+    n_toads, n_days = int(n_toads), int(n_days)
+    if n_toads < 1 or n_days < 1 or n_toads * n_days > TOAD_CELLS_MAX:
+        raise ValueError('the device toad simulator takes n_toads >= 1, n_days >= 1 and '
+                         'n_days * n_toads <= {}, got {} * {}'.format(TOAD_CELLS_MAX, n_days,
+                                                                      n_toads))
+    lags = () if lags is None else tuple(lags)
+    if len(lags) > TOAD_LAGS_MAX:
+        raise ValueError('the device toad simulator fuses at most {} lags, got {}'.format(
+            TOAD_LAGS_MAX, len(lags)))
+    lag_arr = pv = None
+    if lags:
+        lag_arr = np.array([_toad_lag(lag, n_days) for lag in lags], dtype=np.int64)
+        _toad_disp(n_toads, n_days - 1)
+        pv = _toad_p(p)
+    P = _matrix(params)
+    if P.shape[1] != 3:
+        raise ValueError('the toad model has 3 parameters (alpha, gamma, p0), got a parameter '
+                         'width of {}'.format(P.shape[1]))
+    B = P.shape[0]
+    X = dev.empty((B, n_days, n_toads)) if want_data else None
+    w = len(lags) * (pv.size + 1) if lags else 0
+    S = dev.empty((B, w)) if lags else None
+    _lib.call('elfi_b200_sim_toad_f64', dev.context(), dev.ptr(P), _ld(P), B, n_toads, n_days,
+              int(seed), int(offset), dev.ptr(X), len(lags), dev.ptr(lag_arr),
+              0 if pv is None else pv.size, dev.ptr(pv), float(thd), dev.ptr(S), w, dev.stream_ptr())
+    return X, S
+
+
+def toad_summaries(x, lag, p=np.linspace(0, 1, 11), thd=10.):
+    """compute_summaries of elfi/examples/toad.py:73-132 for device data x (n_days, n_toads, batch),
+    any strides: a (batch, len(p) + 1) tensor [number of returns, median, len(p) - 1 log gaps], bit
+    for bit NumPy's except that the logs use the device's log.  1 <= lag < n_days, n_toads *
+    (n_days - lag) <= TOAD_DISP_MAX, 1 <= len(p) <= TOAD_NP_MAX levels in [0, 1]."""
+    x = dev.to_device(x) if not (dev.is_device_array(x) and x.dtype == torch.float64) else x
+    if x.dim() != 3:
+        raise ValueError('toad_summaries takes (n_days, n_toads, batch) data, got shape {}'.format(
+            tuple(x.shape)))
+    n_days, n_toads, B = x.shape
+    lag = _toad_lag(lag, n_days)
+    _toad_disp(n_toads, n_days - lag)
+    pv = _toad_p(p)
+    S = dev.empty((B, pv.size + 1))
+    _lib.call('elfi_b200_toad_summaries_f64', dev.context(), dev.ptr(x), x.stride(0), x.stride(1),
+              x.stride(2), n_days, n_toads, B, lag, pv.size, dev.ptr(pv), float(thd), dev.ptr(S),
+              pv.size + 1, dev.stream_ptr())
+    return S

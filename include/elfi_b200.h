@@ -542,6 +542,35 @@ int elfi_b200_lorenz_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t 
                                    int64_t ld_t, int64_t ld_k, int64_t B, int64_t n_timestep,
                                    int64_t n_obs, double* S, int64_t ldS, void* stream);
 
+/* Toad movement model of elfi/examples/toad.py (throughput mode, statistical parity); stream
+ * layout, thread layout and arithmetic in elfi_b200/csrc/toad.cu and toad.cuh.
+ * sim_toad: row i has parameters (alpha, gamma, p0) = P[i * ldP + 0..2] (ldP >= 3).  Every toad
+ *   starts at 0; on day d >= 1 toad k returns (its uniform < p0) to its position of day j, j
+ *   uniform in [0, d), or steps from day d - 1 by gamma times a symmetric alpha-stable variate
+ *   (SciPy's levy_stable, S1, beta = 0).  The draws of (d, k) are a pure function of
+ *   (seed, offset + i, d, k): Philox blocks (c << 1) | 0 and (c << 1) | 1 with c = d * n_toads + k.
+ *   alpha outside (0, 2] or gamma < 0 or NaN (where the reference raises) give a row of NaN.
+ *   n_toads >= 1, n_days >= 1, n_days * n_toads <= 2^31.
+ *   X (B, n_days, n_toads), C-contiguous, may be NULL.  S (B, n_lags * (n_p + 1); ldS) may be NULL;
+ *   it holds toad_summaries of each lag lags[l] (host array, 1 <= lags[l] < n_days, n_lags <= 8) in
+ *   columns l * (n_p + 1) .. and needs n_toads * (n_days - 1) <= 4096 and 1 <= n_p <= 32 (p a host
+ *   array).  With S and without X the row is simulated into shared memory and summarised there;
+ *   with both, X is written and summarised.  Either way S equals toad_summaries of X bit for bit.
+ * toad_summaries: S[i * ldS + 0 .. n_p] = compute_summaries(X, lag, p, thd) (toad.py:73-132) of the
+ *   row X[d * ld_day + k * ld_toad + i * ld_row] (n_days, n_toads): the number of |displacements|
+ *   < thd, the median of the others (NaN dropped) and the n_p - 1 logs of the gaps between their p
+ *   quantiles floored at exp(-20), through nan_to_num(nan=inf); bit for bit NumPy's except for
+ *   the logs, which use the device's log.  1 <= lag < n_days, n_toads * (n_days - lag) <= 4096,
+ *   1 <= n_p <= 32 levels in [0, 1] (host array p). */
+int elfi_b200_sim_toad_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
+                           int64_t n_toads, int64_t n_days, uint64_t seed, uint64_t offset,
+                           double* X, int64_t n_lags, const int64_t* lags, int64_t n_p,
+                           const double* p, double thd, double* S, int64_t ldS, void* stream);
+int elfi_b200_toad_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_day,
+                                 int64_t ld_toad, int64_t ld_row, int64_t n_days, int64_t n_toads,
+                                 int64_t B, int64_t lag, int64_t n_p, const double* p, double thd,
+                                 double* S, int64_t ldS, void* stream);
+
 /* ---- KLIEP density-ratio estimation (AdaptiveThresholdSMC) -------------------------------------
  * DensityRatioEstimation.fit + max_ratio (elfi/methods/density_ratio_estimation.py:71-207):
  * basis centres = first n_basis rows of x, A = RBF(x, centres), b = weighted RBF mean over y,
