@@ -99,6 +99,10 @@ SIGNATURES = {
                                c_ptr, c_i64, c_ptr, c_dbl, c_ptr, c_i64, c_ptr],
     'elfi_b200_toad_summaries_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
                                      c_i64, c_ptr, c_dbl, c_ptr, c_i64, c_ptr],
+    'elfi_b200_sim_lotka_volterra_f64': [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_i64, c_dbl, c_i64,
+                                         c_u64, c_u64, c_ptr, c_ptr, c_ptr],
+    'elfi_b200_lv_summaries_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr, c_i64,
+                                   c_ptr],
     'elfi_b200_prior_rvs_f64': [c_ptr, c_ptr, c_i64, c_u64, c_u64, c_ptr, c_ptr],
     'elfi_b200_prior_logpdf_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     'elfi_b200_gp_padded_size': [c_i64],

@@ -1174,3 +1174,68 @@ def toad_summaries(x, lag, p=np.linspace(0, 1, 11), thd=10.):
               x.stride(2), n_days, n_toads, B, lag, pv.size, dev.ptr(pv), float(thd), dev.ptr(S),
               pv.size + 1, dev.stream_ptr())
     return S
+
+
+# ---- Lotka-Volterra model (elfi/examples/lotka_volterra.py) ----------------------------------------
+LV_NOBS_MAX = 1024            # observation times staged in shared memory
+LV_SUMM_NOBS_MIN = 3          # the lag-2 autocorrelation needs one product
+LV_SUMM_NOBS_MAX = 128        # one leaf of NumPy's pairwise sum
+LV_NSUMM = 9
+LV_MAX_EVENTS_LIMIT = 2 ** 32 - 1   # the event index is one 32-bit Philox word
+
+
+def sim_lotka_volterra(params, n_obs=16, time_end=30., seed=0, offset=0, max_events=2 ** 20):
+    """Lotka-Volterra simulator on the device (elfi/examples/lotka_volterra.py:18-143), Gillespie's
+    direct method per row.  params: (batch, 6) columns r1, r2, r3, prey0, predator0, sigma.  Row i is
+    a pure function of (seed, offset + i).
+
+    Returns (obs, n_events): obs (batch, n_obs, 2) float64 holding the int32 counts of prey and
+    predators at np.linspace(0, time_end, n_obs) (with noise sigma), n_events (batch,) int64 the
+    events each row ran.  A row that has not reached time_end after max_events events, or whose
+    parameters the reference rejects (a negative or NaN rate or sigma, floor(prey0) or
+    floor(predator0) outside [0, 2^31)), gets NaN observations; a capped row reports
+    n_events == max_events.  1 <= n_obs <= LV_NOBS_MAX, time_end finite and > 0,
+    1 <= max_events <= LV_MAX_EVENTS_LIMIT."""
+    n_obs = int(n_obs)
+    if not 1 <= n_obs <= LV_NOBS_MAX:
+        raise ValueError('the device Lotka-Volterra simulator takes 1 <= n_obs <= {}, got {}'.format(
+            LV_NOBS_MAX, n_obs))
+    time_end = float(time_end)
+    if not (np.isfinite(time_end) and time_end > 0):
+        raise ValueError('the device Lotka-Volterra simulator takes a finite time_end > 0, got '
+                         '{}'.format(time_end))
+    if int(max_events) != max_events or not 1 <= max_events <= LV_MAX_EVENTS_LIMIT:
+        raise ValueError('max_events must be an integer with 1 <= max_events <= {} (the event '
+                         'index is one Philox word), got {}'.format(LV_MAX_EVENTS_LIMIT, max_events))
+    P = _matrix(params)
+    if P.shape[1] != 6:
+        raise ValueError('the Lotka-Volterra model has 6 parameters (r1, r2, r3, prey0, predator0, '
+                         'sigma), got a parameter width of {}'.format(P.shape[1]))
+    B = P.shape[0]
+    t_out = dev.to_device(np.linspace(0, time_end, n_obs))
+    obs = dev.empty((B, n_obs, 2))
+    n_events = dev.empty((B,), dtype=torch.int64)
+    _lib.call('elfi_b200_sim_lotka_volterra_f64', dev.context(), dev.ptr(P), _ld(P), B,
+              dev.ptr(t_out), n_obs, time_end, int(max_events), int(seed), int(offset),
+              dev.ptr(obs), dev.ptr(n_events), dev.stream_ptr())
+    return obs, n_events
+
+
+def lv_summaries(x):
+    """The nine summaries of elfi/examples/lotka_volterra.py:206-277 for device data x
+    (batch, n_obs, 2), any strides: a (batch, 9) tensor [prey_mean, pred_mean, prey_log_var,
+    pred_log_var, prey_autocorr_1, pred_autocorr_1, prey_autocorr_2, pred_autocorr_2, crosscorr],
+    bit for bit NumPy's except that log(var + 1) uses the device's log.
+    LV_SUMM_NOBS_MIN <= n_obs <= LV_SUMM_NOBS_MAX."""
+    x = dev.to_device(x) if not (dev.is_device_array(x) and x.dtype == torch.float64) else x
+    if x.dim() != 3 or x.shape[2] != 2:
+        raise ValueError('lv_summaries takes (batch, n_obs, 2) data, got shape {}'.format(
+            tuple(x.shape)))
+    B, n_obs = x.shape[0], x.shape[1]
+    if not LV_SUMM_NOBS_MIN <= n_obs <= LV_SUMM_NOBS_MAX:
+        raise ValueError('the device Lotka-Volterra summaries take {} <= n_obs <= {}, got {}'.format(
+            LV_SUMM_NOBS_MIN, LV_SUMM_NOBS_MAX, n_obs))
+    S = dev.empty((B, LV_NSUMM))
+    _lib.call('elfi_b200_lv_summaries_f64', dev.context(), dev.ptr(x), x.stride(0), x.stride(1),
+              x.stride(2), B, n_obs, dev.ptr(S), LV_NSUMM, dev.stream_ptr())
+    return S

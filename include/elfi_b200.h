@@ -571,6 +571,34 @@ int elfi_b200_toad_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld
                                  int64_t B, int64_t lag, int64_t n_p, const double* p, double thd,
                                  double* S, int64_t ldS, void* stream);
 
+/* Stochastic Lotka-Volterra model of elfi/examples/lotka_volterra.py (throughput mode, statistical
+ * parity); stream layout, lane layout and arithmetic in elfi_b200/csrc/lotka_volterra.cu and
+ * lotka_volterra.cuh.
+ * sim_lotka_volterra: row i has parameters (r1, r2, r3, prey0, predator0, sigma) = P[i * ldP +
+ *   0..5] (ldP >= 6) and starts from (floor(prey0), floor(predator0)); Gillespie's direct method
+ *   runs it to time_end (finite, > 0).  X[i * 2 n_obs + 2 j + s] (B, n_obs, 2) is the count of
+ *   species s (0 prey, 1 predators) at t_out[j] (device array of n_obs <= 1024 times, t_out[0] = 0,
+ *   t_out[n_obs - 1] = time_end; np.linspace), interpolated linearly between the events around it,
+ *   plus sigma times a standard normal for j >= 1, truncated toward zero as int32 (NaN or out of
+ *   range: -2^31).  n_events[i] (int64) is the number of events row i ran.  Event k draws Philox
+ *   block k, observation j block j, of (seed, offset + i): a pure function of the row, whatever
+ *   the launch.  A row still short of time_end after max_events (1 .. 2^32 - 1) events gets NaN
+ *   observations and n_events = max_events; a negative or NaN rate or sigma, initial counts
+ *   outside [0, 2^31) or a negative or NaN total hazard (where the reference raises) give NaN
+ *   observations.  The kernel is persistent: its lanes take new rows as theirs finish.
+ * lv_summaries: S[i * ldS + 0..8] = prey_mean, pred_mean, prey_log_var, pred_log_var,
+ *   prey_autocorr_1, pred_autocorr_1, prey_autocorr_2, pred_autocorr_2, crosscorr
+ *   (lotka_volterra.py:206-277) of the row X[i * ld_row + j * ld_obs + s * ld_species]
+ *   (n_obs, 2), 3 <= n_obs <= 128, ldS >= 9; bit for bit NumPy's except for log(var + 1), which
+ *   uses the device's log. */
+int elfi_b200_sim_lotka_volterra_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
+                                     const double* t_out, int64_t n_obs, double time_end,
+                                     int64_t max_events, uint64_t seed, uint64_t offset,
+                                     double* X, int64_t* n_events, void* stream);
+int elfi_b200_lv_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_row, int64_t ld_obs,
+                               int64_t ld_species, int64_t B, int64_t n_obs, double* S,
+                               int64_t ldS, void* stream);
+
 /* ---- KLIEP density-ratio estimation (AdaptiveThresholdSMC) -------------------------------------
  * DensityRatioEstimation.fit + max_ratio (elfi/methods/density_ratio_estimation.py:71-207):
  * basis centres = first n_basis rows of x, A = RBF(x, centres), b = weighted RBF mean over y,
