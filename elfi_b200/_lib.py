@@ -103,6 +103,12 @@ SIGNATURES = {
                                          c_u64, c_u64, c_ptr, c_ptr, c_ptr],
     'elfi_b200_lv_summaries_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr, c_i64,
                                    c_ptr],
+    'elfi_b200_sim_daycare_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr, c_i64,
+                                  c_dbl, c_u64, c_u64, c_ptr, c_i64, c_ptr, c_ptr, c_ptr],
+    'elfi_b200_daycare_summaries_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
+                                        c_i64, c_i64, c_ptr, c_i64, c_ptr],
+    'elfi_b200_daycare_distance_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_ptr,
+                                       c_ptr, c_ptr],
     'elfi_b200_prior_rvs_f64': [c_ptr, c_ptr, c_i64, c_u64, c_u64, c_ptr, c_ptr],
     'elfi_b200_prior_logpdf_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     'elfi_b200_gp_padded_size': [c_i64],

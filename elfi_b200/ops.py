@@ -1239,3 +1239,127 @@ def lv_summaries(x):
     _lib.call('elfi_b200_lv_summaries_f64', dev.context(), dev.ptr(x), x.stride(0), x.stride(1),
               x.stride(2), B, n_obs, dev.ptr(S), LV_NSUMM, dev.stream_ptr())
     return S
+
+
+# ---- day care model (elfi/examples/daycare.py) ----------------------------------------------------
+DC_DCC_MAX = 32               # one lane per DCC
+DC_IND_MAX = 64               # the numerators of E_s stay within int64
+DC_STRAINS_MAX = 40           # lcm(1 .. n_strains) < 2^53
+DC_SUMM_STRAINS_MAX = 64      # one 64-bit strain mask per child
+DC_NSUMM = 4                  # Shannon, n_strains, prevalence, multi
+DC_DIST_TERMS_MAX = 128       # n_ss * n_dcc of the distance: one leaf of NumPy's pairwise sum
+DC_BATCH_MAX = 2 ** 31 - 1    # one CTA per row
+
+
+def sim_daycare(params, n_dcc=29, n_ind=53, n_strains=33, freq_strains_commun=None, n_obs=36,
+                time_end=10., seed=0, offset=0, want_data=False, want_summaries=True):
+    """Day care simulator on the device (elfi/examples/daycare.py:16-141), Gillespie's direct
+    method in each DCC.  params: (batch, 3) columns t1, t2, t3.  Within a row every DCC takes as
+    many transitions as the DCC that needs most to pass time_end (the reference's law at
+    batch_size=1); row i is a pure function of (seed, offset + i).
+
+    Returns (summaries, data, K): summaries (batch, 4 n_dcc) float64 in column blocks
+    [Shannon | n_strains | prevalence | multi] of the first n_obs children (None unless
+    want_summaries), data (batch, n_dcc, n_obs, n_strains) bool (None unless want_data), K (batch,)
+    int64 the transitions each row took.  A row whose t1, t2 or t3 is negative, NaN or infinite, or
+    whose expected transitions per DCC could reach 2^32 - 1 (time_end n_ind n_strains
+    max(1, max(1, t3) (t1 + 1e-9 + t2 max(freq_strains_commun))) >= 2^32 - 1), gets NaN summaries,
+    all-False data and K = -1.  Limits: n_dcc <= DC_DCC_MAX, 2 <= n_ind <= DC_IND_MAX,
+    n_strains <= DC_STRAINS_MAX, 1 <= n_obs <= n_ind, freq_strains_commun finite and >= 0,
+    time_end finite and > 0."""
+    n_dcc, n_ind, n_strains, n_obs = int(n_dcc), int(n_ind), int(n_strains), int(n_obs)
+    if not (1 <= n_dcc <= DC_DCC_MAX and 2 <= n_ind <= DC_IND_MAX
+            and 1 <= n_strains <= DC_STRAINS_MAX):
+        raise ValueError('the device day care simulator takes 1 <= n_dcc <= {}, 2 <= n_ind <= {} '
+                         'and 1 <= n_strains <= {}, got n_dcc={}, n_ind={}, n_strains={}'.format(
+                             DC_DCC_MAX, DC_IND_MAX, DC_STRAINS_MAX, n_dcc, n_ind, n_strains))
+    if not 1 <= n_obs <= n_ind:
+        raise ValueError('the device day care simulator takes 1 <= n_obs <= n_ind, got n_obs={}, '
+                         'n_ind={}'.format(n_obs, n_ind))
+    time_end = float(time_end)
+    if not (np.isfinite(time_end) and time_end > 0):
+        raise ValueError('the device day care simulator takes a finite time_end > 0, got '
+                         '{}'.format(time_end))
+    if freq_strains_commun is None:
+        freq_strains_commun = np.full(n_strains, 0.1)
+    f = np.asarray(dev.to_host(freq_strains_commun), dtype=np.float64).reshape(-1)
+    if f.size != n_strains:
+        raise ValueError('freq_strains_commun must have n_strains = {} values, got {}'.format(
+            n_strains, f.size))
+    if not (np.all(np.isfinite(f)) and np.all(f >= 0)):
+        raise ValueError('freq_strains_commun must be finite and >= 0, got {}'.format(f))
+    P = _matrix(params)
+    if P.shape[1] != 3:
+        raise ValueError('the day care model has 3 parameters (t1, t2, t3), got a parameter width '
+                         'of {}'.format(P.shape[1]))
+    B = P.shape[0]
+    if B > DC_BATCH_MAX:
+        raise ValueError('the device day care simulator takes at most {} rows per call, got '
+                         '{}'.format(DC_BATCH_MAX, B))
+    S = dev.empty((B, DC_NSUMM * n_dcc)) if want_summaries else None
+    X = dev.empty((B, n_dcc, n_obs, n_strains), dtype=torch.bool) if want_data else None
+    K = dev.empty((B,), dtype=torch.int64)
+    fd = dev.to_device(f)
+    _lib.call('elfi_b200_sim_daycare_f64', dev.context(), dev.ptr(P), _ld(P), B, n_dcc, n_ind,
+              n_strains, dev.ptr(fd), n_obs, time_end, int(seed), int(offset), dev.ptr(S),
+              DC_NSUMM * n_dcc, dev.ptr(X), dev.ptr(K), dev.stream_ptr())
+    return S, X, K
+
+
+def daycare_summaries(data):
+    """The four summaries of elfi/examples/daycare.py:199-275 for device data (batch, n_dcc, n_obs,
+    n_strains), any strides, nonzero meaning a carrier: a (batch, 4 n_dcc) tensor in column blocks
+    [Shannon | n_strains | prevalence | multi], bit for bit NumPy's except that Shannon uses the
+    device's log.  n_strains <= DC_SUMM_STRAINS_MAX."""
+    if not dev.is_device_array(data):
+        data = dev.to_device(np.asarray(data, dtype=np.float64))
+    if data.dtype not in (torch.bool, torch.uint8):
+        data = data != 0
+    if data.dim() != 4:
+        raise ValueError('daycare_summaries takes (batch, n_dcc, n_obs, n_strains) data, got shape '
+                         '{}'.format(tuple(data.shape)))
+    B, n_dcc, n_obs, n_strains = (int(v) for v in data.shape)
+    if n_dcc < 1 or n_obs < 1 or not 1 <= n_strains <= DC_SUMM_STRAINS_MAX:
+        raise ValueError('the device day care summaries take n_dcc, n_obs >= 1 and 1 <= n_strains '
+                         '<= {}, got shape {}'.format(DC_SUMM_STRAINS_MAX, tuple(data.shape)))
+    S = dev.empty((B, DC_NSUMM * n_dcc))
+    _lib.call('elfi_b200_daycare_summaries_f64', dev.context(), dev.ptr(data), data.stride(0),
+              data.stride(1), data.stride(2), data.stride(3), B, n_dcc, n_obs, n_strains,
+              dev.ptr(S), DC_NSUMM * n_dcc, dev.stream_ptr())
+    return S
+
+
+def daycare_observed(observed):
+    """The observed side of daycare_distance from the k (1, n_dcc) observed summaries, on the host:
+    (obs_max (k,), y (k, n_dcc)) with obs_max the per-summary maximum (0 replaced by 1) and y the
+    observed values divided by it and sorted (elfi/examples/daycare.py:296-306)."""
+    observed = np.stack([np.asarray(dev.to_host(o), dtype=np.float64) for o in observed])
+    obs_max = np.max(observed, axis=2, keepdims=True)
+    obs_max = np.where(obs_max == 0, 1, obs_max)
+    y = np.sort(observed / obs_max, axis=2)
+    return obs_max.reshape(-1), y.reshape(len(observed), -1)
+
+
+def daycare_distance(S, observed, n_dcc):
+    """The distance of elfi/examples/daycare.py:278-312 on the device: S (batch, k n_dcc) holds the
+    k simulated summaries side by side, observed the k (1, n_dcc) observed ones.  Each row is
+    divided by the observed maxima, sorted per summary (NaN last), and its mean absolute difference
+    from the sorted observed values is taken, bit for bit as NumPy does (one pairwise sum for a
+    batch of one row, else one per summary, added in order).  k n_dcc <= DC_DIST_TERMS_MAX."""
+    S = _matrix(S)
+    n_dcc = int(n_dcc)
+    k = len(observed)
+    if S.shape[1] != k * n_dcc or not 1 <= k * n_dcc <= DC_DIST_TERMS_MAX:
+        raise ValueError('daycare_distance takes {} summaries of n_dcc = {} columns, at most {} '
+                         'values per row; got a width of {}'.format(k, n_dcc, DC_DIST_TERMS_MAX,
+                                                                    S.shape[1]))
+    obs_max, y = daycare_observed(observed)
+    if y.shape[1] != n_dcc:
+        raise ValueError('the observed summaries have {} DCCs, the simulated ones {}'.format(
+            y.shape[1], n_dcc))
+    om, yd = dev.to_device(obs_max), dev.to_device(y)
+    B = S.shape[0]
+    d = dev.empty((B,))
+    _lib.call('elfi_b200_daycare_distance_f64', dev.context(), dev.ptr(S), _ld(S), B, k, n_dcc,
+              dev.ptr(om), dev.ptr(yd), dev.ptr(d), dev.stream_ptr())
+    return d

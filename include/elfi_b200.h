@@ -599,6 +599,39 @@ int elfi_b200_lv_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_r
                                int64_t ld_species, int64_t B, int64_t n_obs, double* S,
                                int64_t ldS, void* stream);
 
+/* Day care model of elfi/examples/daycare.py (throughput mode, statistical parity); law, stream
+ * layout, lane layout and arithmetic in elfi_b200/csrc/daycare.cu and daycare.cuh.
+ * sim_daycare: row i has parameters (t1, t2, t3) = P[i * ldP + 0..2] (ldP >= 3); each of its n_dcc
+ *   (<= 32) DCCs of n_ind (2 .. 64) children and n_strains (<= 40) strains, community
+ *   frequencies freq (device, n_strains), runs Gillespie's direct method, and every DCC of the row
+ *   takes as many transitions K[i] (int64) as the one that needs most to pass time_end (finite,
+ *   > 0).  Transition k of DCC c draws Philox block k of (seed, offset + i) salted with c: a pure
+ *   function of the row, whatever the launch.  S (or NULL; ldS >= 4 n_dcc) gets the summaries
+ *   S[i * ldS + j * n_dcc + c], j = Shannon, n_strains, prevalence, multi, of the first n_obs
+ *   (1 .. n_ind) children; X (or NULL) gets their states X[((i * n_dcc + c) * n_obs + o) *
+ *   n_strains + s] as 0 / 1.  t1, t2 or t3 negative, NaN or infinite, time_end n_ind n_strains
+ *   max(1, max(1, t3) (t1 + 1e-9 + t2 max(freq))) >= 2^32 - 1, or freq negative or not finite:
+ *   NaN summaries, zero data, K = -1.  B < 2^31 (one CTA per row).
+ * daycare_summaries: S[i * ldS + j * n_dcc + c] as above from X[i * ld_b + c * ld_c + o * ld_i +
+ *   s * ld_s] (uint8, nonzero = carrier; n_strains <= 64); bit for bit NumPy's except for the log
+ *   in Shannon, which uses the device's log.
+ * daycare_distance: d[i] (daycare.py:278-312) of the n_ss summaries S[i * ldS + k * n_dcc + c]
+ *   (n_ss * n_dcc <= 128) against the observed maxima obs_max (n_ss, 0 replaced by 1) and the
+ *   sorted observed values divided by them y (n_ss, n_dcc), both device; bit for bit NumPy's,
+ *   including its summation order for B == 1 and B > 1. */
+int elfi_b200_sim_daycare_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
+                              int64_t n_dcc, int64_t n_ind, int64_t n_strains,
+                              const double* freq, int64_t n_obs, double time_end, uint64_t seed,
+                              uint64_t offset, double* S, int64_t ldS, uint8_t* X, int64_t* K,
+                              void* stream);
+int elfi_b200_daycare_summaries_f64(elfi_b200_ctx* ctx, const uint8_t* X, int64_t ld_b,
+                                    int64_t ld_c, int64_t ld_i, int64_t ld_s, int64_t B,
+                                    int64_t n_dcc, int64_t n_obs, int64_t n_strains, double* S,
+                                    int64_t ldS, void* stream);
+int elfi_b200_daycare_distance_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
+                                   int64_t n_ss, int64_t n_dcc, const double* obs_max,
+                                   const double* y, double* d, void* stream);
+
 /* ---- KLIEP density-ratio estimation (AdaptiveThresholdSMC) -------------------------------------
  * DensityRatioEstimation.fit + max_ratio (elfi/methods/density_ratio_estimation.py:71-207):
  * basis centres = first n_basis rows of x, A = RBF(x, centres), b = weighted RBF mean over y,
