@@ -15,6 +15,7 @@
 #include <cstdlib>
 
 #include "common.cuh"
+#include "gmterm.cuh"
 
 namespace elfi {
 
@@ -66,24 +67,28 @@ __global__ void colmoments_final_kernel(const double* __restrict__ S, const doub
 }
 
 // ---------------------------------------------------------------------------------------------
-// K8: weighted statistics.  pass 0: V1 = sum w, V2 = sum w^2, xw_j = sum w x_j.
-//     pass 1: num_j = sum w (x_j - xbar_j)^2.   p <= 16.
+// K8: weighted statistics.  pass 0: V1 = sum w, V2 = sum w^2, xw_j = sum w x_j, and the number
+//     of nonzero weights.  pass 1: num_j = sum w (x_j - xbar_j)^2.   p <= 16.
+// Partial row layout: [V1, V2, xw_0 .. xw_15 | num_0 .. num_15, nonzero count].
 constexpr int WS_MAXP = 16;
+constexpr int WS_NZ = WS_MAXP + 2;       // slot of the nonzero-weight count
+constexpr int WS_ROW = WS_MAXP + 3;
 
 __global__ void __launch_bounds__(256)
 wstats_partial_kernel(const double* __restrict__ x, int64_t ld, const double* __restrict__ w,
                       int64_t N, int p, int pass, const double* __restrict__ stats,
                       double* __restrict__ partial) {
-    __shared__ double red[8][WS_MAXP + 2];
-    double acc[WS_MAXP + 2];
+    __shared__ double red[8][WS_ROW];
+    double acc[WS_ROW];
 #pragma unroll
-    for (int k = 0; k < WS_MAXP + 2; ++k) acc[k] = 0.0;
+    for (int k = 0; k < WS_ROW; ++k) acc[k] = 0.0;
     const int64_t stride = int64_t(gridDim.x) * blockDim.x;
     for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < N; i += stride) {
         const double wi = w ? w[i] : 1.0;
         if (pass == 0) {
             acc[0] += wi;
             acc[1] = fma(wi, wi, acc[1]);
+            acc[WS_NZ] += (wi != 0.0) ? 1.0 : 0.0;
 #pragma unroll
             for (int j = 0; j < WS_MAXP; ++j)
                 if (j < p) acc[2 + j] = fma(wi, x[i * ld + j], acc[2 + j]);
@@ -98,33 +103,43 @@ wstats_partial_kernel(const double* __restrict__ x, int64_t ld, const double* __
     }
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 #pragma unroll
-    for (int k = 0; k < WS_MAXP + 2; ++k) {
+    for (int k = 0; k < WS_ROW; ++k) {
         double v = acc[k];
         for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
         if (lane == 0) red[wid][k] = v;
     }
     __syncthreads();
-    if (threadIdx.x < p + 2) {
+    const int k = threadIdx.x;
+    if (k < p + 2 || (pass == 0 && k == WS_NZ)) {
         double v = 0.0;
-        for (int k = 0; k < 8; ++k) v += red[k][threadIdx.x];
-        partial[int64_t(blockIdx.x) * (WS_MAXP + 2) + threadIdx.x] = v;
+        for (int b = 0; b < 8; ++b) v += red[b][k];
+        partial[int64_t(blockIdx.x) * WS_ROW + k] = v;
     }
 }
 
-// stats layout: [V1, V2, xbar_0..p-1, s2_0..p-1]
+// stats layout: [V1, V2, xbar_0..p-1, s2_0..p-1]; one warp.  Every thread reaches the barrier:
+// the body is guarded rather than left early.  The partial sums of the nonzero-weight count
+// (slot WS_NZ) are written by pass 0 and still in place in pass 1.
 __global__ void wstats_final_kernel(const double* __restrict__ partial, int nblocks, int p, int pass,
                                     double* __restrict__ stats) {
     const int k = threadIdx.x;
-    if (k >= p + 2) return;
+    const bool active = k < p + 2;
     double v = 0.0;
-    for (int b = 0; b < nblocks; ++b) v += partial[int64_t(b) * (WS_MAXP + 2) + k];
+    if (active)
+        for (int b = 0; b < nblocks; ++b) v += partial[int64_t(b) * WS_ROW + k];
     if (pass == 0) {
-        if (k < 2) stats[k] = v;
+        if (active && k < 2) stats[k] = v;
         __syncthreads();
-        if (k >= 2) stats[k] = v / stats[0];                 // np.average: sum(w x) / sum(w)
-    } else if (k >= 2) {
+        if (active && k >= 2) stats[k] = v / stats[0];       // np.average: sum(w x) / sum(w)
+    } else if (active && k >= 2) {
         const double V1 = stats[0], V2 = stats[1];
-        stats[p + k] = v / (V1 - (V2 / V1));                 // utils.py:138
+        double nz = 0.0;
+        for (int b = 0; b < nblocks; ++b) nz += partial[int64_t(b) * WS_ROW + WS_NZ];
+        // utils.py:138.  With fewer than two nonzero weights V1 - V2 / V1 is exactly zero, but
+        // the rounded w^2 / w can miss w by an ulp; the zero keeps s2 non-finite there, which is
+        // what SMC's fallback to the unit covariance tests for.
+        const double denom = nz > 1.0 ? V1 - (V2 / V1) : 0.0;
+        stats[p + k] = v / denom;
     }
 }
 
@@ -138,37 +153,20 @@ __global__ void wstats_final_kernel(const double* __restrict__ partial, int nblo
 // log2 w_j), per point it keeps (y_i, |y_i|^2), and a pair costs P DFMA + 1 DADD instead of P DSUB
 // + P DFMA + the weight multiply.  The cancellation error is |y|^2 * 2^-52 ~ 1e-14 ABSOLUTE in nt,
 // i.e. 1e-14 relative in the term (what matters for a density), thanks to the centring.
-// 2^(-nt): k = rint(-nt) through the 2^52 trick (no 64-bit conversions, which run on the slow
-// XU pipe), f = -nt - k in [-.5, .5], 2^f by the degree-6 minimax polynomial (relative error
-// < 1.9e-9, Remez on [-.5, .5]), scaled by 2^k through the exponent field; nt > 1020 flushes to 0
-// (and so does a zero weight, whose c_j is +inf).
+// 2^(-nt) is exp2_neg of gmterm.cuh (range reduction and a degree-6 minimax polynomial, relative
+// error < 1.9e-9; nt > 1020 flushes to 0, and so does a zero weight, whose c_j is +inf).
 // fp64-pipe instructions per pair: P + 1 (distance) + 3 (range reduction) + 6 (polynomial)
 // + 1 (compare) + 1 (accumulate) = P + 12  (round 1: 2P + 12).
-__device__ __forceinline__ double exp2_neg(double nt) {
-    const double magic = 6755399441055744.0;  // 1.5 * 2^52
-    const double tm = magic - nt;
-    const double kd = tm - magic;             // rint(-nt)
-    const double f = -nt - kd;
-    double pz = 1.5345812158740182e-04;
-    pz = fma(pz, f, 1.3399931209474140e-03);
-    pz = fma(pz, f, 9.6184889565227916e-03);
-    pz = fma(pz, f, 5.5503287769976638e-02);
-    pz = fma(pz, f, 2.4022646890639572e-01);
-    pz = fma(pz, f, 6.9314720573725268e-01);
-    pz = fma(pz, f, 1.0000000005541663e+00);
-    const int k = __double2loint(tm);         // low word of (magic - nt) holds rint(-nt)
-    const int hi = __double2hiint(pz) + (k << 20);
-    const double r = __hiloint2double(hi, __double2loint(pz));
-    return (nt <= 1020.0) ? r : 0.0;
-}
-
-// Mixed-precision variant of exp2_neg (opt-in, ELFI_B200_GM_MODE=mixed): the range reduction
-// stays in fp64 (the integer / fraction split of nt needs it), but 2^f for f in [-.5, .5] comes
-// from the special-function unit in fp32 (ex2.approx: 2 ulp, ~1.7e-7 relative) and is widened
-// back to fp64 with integer operations while the exponent k is added -- no polynomial: the
-// fp64 pipe issues 8 instructions per pair at P = 2 instead of 14, the rest runs on the
-// XU (F2F + MUFU) and integer pipes concurrently.  Accuracy ~2e-7 per term against the 1e-5
-// relative tolerance on the weights; the fp64 path (1.9e-9) stays the default.
+//
+// Mixed-precision variant of exp2_neg (the ops.gm_logpdf(mixed=True) entry point): the range
+// reduction stays in fp64 (the integer / fraction split of nt needs it), but 2^f for f in
+// [-.5, .5] comes from the special-function unit in fp32 and is widened back to fp64 with integer
+// operations while the exponent k is added -- no polynomial: the fp64 pipe issues 8 instructions
+// per pair at P = 2 instead of 14, the rest runs on the XU (F2F + MUFU) and integer pipes
+// concurrently.  Term error: ex2.approx.f32 is within 2 ulp of 2^f, which is 2^-22 = 2.4e-7
+// relative just above 1.0, plus the fp32 rounding of f (<= 2^-26 absolute, 1.0e-8 relative in
+// 2^f): <= 2.5e-7 against the 1e-5 relative tolerance on the weights.  The fp64 path (1.9e-9)
+// stays the default.
 __device__ __forceinline__ double exp2_neg_mixed(double nt) {
     const double magic = 6755399441055744.0;  // 1.5 * 2^52
     const double tm = magic - nt;
@@ -337,7 +335,7 @@ int elfi_b200_weighted_stats_f64(elfi_b200_ctx* ctx, const double* x, int64_t ld
     ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     int blocks = int((N + 255) / 256);
     if (blocks > ctx->sm_count * 4) blocks = ctx->sm_count * 4;
-    double* partial = static_cast<double*>(ctx_scratch(ctx, size_t(blocks) * (WS_MAXP + 2) * 8 + 256));
+    double* partial = static_cast<double*>(ctx_scratch(ctx, size_t(blocks) * WS_ROW * 8 + 256));
     if (!partial) return ELFI_B200_ERR_NOMEM;
     for (int pass = 0; pass < 2; ++pass) {
         wstats_partial_kernel<<<blocks, 256, 0, stream>>>(x, ldx, w, N, int(p), pass, stats, partial);
@@ -352,7 +350,8 @@ static int gm_logpdf_impl(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int6
                           const double* Linv_host, double logdet, double* logq, void* stream_,
                           bool mixed_entry) {
     using namespace elfi;
-    ELFI_REQUIRE(ctx && x && means && Linv_host && logq, "gm_logpdf: NULL argument");
+    // an empty batch has no x or logq storage (an empty tensor's data pointer is NULL)
+    ELFI_REQUIRE(ctx && (N == 0 || (x && logq)) && means && Linv_host, "gm_logpdf: NULL argument");
     ELFI_REQUIRE(N >= 0 && M >= 1 && p >= 1 && p <= WS_MAXP && ldx >= p && ldm >= p,
                  "gm_logpdf: bad shape (p <= %d)", WS_MAXP);
     if (N == 0) return ELFI_B200_OK;

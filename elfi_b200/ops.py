@@ -501,7 +501,7 @@ def gm_logpdf(x, means, cov=1, weights=None, validate=True, mixed=False):
     x (N, p) and means (M, p) may be host or device arrays; returns a device tensor (N,).
     ``validate=False`` skips the two synchronising weight checks of normalize_weights
     (utils.py:80-88) for weights the caller produced itself.  ``mixed=True`` takes 2^f from the
-    fp32 special-function unit (term error <= 2e-7 instead of 2e-9, fewer fp64 instructions
+    fp32 special-function unit (term error <= 2.5e-7 instead of 1.9e-9, fewer fp64 instructions
     per term): the throughput
     mode's choice, where parity with the reference is statistical."""
     means = _matrix(means)

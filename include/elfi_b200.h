@@ -261,6 +261,9 @@ int elfi_b200_wquantile_f64(elfi_b200_ctx* ctx, const double* x, const double* w
  * elfi_b200_weighted_stats_f64: weighted_var and its ingredients (elfi/methods/utils.py:108-139):
  *   stats = [V1 = sum w, V2 = sum w^2, xbar_0..p-1 = np.average(x, weights=w),
  *            s2_0..p-1 = sum w (x - xbar)^2 / (V1 - V2/V1)],   w == NULL means all ones.
+ *   With fewer than two nonzero weights (N = 1 included) the denominator is exactly zero and s2
+ *   is non-finite (SMC then falls back to the unit covariance), even where the rounded
+ *   V2 / V1 would miss V1 by an ulp.
  *
  * elfi_b200_gm_logpdf_f64: GMDistribution.logpdf (elfi/methods/utils.py:146-197) --
  *   logq[i] = log sum_j (w_j / sum w) N(x_i; means_j, Sigma), plain sum of densities as in the
@@ -270,8 +273,12 @@ int elfi_b200_wquantile_f64(elfi_b200_ctx* ctx, const double* x, const double* w
  *   term error 1.9e-9; fp64 accumulation).
  * elfi_b200_gm_logpdf_mixed_f64: the same density with 2^f taken from the special-function unit in
  *   fp32 (range reduction and accumulation stay fp64): fewer fp64 instructions per term, term
- *   error <= 2e-7 -- used where parity with the reference is
- *   statistical anyway (throughput mode: device RNG), 50x inside the 1e-5 tolerance on SMC weights.
+ *   error <= 2.5e-7 (ex2.approx.f32's 2 ulp, 2^-22 relative just above 1.0, plus the fp32
+ *   rounding of the fraction, ln 2 * 2^-26) -- used where parity with the reference is
+ *   statistical anyway (throughput mode: device RNG), 40x inside the 1e-5 tolerance on SMC weights.
+ *   Both: terms (w_j / sum w) exp(-maha_ij / 2) below 2^-1020 are flushed to zero, and logq[i]
+ *   = -inf where all of them are; the reference underflows only below 2^-1074, with the
+ *   normaliser inside the exp, so in a narrow band of far-out points the two differ.
  *
  * elfi_b200_smc_weights_f64: w_i = exp(logprior_i - logq_i) (samplers.py:514).
  */

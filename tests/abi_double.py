@@ -275,6 +275,7 @@ def colmoments_f64(ctx, S, ldS, B, D, out, stream):
 
 
 def weighted_stats_f64(ctx, x, ldx, w, N, p, stats, stream):
+    _require(N >= 1 and 1 <= p <= 16 and ldx >= p, 'weighted_stats: bad shape (p <= 16)')
     x = np.ascontiguousarray(_mat(x, N, p, ldx))
     w = np.ones(N) if not _addr(w) else _vec(w, N).copy()
     s = _vec(stats, 2 + 2 * p)
@@ -283,15 +284,31 @@ def weighted_stats_f64(ctx, x, ldx, w, N, p, stats, stream):
     with np.errstate(all='ignore'):
         s[2:2 + p] = np.average(x, weights=w, axis=0)
         s[2 + p:] = o.weighted_var(x, w)
+        if np.count_nonzero(w) < 2:        # the header: V1 - V2 / V1 is exactly zero there
+            s[2 + p:] = (w @ (x - s[2:2 + p]) ** 2) / 0.0
 
 
 def gm_logpdf_f64(ctx, x, ldx, N, means, ldm, w, M, p, Linv_host, logdet, logq, stream):
+    _require(N >= 0 and M >= 1 and 1 <= p <= 16 and ldx >= p and ldm >= p,
+             'gm_logpdf: bad shape (p <= 16)')
+    if N == 0:
+        return
+    # the oracle's density (SciPy's exp(lognorm - maha / 2), summed as plain densities), but
+    # whitened with the Linv and logdet the caller passes, as the device does, and summed per
+    # point so that a point's value does not depend on the rest of the batch
     x = np.ascontiguousarray(_mat(x, N, p, ldx))
     means = np.ascontiguousarray(_mat(means, M, p, ldm))
-    Linv = _mat(Linv_host, p, p)
-    L = np.linalg.inv(Linv)
-    weights = None if not _addr(w) else _vec(w, M).copy()
-    _vec(logq, N)[:] = o.gm_logpdf(x, means, L @ L.T, weights)
+    Linv = np.array(_mat(Linv_host, p, p))
+    weights = np.full(M, 1.0 / M) if not _addr(w) else _vec(w, M) / np.sum(_vec(w, M))
+    lognorm = -0.5 * (p * np.log(2 * np.pi) + logdet)
+    out = _vec(logq, N)
+    b = max(1, (1 << 20) // M)
+    for lo in range(0, N, b):
+        z = (x[lo:lo + b, None, :] - means[None, :, :]) @ Linv.T
+        with np.errstate(under='ignore'):
+            dens = np.exp(lognorm - 0.5 * np.einsum('ijk,ijk->ij', z, z))
+        with np.errstate(divide='ignore'):
+            out[lo:lo + b] = np.log(np.sum(dens * weights, axis=1))
 
 
 def gm_logpdf_mixed_f64(*args):
