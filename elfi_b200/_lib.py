@@ -109,6 +109,10 @@ SIGNATURES = {
                                         c_i64, c_i64, c_ptr, c_i64, c_ptr],
     'elfi_b200_daycare_distance_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_ptr,
                                        c_ptr, c_ptr],
+    'elfi_b200_sim_arch_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_u64, c_u64, c_ptr, c_i64,
+                               c_ptr, c_i64, c_ptr],
+    'elfi_b200_arch_summaries_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr, c_i64,
+                                     c_ptr],
     'elfi_b200_prior_rvs_f64': [c_ptr, c_ptr, c_i64, c_u64, c_u64, c_ptr, c_ptr],
     'elfi_b200_prior_logpdf_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     'elfi_b200_gp_padded_size': [c_i64],

@@ -1363,3 +1363,63 @@ def daycare_distance(S, observed, n_dcc):
     _lib.call('elfi_b200_daycare_distance_f64', dev.context(), dev.ptr(S), _ld(S), B, k, n_dcc,
               dev.ptr(om), dev.ptr(yd), dev.ptr(d), dev.stream_ptr())
     return d
+
+
+# ---- ARCH(1) model (elfi/examples/arch.py) --------------------------------------------------------
+ARCH_NOBS_MIN, ARCH_NOBS_MAX = 2, 128   # one leaf of NumPy's pairwise sum per reduction
+ARCH_LAGS_MAX = 8
+
+
+def arch_nsumm(n_lags):
+    """The number of ARCH summaries for n_lags lags: MU, VAR, the n_lags AC and their pairwise
+    products."""
+    return 2 + n_lags + n_lags * (n_lags - 1) // 2
+
+
+def _arch_shape(n_obs, n_lags, what):
+    if int(n_obs) != n_obs or not ARCH_NOBS_MIN <= n_obs <= ARCH_NOBS_MAX:
+        raise ValueError('{} take {} <= n_obs <= {}, got {}'.format(what, ARCH_NOBS_MIN,
+                                                                    ARCH_NOBS_MAX, n_obs))
+    top = min(ARCH_LAGS_MAX, int(n_obs) - 1)
+    if int(n_lags) != n_lags or not 1 <= n_lags <= top:
+        raise ValueError('{} take 1 <= n_lags <= min({}, n_obs - 1) = {}, got {}'.format(
+            what, ARCH_LAGS_MAX, top, n_lags))
+    return int(n_obs), int(n_lags)
+
+
+def sim_arch(params, n_obs=100, n_lags=5, seed=0, offset=0, want_data=False, want_summaries=True):
+    """ARCH(1) simulator on the device (elfi/examples/arch.py:65-132).  params: (batch, 2) columns
+    t1, t2.  Row i is a pure function of (seed, offset + i).
+
+    Returns (Y, S), each None unless asked for: Y (batch, n_obs) the series y_1 .. y_n, S (batch,
+    arch_nsumm(n_lags)) its summaries [MU, VAR, AC_1 .. AC_L, PW in itertools.combinations order],
+    computed in the simulator without writing Y, bit for bit :func:`arch_summaries` of Y."""
+    n_obs, n_lags = _arch_shape(n_obs, n_lags, 'the device ARCH simulator and its summaries')
+    P = _matrix(params)
+    if P.shape[1] != 2:
+        raise ValueError('the ARCH model has 2 parameters (t1, t2), got a parameter width of {}'
+                         .format(P.shape[1]))
+    B = P.shape[0]
+    K = arch_nsumm(n_lags)
+    Y = dev.empty((B, n_obs)) if want_data else None
+    S = dev.empty((B, K)) if want_summaries else None
+    _lib.call('elfi_b200_sim_arch_f64', dev.context(), dev.ptr(P), _ld(P), B, n_obs, n_lags,
+              int(seed), int(offset), dev.ptr(Y), n_obs, dev.ptr(S), K, dev.stream_ptr())
+    return Y, S
+
+
+def arch_summaries(y, n_lags=5):
+    """The ARCH summaries of elfi/examples/arch.py:135-208 for each row of device data y (batch, n),
+    any strides (the reference's y[:, 1:] view included): a (batch, arch_nsumm(n_lags)) tensor
+    [MU, VAR, AC_1 .. AC_L, PW_i_j in itertools.combinations order], bit for bit NumPy's."""
+    if not (dev.is_device_array(y) and y.dtype == torch.float64):
+        y = dev.to_device(y)
+    if y.dim() != 2:
+        raise ValueError('arch_summaries takes (batch, n) data, got shape {}'.format(tuple(y.shape)))
+    B = int(y.shape[0])
+    n, n_lags = _arch_shape(int(y.shape[1]), n_lags, 'the device ARCH summaries')
+    K = arch_nsumm(n_lags)
+    S = dev.empty((B, K))
+    _lib.call('elfi_b200_arch_summaries_f64', dev.context(), dev.ptr(y), y.stride(0), y.stride(1),
+              B, n, n_lags, dev.ptr(S), K, dev.stream_ptr())
+    return S

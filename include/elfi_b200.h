@@ -639,6 +639,23 @@ int elfi_b200_daycare_distance_f64(elfi_b200_ctx* ctx, const double* S, int64_t 
                                    int64_t n_ss, int64_t n_dcc, const double* obs_max,
                                    const double* y, double* d, void* stream);
 
+/* ARCH(1) model of elfi/examples/arch.py (throughput mode, statistical parity); stream layout,
+ * thread layout and arithmetic in elfi_b200/csrc/arch.cu and arch.cuh.
+ * Both take 2 <= n_obs (n) <= 128 and 1 <= n_lags <= min(8, n - 1); the summaries are
+ * S[i * ldS + k], k < 2 + L + L(L-1)/2 (ldS at least that): MU, VAR (ddof = 1), AC_1 .. AC_L, then
+ * PW_i_j = AC_i * AC_j in itertools.combinations order, bit for bit NumPy's.
+ * sim_arch: row i has parameters (t1, t2) = P[i * ldP + 0..1] (ldP >= 2) and observations
+ *   Y[i * ldY + 0 .. n_obs - 1] (y_1 .. y_n of the reference).  Block m of (seed, offset + i) gives
+ *   the normals z_{2m}, z_{2m+1}, z_0 = e_0, z_k = xi_k: a pure function of the row, whatever the
+ *   launch.  Y and S may each be NULL; S is computed from the row without writing Y.
+ * arch_summaries: the summaries of the row X[i * ld_b + j * ld_j], j < n, any strides. */
+int elfi_b200_sim_arch_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
+                           int64_t n_obs, int64_t n_lags, uint64_t seed, uint64_t offset,
+                           double* Y, int64_t ldY, double* S, int64_t ldS, void* stream);
+int elfi_b200_arch_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_b, int64_t ld_j,
+                                 int64_t B, int64_t n, int64_t n_lags, double* S, int64_t ldS,
+                                 void* stream);
+
 /* ---- KLIEP density-ratio estimation (AdaptiveThresholdSMC) -------------------------------------
  * DensityRatioEstimation.fit + max_ratio (elfi/methods/density_ratio_estimation.py:71-207):
  * basis centres = first n_basis rows of x, A = RBF(x, centres), b = weighted RBF mean over y,
