@@ -68,6 +68,12 @@ __device__ __forceinline__ uint64_t shfl_xor_u64(uint64_t v, int m) {
     return (uint64_t(hi) << 32) | lo;
 }
 
+__device__ __forceinline__ uint64_t shfl_u64(uint64_t v, int src) {
+    const uint32_t lo = __shfl_sync(0xffffffffu, uint32_t(v), src);
+    const uint32_t hi = __shfl_sync(0xffffffffu, uint32_t(v >> 32), src);
+    return (uint64_t(hi) << 32) | lo;
+}
+
 template <int KPL>
 __device__ __forceinline__ void bitonic_in_registers(uint64_t (&key)[KPL], int lane) {
     constexpr int N = KPL * 32;
@@ -99,6 +105,30 @@ __device__ __forceinline__ void bitonic_in_registers(uint64_t (&key)[KPL], int l
             }
         }
     }
+}
+
+// sorted key i of a register-resident series after bitonic_in_registers (all lanes call it; i is
+// warp-uniform)
+template <int KPL>
+__device__ __forceinline__ uint64_t pick_reg(const uint64_t (&key)[KPL], int i) {
+    const int r = i % KPL;
+    uint64_t v = key[0];
+#pragma unroll
+    for (int s = 1; s < KPL; ++s)
+        if (r == s) v = key[s];
+    return __shfl_sync(0xffffffffu, v, i / KPL);
+}
+
+// sorted key i of a register-resident series, where i may differ between lanes: KPL shuffles
+template <int KPL>
+__device__ __forceinline__ uint64_t pick_reg_lane(const uint64_t (&key)[KPL], int i) {
+    uint64_t v = 0;
+#pragma unroll
+    for (int s = 0; s < KPL; ++s) {
+        const uint64_t o = shfl_u64(key[s], i / KPL);
+        if (i % KPL == s) v = o;
+    }
+    return v;
 }
 
 }  // namespace elfi

@@ -25,17 +25,6 @@ constexpr uint32_t SALT_SIM_BIGNK = 0x42474e4bu;   // one block per (row, observ
 constexpr int GNK_REGS_MAX = 512;                  // 32 lanes x 16 keys
 constexpr int GNK_SERIES_MAX = 2048;
 
-// sorted key i of a register-resident series (all lanes call it; i is warp-uniform)
-template <int KPL>
-__device__ __forceinline__ uint64_t pick_reg(const uint64_t (&key)[KPL], int i) {
-    const int r = i % KPL;
-    uint64_t v = key[0];
-#pragma unroll
-    for (int s = 1; s < KPL; ++s)
-        if (r == s) v = key[s];
-    return __shfl_sync(0xffffffffu, v, i / KPL);
-}
-
 // sort one series held in registers, then lane 0 writes its summary to out[j * step]
 template <int KPL>
 __device__ __forceinline__ void summarize_regs(uint64_t (&key)[KPL], int lane, int n, int kind,

@@ -17,6 +17,9 @@
 //   beta       X = G(a) of component 0, Y = G(b) of component 1;  loc + scale X / (X + Y)
 // At most PRIOR_MAX_TRIALS = 64 trials per component (include/elfi_b200.h says what the bound
 // returns; for every valid shape a trial is rejected with probability below 0.05).
+// The draw is fma(scale, y, loc) (loc + scale y, one rounding) with the table's loc and scale, or
+// per row with loc[i] / scale[i] when those vectors are given (a conditional prior): y and its
+// stream do not depend on them.  A per-row scale < 0 or NaN gives NaN (priors.cuh).
 #include "boxmuller.cuh"
 #include "common.cuh"
 #include "philox.cuh"
@@ -49,6 +52,7 @@ __device__ __forceinline__ double gamma_component(const Philox& ph, uint32_t r0,
 
 __global__ void __launch_bounds__(256)
 prior_rvs_kernel(int64_t B, uint64_t seed, uint64_t offset, const PriorEntry e,
+                 const double* __restrict__ loc, const double* __restrict__ scale,
                  double* __restrict__ out) {
     const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= B) return;
@@ -77,7 +81,9 @@ prior_rvs_kernel(int64_t B, uint64_t seed, uint64_t offset, const PriorEntry e,
             y = -log(u);                                     // expon
         }
     }
-    out[i] = e.loc + e.scale * y;
+    const double l = loc ? loc[i] : e.loc;
+    const double c = scale ? scale[i] : e.scale;
+    out[i] = (c >= 0.0) ? fma(c, y, l) : NAN;
 }
 
 __global__ void __launch_bounds__(256)
@@ -85,9 +91,59 @@ prior_logpdf_kernel(const double* __restrict__ x, int64_t ld, int64_t B, int p,
                     const PriorTable tab, double* __restrict__ out) {
     const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= B) return;
+    const double* row = x + i * ld;
+    const auto col = [&](int j) { return row[j]; };
     double s = 0.0;
-    for (int a = 0; a < p; ++a) s += prior_logpdf1(tab.e[a], x[i * ld + a]);
+    for (int a = 0; a < p; ++a) s += prior_logpdf1(tab.e[a], row[a], col);
     out[i] = s;
+}
+
+// the table of p parameters from 5 or 7 words each
+static int prior_table_from_host(const char* what, const double* spec_host, int p, int words,
+                                 PriorTable* tab) {
+    memset(tab, 0, sizeof(*tab));
+    for (int a = 0; a < p; ++a) {
+        char why[200];
+        const double* s = spec_host + words * a;
+        const bool ok = words == PRIOR_COND_SPEC_WORDS
+                            ? prior_entry_from_spec7(s, a, p, &tab->e[a], why, sizeof(why))
+                            : prior_entry_from_spec(s, &tab->e[a], why, sizeof(why));
+        ELFI_REQUIRE(ok, "%s: prior parameter %d: %s", what, a, why);
+    }
+    return ELFI_B200_OK;
+}
+
+static int prior_rvs_launch(elfi_b200_ctx* ctx, const double* spec_host, int64_t B, uint64_t seed,
+                            uint64_t offset, const double* loc, const double* scale, double* out,
+                            void* stream_) {
+    ELFI_REQUIRE(ctx && spec_host && B >= 0 && (B == 0 || out), "prior_rvs: bad argument");
+    PriorEntry e;
+    char why[160];
+    ELFI_REQUIRE(prior_entry_from_words(spec_host, loc ? 0 : -1, scale ? 0 : -1, &e, why, sizeof(why)),
+                 "prior_rvs: prior parameter 0: %s", why);
+    if (B == 0) return ELFI_B200_OK;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
+    prior_rvs_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(B, seed, offset, e, loc, scale,
+                                                                    out);
+    ELFI_CUDA_OK(cudaGetLastError());
+    return ELFI_B200_OK;
+}
+
+static int prior_logpdf_launch(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int64_t B,
+                               int64_t p, const double* spec_host, int words, double* out,
+                               void* stream_) {
+    ELFI_REQUIRE(ctx && spec_host && B >= 0 && (B == 0 || (x && out)), "prior_logpdf: bad argument");
+    ELFI_REQUIRE(p >= 1 && p <= PRIOR_MAX_PARAMS && ldx >= p, "prior_logpdf: bad shape (1 <= p <= 16)");
+    PriorTable tab;
+    const int rc = prior_table_from_host("prior_logpdf", spec_host, int(p), words, &tab);
+    if (rc != ELFI_B200_OK) return rc;
+    if (B == 0) return ELFI_B200_OK;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
+    prior_logpdf_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(x, ldx, B, int(p), tab, out);
+    ELFI_CUDA_OK(cudaGetLastError());
+    return ELFI_B200_OK;
 }
 
 }  // namespace elfi
@@ -96,38 +152,25 @@ extern "C" {
 
 int elfi_b200_prior_rvs_f64(elfi_b200_ctx* ctx, const double* spec_host, int64_t B, uint64_t seed,
                             uint64_t offset, double* out, void* stream_) {
-    using namespace elfi;
-    ELFI_REQUIRE(ctx && spec_host && B >= 0 && (B == 0 || out), "prior_rvs: bad argument");
-    PriorEntry e;
-    char why[160];
-    ELFI_REQUIRE(prior_entry_from_spec(spec_host, &e, why, sizeof(why)),
-                 "prior_rvs: prior parameter 0: %s", why);
-    if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    prior_rvs_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(B, seed, offset, e, out);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return elfi::prior_rvs_launch(ctx, spec_host, B, seed, offset, nullptr, nullptr, out, stream_);
+}
+
+int elfi_b200_prior_rvs_cond_f64(elfi_b200_ctx* ctx, const double* spec_host, int64_t B,
+                                 uint64_t seed, uint64_t offset, const double* loc,
+                                 const double* scale, double* out, void* stream_) {
+    return elfi::prior_rvs_launch(ctx, spec_host, B, seed, offset, loc, scale, out, stream_);
 }
 
 int elfi_b200_prior_logpdf_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int64_t B, int64_t p,
                                const double* spec_host, double* out, void* stream_) {
-    using namespace elfi;
-    ELFI_REQUIRE(ctx && spec_host && B >= 0 && (B == 0 || (x && out)), "prior_logpdf: bad argument");
-    ELFI_REQUIRE(p >= 1 && p <= PRIOR_MAX_PARAMS && ldx >= p, "prior_logpdf: bad shape (1 <= p <= 16)");
-    PriorTable tab;
-    memset(&tab, 0, sizeof(tab));
-    for (int a = 0; a < p; ++a) {
-        char why[160];
-        ELFI_REQUIRE(prior_entry_from_spec(spec_host + PRIOR_SPEC_WORDS * a, &tab.e[a], why, sizeof(why)),
-                     "prior_logpdf: prior parameter %d: %s", a, why);
-    }
-    if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    prior_logpdf_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(x, ldx, B, int(p), tab, out);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return elfi::prior_logpdf_launch(ctx, x, ldx, B, p, spec_host, elfi::PRIOR_SPEC_WORDS, out,
+                                     stream_);
+}
+
+int elfi_b200_prior_logpdf_cond_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int64_t B,
+                                    int64_t p, const double* spec_host, double* out, void* stream_) {
+    return elfi::prior_logpdf_launch(ctx, x, ldx, B, p, spec_host, elfi::PRIOR_COND_SPEC_WORDS, out,
+                                     stream_);
 }
 
 }  // extern "C"

@@ -16,6 +16,19 @@
 // closed support, else the standardised log density of y minus log(scale) -- with scipy's values
 // on the support edges (xlogy / xlog1py: +inf for gamma a < 1 or beta a < 1 at y = 0, finite for
 // a = 1, -inf for a > 1; the same for beta's b at y = 1).  NaN in, NaN out.
+//
+// Conditional loc / scale.  An entry's loc and scale may instead come from another column of the
+// same row (loc_src, scale_src: -1 the table's constant, j the column j != the parameter itself),
+// as in a hierarchical model where t2 ~ U(t1, t1 + 10).  The 7-word form [kind, p0, p1, p2, p3,
+// loc_src, scale_src] carries them; a sourced word among the first five is a placeholder and is
+// not validated.  Shape parameters always are constants.  The draw loc + scale y keeps y's stream,
+// so only the affine step and the density's (x - loc) / scale and log(scale) become per-row.
+// Per-row rule (SciPy 1.18.1's):
+//   logpdf: a scale that is not > 0, or NaN, gives NaN; a NaN loc gives NaN; an infinite scale
+//           gives y = 0 (or NaN for an infinite x - loc) and so -inf for uniform (-log(inf));
+//   rvs:    a scale of 0 gives loc; a NaN loc gives NaN; a scale < 0 or NaN gives NaN (SciPy raises).
+// A sourced scale takes its log on the device; a constant one keeps the host-computed log_scale,
+// so with every source at -1 the densities are the bits of the 5-word table.
 #pragma once
 
 #include <math.h>
@@ -33,12 +46,14 @@ namespace elfi {
 enum PriorKind { PRIOR_UNIFORM = 0, PRIOR_NORM = 1, PRIOR_TRUNCNORM = 2, PRIOR_EXPON = 3,
                  PRIOR_GAMMA = 4, PRIOR_BETA = 5 };
 constexpr int PRIOR_SPEC_WORDS = 5;      // [kind, p0, p1, p2, p3] per parameter
+constexpr int PRIOR_COND_SPEC_WORDS = 7; // [kind, p0, p1, p2, p3, loc_src, scale_src]
 constexpr int PRIOR_MAX_PARAMS = 16;
 constexpr int PRIOR_MAX_TRIALS = 64;     // Marsaglia-Tsang trials per gamma component
 constexpr double PRIOR_NORM_LOGC = 0.91893853320467274178;   // log(sqrt(2 pi))
 
 struct PriorEntry {
     int kind;
+    int loc_src, scale_src;   // -1: loc / scale are the constants below; j: column j of the row
     double loc, scale, log_scale;
     double a, b;           // shapes: truncnorm's bounds, gamma's a, beta's a and b
     double lognorm;        // truncnorm: log of the mass in [a, b]; gamma: lgamma(a); beta: betaln(a, b)
@@ -84,22 +99,44 @@ ELFI_PRIOR_HD double prior_std_logpdf(const PriorEntry& e, double y) {
     }
 }
 
-// scipy.stats.<kind>.logpdf(x, *params)
-ELFI_PRIOR_HD double prior_logpdf1(const PriorEntry& e, double x) {
-    const double y = (x - e.loc) / e.scale;
+// scipy.stats.<kind>.logpdf(x, *params) of a parameter of the row whose column j is col(j)
+// (read only for a sourced loc or scale).  COND = false compiles the sources out, for tables
+// known to have none.
+template <bool COND = true, class Col>
+ELFI_PRIOR_HD double prior_logpdf1(const PriorEntry& e, double x, const Col& col) {
+    const double loc = (COND && e.loc_src >= 0) ? col(e.loc_src) : e.loc;
+    double scale = e.scale, log_scale = e.log_scale;
+    if (COND && e.scale_src >= 0) {
+        scale = col(e.scale_src);
+        if (!(scale > 0.0)) return NAN;
+        log_scale = log(scale);
+    }
+    const double y = (x - loc) / scale;
     if (y != y) return y;
     if (!prior_in_support(e, y)) return -INFINITY;
-    return prior_std_logpdf(e, y) - e.log_scale;
+    return prior_std_logpdf(e, y) - log_scale;
 }
 
-// joint log density of p <= PMAX independent parameters: the terms summed left to right (the
-// loop is unrolled over PMAX so that a caller's x[] can live in registers)
-template <int PMAX = PRIOR_MAX_PARAMS>
+// x[src] of a row held in a local array: an unrolled select over PMAX, so that x[] can stay in
+// registers (an indexed load would put it on the stack)
+template <int PMAX>
+ELFI_PRIOR_HD double prior_pick(const double* x, int src) {
+    double v = 0.0;
+#pragma unroll
+    for (int b = 0; b < PMAX; ++b)
+        if (b == src) v = x[b];
+    return v;
+}
+
+// joint log density of p <= PMAX parameters: the terms summed left to right (the loop is
+// unrolled over PMAX so that a caller's x[] can live in registers)
+template <int PMAX = PRIOR_MAX_PARAMS, bool COND = true>
 ELFI_PRIOR_HD double prior_joint_logpdf(const PriorEntry* e, const double* x, int p) {
     double s = 0.0;
+    const auto col = [&](int j) { return prior_pick<PMAX>(x, j); };
 #pragma unroll
     for (int a = 0; a < PMAX; ++a)
-        if (a < p) s += prior_logpdf1(e[a], x[a]);
+        if (a < p) s += prior_logpdf1<COND>(e[a], x[a], col);
     return s;
 }
 
@@ -137,9 +174,14 @@ inline void prior_gamma_constants(double s, double* d, double* c, double* inv_a)
     *c = 1.0 / sqrt(9.0 * *d);
 }
 
-inline bool prior_entry_from_spec(const double* s, PriorEntry* e, char* why, size_t n) {
+// loc_src / scale_src: -1 or the column the row supplies it from (checked by the caller); a sourced
+// loc or scale word of s is not read
+inline bool prior_entry_from_words(const double* s, int loc_src, int scale_src, PriorEntry* e,
+                                   char* why, size_t n) {
     const double k = s[0];
     *e = PriorEntry();
+    e->loc_src = loc_src;
+    e->scale_src = scale_src;
     if (!(k == 0.0 || k == 1.0 || k == 2.0 || k == 3.0 || k == 4.0 || k == 5.0)) {
         snprintf(why, n, "unknown kind %g (0 uniform, 1 norm, 2 truncnorm, 3 expon, 4 gamma, 5 beta)", k);
         return false;
@@ -149,8 +191,8 @@ inline bool prior_entry_from_spec(const double* s, PriorEntry* e, char* why, siz
                        (e->kind == PRIOR_GAMMA ? 1 : 0);
     e->a = nshape >= 1 ? s[1] : 0.0;
     e->b = nshape >= 2 ? s[2] : 0.0;
-    e->loc = s[1 + nshape];
-    e->scale = s[2 + nshape];
+    e->loc = loc_src < 0 ? s[1 + nshape] : 0.0;
+    e->scale = scale_src < 0 ? s[2 + nshape] : 1.0;
     if (!(e->scale > 0.0) || !isfinite(e->scale) || !isfinite(e->loc)) {
         snprintf(why, n, "loc must be finite and scale finite and > 0 (loc %g, scale %g)", e->loc, e->scale);
         return false;
@@ -192,6 +234,28 @@ inline bool prior_entry_from_spec(const double* s, PriorEntry* e, char* why, siz
         break;
     }
     return true;
+}
+
+// the 5-word form: constant loc and scale
+inline bool prior_entry_from_spec(const double* s, PriorEntry* e, char* why, size_t n) {
+    return prior_entry_from_words(s, -1, -1, e, why, n);
+}
+
+// the 7-word form of parameter a of p: words 5 and 6 are loc_src and scale_src, each -1 or an
+// integer column 0 <= j < p other than a
+inline bool prior_entry_from_spec7(const double* s, int a, int p, PriorEntry* e, char* why,
+                                   size_t n) {
+    int src[2];
+    for (int w = 0; w < 2; ++w) {
+        const double v = s[PRIOR_SPEC_WORDS + w];
+        if (!(v == -1.0 || (v >= 0.0 && v < double(p) && v == floor(v) && v != double(a)))) {
+            snprintf(why, n, "%s source must be -1 or a column 0 <= j < %d other than %d (got %g)",
+                     w ? "scale" : "loc", p, a, v);
+            return false;
+        }
+        src[w] = int(v);
+    }
+    return prior_entry_from_words(s, src[0], src[1], e, why, n);
 }
 
 }  // namespace elfi

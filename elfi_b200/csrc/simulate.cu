@@ -235,7 +235,8 @@ __global__ void gm_rvs_kernel(const double* __restrict__ means, int64_t ldm, con
 
 // The same proposals for p <= 16 and for support 3, "prior": a draw is kept iff the joint log
 // density of the prior table (priors.cuh) is finite, the rule of GMDistribution.rvs
-// (x[np.isfinite(prior_logpdf(x))], utils.py:200-261).  Trial t uses blocks 4t .. 4t + 2 of
+// (x[np.isfinite(prior_logpdf(x))], utils.py:200-261); a conditional entry's loc / scale is
+// read from the draw's own columns (support 4 on the host side).  Trial t uses blocks 4t .. 4t + 2 of
 // SALT_GM_RVS exactly as gm_rvs_kernel does (component uniform, z_0 z_1, z_2 z_3), so for p <= 4
 // the two kernels draw the same particles; z_{4+2k}, z_{5+2k} come from block 8t + k of
 // SALT_GM_RVS_WIDE (k = 0 .. 5).  The factor is packed: row a of L starts at a (a + 1) / 2.
@@ -244,7 +245,9 @@ struct PackedLower16 { double v[PRIOR_MAX_PARAMS * (PRIOR_MAX_PARAMS + 1) / 2]; 
 struct BoxSupport16 { double lo[PRIOR_MAX_PARAMS], hi[PRIOR_MAX_PARAMS]; };
 
 // PMAX (4, 8 or 16) >= p: the loops are unrolled over PMAX so that x[] and z[] stay in registers.
-template <int PMAX>
+// COND: the prior table has conditional entries (support 4); without them the sources are
+// compiled out (at PMAX 16 resolving them takes 168 registers instead of 96).
+template <int PMAX, bool COND>
 __global__ void __launch_bounds__(128)
 gm_rvs_wide_kernel(const double* __restrict__ means, int64_t ldm, const double* __restrict__ cumw,
                    int64_t N, int p, const PackedLower16 Lc, int64_t B, uint64_t seed,
@@ -287,7 +290,7 @@ gm_rvs_wide_kernel(const double* __restrict__ means, int64_t ldm, const double* 
             for (int a = 0; a < PMAX; ++a)
                 if (a < p) ok = ok && x[a] >= box.lo[a] && x[a] <= box.hi[a];
         } else if (support == 3) {
-            ok = isfinite(prior_joint_logpdf<PMAX>(prior.e, x, p));
+            ok = isfinite(prior_joint_logpdf<PMAX, COND>(prior.e, x, p));
         }
         if (ok) break;
     }
@@ -599,19 +602,27 @@ int elfi_b200_gm_rvs_cdf_f64(elfi_b200_ctx* ctx, const double* means, int64_t ld
     ELFI_REQUIRE(ctx && means && cumw && Lchol_host && (B == 0 || out), "gm_rvs: NULL argument");
     ELFI_REQUIRE(N >= 1 && p >= 1 && p <= PRIOR_MAX_PARAMS && ldm >= p && ldo >= p,
                  "gm_rvs: bad shape (p <= 16)");
-    ELFI_REQUIRE(support == 0 || (support == 1 && p == 2) || ((support == 2 || support == 3) && box_host),
+    ELFI_REQUIRE(support == 0 || (support == 1 && p == 2) ||
+                     ((support == 2 || support == 3 || support == 4) && box_host),
                  "gm_rvs: unknown support %d", support);
-    if (support == 3 || p > 4) {
-        // the wide kernel: support 3 (the prior table travels in box_host) or p > 4
+    if (support >= 3 || p > 4) {
+        // the wide kernel: support 3 or 4 (the prior table of 5 or 7 words per parameter travels
+        // in box_host; the kernel treats both as support 3) or p > 4
         PriorTable prior;
         memset(&prior, 0, sizeof(prior));
-        if (support == 3) {
+        const bool cond = support == 4;
+        if (support >= 3) {
             for (int a = 0; a < p; ++a) {
-                char why[160];
-                ELFI_REQUIRE(prior_entry_from_spec(box_host + PRIOR_SPEC_WORDS * a, &prior.e[a], why,
-                                                   sizeof(why)),
-                             "gm_rvs: prior parameter %d: %s", a, why);
+                char why[200];
+                const bool ok =
+                    support == 4
+                        ? prior_entry_from_spec7(box_host + PRIOR_COND_SPEC_WORDS * a, a, int(p),
+                                                 &prior.e[a], why, sizeof(why))
+                        : prior_entry_from_spec(box_host + PRIOR_SPEC_WORDS * a, &prior.e[a], why,
+                                                sizeof(why));
+                ELFI_REQUIRE(ok, "gm_rvs: prior parameter %d: %s", a, why);
             }
+            support = 3;
         }
         BoxSupport16 box16;
         memset(&box16, 0, sizeof(box16));
@@ -624,12 +635,13 @@ int elfi_b200_gm_rvs_cdf_f64(elfi_b200_ctx* ctx, const double* means, int64_t ld
         memset(&Lp, 0, sizeof(Lp));
         for (int a = 0; a < p; ++a)
             for (int b = 0; b <= a; ++b) Lp.v[a * (a + 1) / 2 + b] = Lchol_host[a * p + b];
-#define ELFI_GM_RVS_WIDE(PMAX)                                                                   \
-        gm_rvs_wide_kernel<PMAX><<<unsigned((B + 127) / 128), 128, 0, stream>>>(                  \
+#define ELFI_GM_RVS_WIDE(PMAX, COND)                                                             \
+        gm_rvs_wide_kernel<PMAX, COND><<<unsigned((B + 127) / 128), 128, 0, stream>>>(            \
             means, ldm, cumw, N, int(p), Lp, B, seed, offset, support, box16, prior, out, ldo)
-        if (p <= 4) ELFI_GM_RVS_WIDE(4);
-        else if (p <= 8) ELFI_GM_RVS_WIDE(8);
-        else ELFI_GM_RVS_WIDE(16);
+        if (p <= 4) { if (cond) ELFI_GM_RVS_WIDE(4, true); else ELFI_GM_RVS_WIDE(4, false); }
+        else if (p <= 8) { if (cond) ELFI_GM_RVS_WIDE(8, true); else ELFI_GM_RVS_WIDE(8, false); }
+        else if (cond) ELFI_GM_RVS_WIDE(16, true);
+        else ELFI_GM_RVS_WIDE(16, false);
 #undef ELFI_GM_RVS_WIDE
         ELFI_CUDA_OK(cudaGetLastError());
         return ELFI_B200_OK;

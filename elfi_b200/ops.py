@@ -589,12 +589,14 @@ def gm_cdf(weights, n=None):
     return cumw
 
 
-def gm_rvs(means, cov, weights, size, seed, offset=0, support=0, box=None, cdf=None, prior=None):
+def gm_rvs(means, cov, weights, size, seed, offset=0, support=0, box=None, cdf=None, prior=None,
+           sources=None):
     """GMDistribution.rvs on the device (elfi/methods/utils.py:200-261) for p <= 16; support=1
     keeps only draws inside the MA2 prior support, support=2 inside ``box`` = (lo (p,), hi (p,)),
     support=3 where the joint log density of ``prior`` (a (p, 5) table of :func:`prior_logpdf`) is
-    finite (redrawn per particle).  ``cdf`` = :func:`gm_cdf` of the weights (then ``weights`` is
-    not read)."""
+    finite (redrawn per particle), support=4 the same with conditional priors (``sources`` (p, 2)
+    as in :func:`prior_logpdf`; the draws of support 3 when every source is -1).  ``cdf`` =
+    :func:`gm_cdf` of the weights (then ``weights`` is not read)."""
     means = _matrix(means)
     N, p = means.shape
     cov = np.atleast_2d(np.asarray(cov, dtype=np.float64))
@@ -605,8 +607,10 @@ def gm_rvs(means, cov, weights, size, seed, offset=0, support=0, box=None, cdf=N
     if support == 2:
         boxarr = np.ascontiguousarray(np.concatenate([np.asarray(box[0], dtype=np.float64),
                                                       np.asarray(box[1], dtype=np.float64)]))
-    elif support == 3:
-        boxarr = _prior_table(prior)
+    elif support in (3, 4):
+        boxarr = _prior_table(prior, sources if support == 4 else None)
+        if support == 4 and sources is None:
+            raise ValueError('support 4 takes the sources of the conditional priors')
         if boxarr.shape[0] != p:
             raise ValueError('the prior table has {} parameters, the mixture {}'.format(
                 boxarr.shape[0], p))
@@ -628,16 +632,20 @@ PRIOR_SHAPES = {'uniform': (), 'norm': (), 'truncnorm': ('a', 'b'), 'expon': (),
                 'beta': ('a', 'b')}
 MAX_PRIOR_PARAMS = 16
 PRIOR_SPEC_WORDS = 5
+PRIOR_COND_SPEC_WORDS = 7      # [kind, p0, p1, p2, p3, loc_src, scale_src]
 
 
-def _prior_spec_error(spec):
-    """Why a [kind, p0, p1, p2, p3] row is invalid (the library's checks), or None."""
+def _prior_spec_error(spec, loc_src=-1, scale_src=-1):
+    """Why a [kind, p0, p1, p2, p3] row is invalid (the library's checks), or None.  A loc or
+    scale with a source (>= 0) is a placeholder and is not checked."""
     k = spec[0]
     if k not in range(len(PRIOR_KINDS)):
         return 'unknown kind {!r} (supported: {})'.format(k, ', '.join(PRIOR_KINDS))
     name = PRIOR_KINDS[int(k)]
     ns = len(PRIOR_SHAPES[name])
-    shapes, loc, scale = spec[1:1 + ns], spec[1 + ns], spec[2 + ns]
+    shapes = spec[1:1 + ns]
+    loc = spec[1 + ns] if loc_src < 0 else 0.0
+    scale = spec[2 + ns] if scale_src < 0 else 1.0
     if not (np.isfinite(loc) and np.isfinite(scale) and scale > 0):
         return 'loc must be finite and scale finite and > 0 (loc {}, scale {})'.format(loc, scale)
     if name == 'truncnorm' and not shapes[0] < shapes[1]:
@@ -648,43 +656,89 @@ def _prior_spec_error(spec):
     return None
 
 
-def _prior_table(specs):
+def _prior_sources(sources, p):
+    """(p, 2) float64 [loc_src, scale_src] per parameter: -1 or another column 0 <= j < p."""
+    s = np.asarray(sources, dtype=np.float64)
+    if s.shape != (p, 2):
+        raise ValueError('sources are (p, 2) = ({}, 2) [loc_src, scale_src], got shape {}'.format(
+            p, s.shape))
+    for a in range(p):
+        for w, what in enumerate(('loc', 'scale')):
+            v = s[a, w]
+            if not (v == -1 or (0 <= v < p and v == int(v) and v != a)):
+                raise ValueError('prior parameter {}: the {} source must be -1 or a column '
+                                 '0 <= j < {} other than {}, got {}'.format(a, what, p, a, v))
+    return s
+
+
+def _prior_table(specs, sources=None):
+    """The (p, 5) table, or with sources the (p, 7) table of conditional priors."""
     t = np.ascontiguousarray(np.atleast_2d(np.asarray(specs, dtype=np.float64)))
     if t.ndim != 2 or t.shape[1] != 5 or not 1 <= t.shape[0] <= MAX_PRIOR_PARAMS:
         raise ValueError('a prior table is (p, 5) with 1 <= p <= {}, got shape {}'.format(
             MAX_PRIOR_PARAMS, np.shape(specs)))
+    src = None if sources is None else _prior_sources(sources, t.shape[0])
     for i, row in enumerate(t):
-        why = _prior_spec_error(row)
+        why = _prior_spec_error(row, *(() if src is None else src[i]))
         if why:
             raise ValueError('prior parameter {}: {}'.format(i, why))
-    return t
+    return t if src is None else np.ascontiguousarray(np.concatenate([t, src], axis=1))
 
 
-def prior_rvs(spec, size, seed, offset=0):
+def _row_vector(v, size, what):
+    if v is None:
+        return None
+    v = dev.to_device(v).reshape(-1)
+    if v.numel() == 1 and size != 1:
+        v = v.expand(size)
+    if v.numel() != size:
+        raise ValueError('{} has {} values for {} draws'.format(what, v.numel(), size))
+    return v.contiguous()
+
+
+def prior_rvs(spec, size, seed, offset=0, loc=None, scale=None):
     """``size`` draws of one stock prior on the device: spec = [kind, p0, p1, p2, p3]
     (PRIOR_KINDS, scipy's positional parameters).  Row i is a pure function of (seed, offset + i).
+    ``loc`` / ``scale``: per-row values (size,) that replace spec's (then its word is a
+    placeholder), for a prior whose loc or scale is another parameter; draw i is then loc_i +
+    scale_i y_i with y_i the standard draw of the same stream, NaN where scale_i < 0 or NaN.
     Returns a device tensor (size,)."""
-    t = _prior_table(spec)
+    size = int(size)
+    t = np.ascontiguousarray(np.atleast_2d(np.asarray(spec, dtype=np.float64)))
     if t.shape[0] != 1:
         raise ValueError('prior_rvs draws one parameter; got {} specs'.format(t.shape[0]))
-    out = dev.empty((int(size),))
-    _lib.call('elfi_b200_prior_rvs_f64', dev.context(), dev.ptr(t), int(size), int(seed), int(offset),
-              dev.ptr(out), dev.stream_ptr())
+    lv, sv = _row_vector(loc, size, 'loc'), _row_vector(scale, size, 'scale')
+    if t.shape[1] == 5:
+        why = _prior_spec_error(t[0], -1 if lv is None else 0, -1 if sv is None else 0)
+        if why:
+            raise ValueError('prior parameter 0: ' + why)
+    else:
+        _prior_table(t)                     # the shape error
+    out = dev.empty((size,))
+    if lv is None and sv is None:
+        _lib.call('elfi_b200_prior_rvs_f64', dev.context(), dev.ptr(t), size, int(seed),
+                  int(offset), dev.ptr(out), dev.stream_ptr())
+    else:
+        _lib.call('elfi_b200_prior_rvs_cond_f64', dev.context(), dev.ptr(t), size, int(seed),
+                  int(offset), dev.ptr(lv), dev.ptr(sv), dev.ptr(out), dev.stream_ptr())
     return out
 
 
-def prior_logpdf(params, specs):
+def prior_logpdf(params, specs, sources=None):
     """Joint log density of independent stock priors at the rows of params (B, p): the sum, left
     to right, of scipy.stats.<kind>.logpdf per column; -inf outside the support.  specs (p, 5).
-    Returns a device tensor (B,)."""
-    t = _prior_table(specs)
+    ``sources`` (p, 2) [loc_src, scale_src]: -1 for the table's constant, j for column j of the
+    same row (a conditional prior; include/elfi_b200.h has the per-row rule).  Returns a device
+    tensor (B,)."""
+    t = _prior_table(specs, sources)
     x = _matrix(params)
     if x.shape[1] != t.shape[0]:
         raise ValueError('params have {} columns, the prior table {} rows'.format(x.shape[1],
                                                                                  t.shape[0]))
     out = dev.empty((x.shape[0],))
-    _lib.call('elfi_b200_prior_logpdf_f64', dev.context(), dev.ptr(x), _ld(x), x.shape[0],
-              t.shape[0], dev.ptr(t), dev.ptr(out), dev.stream_ptr())
+    name = 'elfi_b200_prior_logpdf_f64' if sources is None else 'elfi_b200_prior_logpdf_cond_f64'
+    _lib.call(name, dev.context(), dev.ptr(x), _ld(x), x.shape[0], t.shape[0], dev.ptr(t),
+              dev.ptr(out), dev.stream_ptr())
     return out
 
 
@@ -1422,4 +1476,68 @@ def arch_summaries(y, n_lags=5):
     S = dev.empty((B, K))
     _lib.call('elfi_b200_arch_summaries_f64', dev.context(), dev.ptr(y), y.stride(0), y.stride(1),
               B, n, n_lags, dev.ptr(S), K, dev.stream_ptr())
+    return S
+
+
+# ---- M/G/1 queue (elfi/examples/mg1.py) ------------------------------------------------------------
+MG1_NOBS_MIN = 2
+MG1_NOBS_MAX = 512            # a row is sorted by one warp in registers
+MG1_NQ_MAX = 32               # quantile levels
+
+
+def _mg1_q(q):
+    q = np.array(q, dtype=np.float64).reshape(-1)
+    if not 1 <= q.size <= MG1_NQ_MAX:
+        raise ValueError('the device quantiles take 1 <= len(q) <= {} levels, got {}'.format(
+            MG1_NQ_MAX, q.size))
+    if not np.all((q >= 0) & (q <= 1)):
+        raise ValueError('the quantile levels q must lie in [0, 1]')
+    return np.ascontiguousarray(q)
+
+
+def _mg1_n(n, what):
+    if int(n) != n or not MG1_NOBS_MIN <= n <= MG1_NOBS_MAX:
+        raise ValueError('{} take {} <= n <= {} observations per row, got {}'.format(
+            what, MG1_NOBS_MIN, MG1_NOBS_MAX, n))
+    return int(n)
+
+
+def sim_mg1(params, n_obs=50, q=np.linspace(0, 1, 10), seed=0, offset=0, want_data=False,
+            want_summaries=True):
+    """M/G/1 queue simulator on the device (elfi/examples/mg1.py:21-54).  params: (batch, 3) columns
+    t1, t2, t3.  Row i is a pure function of (seed, offset + i); rows where the reference raises
+    (1/t3 with its sign bit set, t2 - t1 not finite) are NaN.
+
+    Returns (Y, S), each None unless asked for: Y (batch, n_obs) the inter-departure times, S
+    (batch, len(q)) their quantiles np.quantile(y, q) (method 'linear'), computed in the simulator
+    without writing Y, bit for bit :func:`row_quantiles` of Y."""
+    n_obs = _mg1_n(n_obs, 'the device M/G/1 simulator and its quantiles')
+    qv = _mg1_q(q)
+    P = _matrix(params)
+    if P.shape[1] != 3:
+        raise ValueError('the M/G/1 model has 3 parameters (t1, t2, t3), got a parameter width '
+                         'of {}'.format(P.shape[1]))
+    B = P.shape[0]
+    Y = dev.empty((B, n_obs)) if want_data else None
+    S = dev.empty((B, qv.size)) if want_summaries else None
+    _lib.call('elfi_b200_sim_mg1_f64', dev.context(), dev.ptr(P), _ld(P), B, n_obs, qv.size,
+              dev.ptr(qv), int(seed), int(offset), dev.ptr(Y), n_obs, dev.ptr(S), qv.size,
+              dev.stream_ptr())
+    return Y, S
+
+
+def row_quantiles(x, q):
+    """np.quantile(x, q, axis=1).T (method 'linear') of device data x (batch, n), any strides:
+    a (batch, len(q)) tensor, bit for bit NumPy's; a row containing NaN has every quantile NaN.
+    Limits: 2 <= n <= MG1_NOBS_MAX, 1 <= len(q) <= MG1_NQ_MAX, q in [0, 1]."""
+    if not (dev.is_device_array(x) and x.dtype == torch.float64):
+        x = dev.to_device(x)
+    if x.dim() != 2:
+        raise ValueError('row_quantiles takes (batch, n) data, got shape {}'.format(tuple(x.shape)))
+    n = _mg1_n(int(x.shape[1]), 'the device row quantiles')
+    qv = _mg1_q(q)
+    B = int(x.shape[0])
+    S = dev.empty((B, qv.size))
+    _lib.call('elfi_b200_row_quantiles_f64', dev.context(), dev.ptr(x), x.stride(0), x.stride(1),
+              B, n, qv.size, dev.ptr(qv), dev.ptr(S), qv.size, dev.stream_ptr())
     return S

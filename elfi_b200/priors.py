@@ -15,14 +15,30 @@ then offers the throughput mode's two device paths for it:
     dp = elfi_b200.DeviceModelPrior(m)
     elfi_b200.SMC(dp.model['d'], device_proposal=dp, batch_size=..., seed=...)
 
-Conditional priors (a parameter that is another node), vector priors (``size=``) and other
-distributions are rejected with a ValueError naming the node.
+Conditional priors.  ``DeviceModelPrior(model, conditional=True)`` also accepts a prior whose loc
+and / or scale is another Prior of the model, ELFI's hierarchical style, as in
+``Prior('uniform', m['t1'], 10, name='t2')`` (t2 ~ U(t1, t1 + 10)).  The parent's column is recorded
+in ``sources`` ((p, 2): [loc_src, scale_src], -1 for a constant): the device draws take the
+parent's draws as per-row loc / scale (ops.prior_rvs), and the proposals and densities read them
+from the same row (ops.gm_rvs support 4, ops.prior_logpdf with sources).  A model without such a
+parameter makes exactly the calls of one with constant priors (support 3, a (p, 5) table).  The
+default, ``conditional=False``, keeps the constant-parameter contract: a prior with a node parent
+is refused, so a model is never silently given a different device prior family than it was
+checked for.
+
+Rejected with a ValueError naming the node: a node parent (without ``conditional=True``; with it, a
+node parent in a shape position -- truncnorm's a, b, gamma's a, beta's a, b -- or a parent that is
+not a Prior, such as an Operation or a Simulator), vector priors (``size=``) and other
+distributions.
+
+    dp = elfi_b200.DeviceModelPrior(m, conditional=True)     # e.g. examples.mg1
 """
 from functools import partial
 
 import numpy as np
 import scipy.stats as ss
 
+from . import device as dev
 from . import model as em
 from . import ops
 from .throughput import batch_key
@@ -71,8 +87,17 @@ class DevicePriorDistribution:
         self.__name__ = 'device_' + kind
 
     def rvs(self, *params, size=1, random_state=None):
+        """Draws with scalar parameters; a loc or scale that is a vector (the draws of a parent
+        prior, one per row) goes to ops.prior_rvs per row."""
         n = int(np.prod(size))
-        return ops.prior_rvs(prior_spec(self.kind, params), n, batch_key(random_state))
+        ns = len(ops.PRIOR_SHAPES[self.kind])
+        consts, rows = [], {}
+        for i, v in enumerate(params):
+            if i >= ns and (dev.is_device_array(v) or np.ndim(v) > 0):
+                rows['loc' if i == ns else 'scale'] = v
+                v = 0.0 if i == ns else 1.0
+            consts.append(v)
+        return ops.prior_rvs(prior_spec(self.kind, consts), n, batch_key(random_state), **rows)
 
     def pdf(self, x, *params):
         return self.scipy.pdf(x, *params)
@@ -81,7 +106,7 @@ class DevicePriorDistribution:
         return self.scipy.logpdf(x, *params)
 
 
-def _node_spec(model, name):
+def _node_spec(model, name, conditional):
     rec = model.record(name)
     if not issubclass(rec.cls, em.RandomVariable):
         raise ValueError("parameter '{}' is not a Prior ({})".format(name, rec.cls.__name__))
@@ -92,12 +117,27 @@ def _node_spec(model, name):
     if kind is None:
         raise ValueError("prior '{}': {} is not supported on the device (supported: {})".format(
             name, what, ', '.join(SUPPORTED)))
-    values = []
+    ns = len(ops.PRIOR_SHAPES[kind])
+    values, parents = [], [None, None]
     for i, parent in enumerate(rec.inputs):
         prec = model.record(parent)
         if not issubclass(prec.cls, em.Constant):
-            raise ValueError("prior '{}': parameter {} depends on node '{}'; only priors with "
-                             "constant parameters run on the device".format(name, i, parent))
+            if not conditional:
+                raise ValueError("prior '{}': parameter {} depends on node '{}'; only priors with "
+                                 "constant parameters run on the device (a loc or scale that is "
+                                 "another Prior needs DeviceModelPrior(model, conditional=True))"
+                                 .format(name, i, parent))
+            if i < ns:
+                raise ValueError("prior '{}': its shape parameter {} ({}) depends on node '{}'; "
+                                 "only loc and scale may come from another prior".format(
+                                     name, i, ops.PRIOR_SHAPES[kind][i], parent))
+            if not issubclass(prec.cls, em.Prior) or i > ns + 1:
+                raise ValueError("prior '{}': parameter {} depends on node '{}' ({}); loc and "
+                                 "scale may come from another Prior only".format(
+                                     name, i, parent, prec.cls.__name__))
+            parents[i - ns] = parent
+            values.append(0.0 if i == ns else 1.0)     # placeholders
+            continue
         v = prec.constant
         if np.ndim(v) != 0 or not np.isreal(v):
             raise ValueError("prior '{}': parameter {} is not a real scalar ({!r})".format(
@@ -110,7 +150,7 @@ def _node_spec(model, name):
     why = ops._prior_spec_error(np.asarray(spec))
     if why:
         raise ValueError("prior '{}': {}".format(name, why))
-    return kind, spec
+    return kind, spec, parents
 
 
 def _device_copy(model, kinds):
@@ -129,30 +169,38 @@ def _device_copy(model, kinds):
 class DeviceModelPrior:
     """Joint prior of a model with stock scipy.stats priors, on the device (see the module
     docstring).  ``parameter_names`` are the model's (sorted) parameter names; ``specs`` is the
-    (p, 5) table handed to the kernels."""
+    (p, 5) table handed to the kernels and ``sources`` (p, 2) the columns a conditional loc /
+    scale comes from (-1: the constant in ``specs``).  ``conditional=True`` accepts a loc or scale
+    that is another Prior; by default only constant parameters are accepted."""
 
-    def __init__(self, model):
+    def __init__(self, model, conditional=False):
         names = list(model.parameter_names)
         if not names:
             raise ValueError('the model has no parameters')
         if len(names) > ops.MAX_PRIOR_PARAMS:
             raise ValueError('{} parameters; the device priors take at most {}'.format(
                 len(names), ops.MAX_PRIOR_PARAMS))
-        kinds, specs = {}, []
+        kinds, specs, sources = {}, [], []
         for name in names:
-            kind, spec = _node_spec(model, name)
+            kind, spec, parents = _node_spec(model, name, conditional)
             kinds[name] = kind
             specs.append(spec)
+            sources.append([-1 if p is None else names.index(p) for p in parents])
         self.parameter_names = names
         self.kinds = [kinds[n] for n in names]
         self.specs = np.asarray(specs, dtype=np.float64)
+        self.sources = np.asarray(sources, dtype=np.int64).reshape(len(names), 2)
+        self._cond = bool((self.sources >= 0).any())
         self.model = _device_copy(model, kinds)
 
     def rvs(self, means, cov, weights, size, key, cdf=None):
         """Mixture proposals (GMDistribution.rvs) redrawn until the joint prior density is
         positive; a (size, p) device tensor."""
+        if self._cond:
+            return ops.gm_rvs(means, cov, weights, size, seed=key, support=4, prior=self.specs,
+                              sources=self.sources, cdf=cdf)
         return ops.gm_rvs(means, cov, weights, size, seed=key, support=3, prior=self.specs, cdf=cdf)
 
     def logpdf(self, params):
         """Joint prior log density of the rows of params (B, p); a device tensor (B,)."""
-        return ops.prior_logpdf(params, self.specs)
+        return ops.prior_logpdf(params, self.specs, self.sources if self._cond else None)

@@ -379,7 +379,8 @@ int elfi_b200_probe_fp64_f64(elfi_b200_ctx* ctx, double* tflops_host);
  *                               (p = 2), 2 = box: box_host = [lo_0..lo_{p-1}, hi_0..hi_{p-1}],
  *                               3 = prior: box_host = the 5p-word prior table of
  *                               elfi_b200_prior_logpdf_f64, a draw is kept iff its joint log
- *                               density is finite).  At most 1000 draws per row: when all of them
+ *                               density is finite; 4 = the same with the 7p-word table of
+ *                               conditional priors).  At most 1000 draws per row: when all of them
  *                               fall outside the support, the 1000th draw is returned as it is
  *                               (outside the support).  For p <= 4 with supports 0-2 the streams
  *                               are those of earlier versions; support 3 uses the same blocks, and
@@ -428,11 +429,37 @@ int elfi_b200_gm_rvs_cdf_f64(elfi_b200_ctx* ctx, const double* means, int64_t ld
  *                               x (B, p; leading dimension ldx): the sum, left to right, of
  *                               scipy.stats.<kind>.logpdf, -inf outside the closed support and
  *                               scipy's values on its edges (spec_host: 5p words)
+ *
+ * Conditional loc / scale (a hierarchical prior such as t2 ~ U(t1, t1 + 10)): the 7-word form
+ * [kind, p0, p1, p2, p3, loc_src, scale_src] takes the loc and / or the scale of a parameter from
+ * column loc_src / scale_src of the same row (-1: the constant word; j: column j, 0 <= j < p, not
+ * the parameter itself).  A sourced word among the first five is a placeholder and is not
+ * validated; shape parameters are always constants; a bad source returns ELFI_B200_ERR_ARG.  Per
+ * row, as SciPy 1.18.1:
+ *   logpdf: a scale that is not > 0, or NaN, gives NaN; a NaN loc gives NaN; an infinite scale
+ *           gives -inf for uniform (y = 0 and -log(inf)).  A sourced scale takes its log on the
+ *           device, a constant one keeps the host's; with every source -1 the result is the bits
+ *           of the 5-word table.
+ *   rvs:    a scale of 0 gives loc; a NaN loc gives NaN; a scale < 0 or NaN gives NaN (where
+ *           SciPy raises).
+ *   elfi_b200_prior_rvs_cond_f64     prior_rvs with per-row loc and / or scale: `loc`, `scale` are
+ *                                    device (B,) vectors or NULL (then spec_host's word is used);
+ *                                    out[i] = fma(scale_i, y_i, loc_i) with y_i the standard draw
+ *                                    of the same stream as elfi_b200_prior_rvs_f64 (which computes
+ *                                    fma(scale, y_i, loc)); with both NULL the two are the same bits
+ *   elfi_b200_prior_logpdf_cond_f64  prior_logpdf with the 7p-word table
+ *   elfi_b200_gm_rvs(_cdf)_f64 with support = 4: box_host is the 7p-word table; the draws use the
+ *                                    blocks of support 3, so with every source -1 they are its bits
  */
 int elfi_b200_prior_rvs_f64(elfi_b200_ctx* ctx, const double* spec_host, int64_t B, uint64_t seed,
                             uint64_t offset, double* out, void* stream);
 int elfi_b200_prior_logpdf_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int64_t B, int64_t p,
                                const double* spec_host, double* out, void* stream);
+int elfi_b200_prior_rvs_cond_f64(elfi_b200_ctx* ctx, const double* spec_host, int64_t B,
+                                 uint64_t seed, uint64_t offset, const double* loc,
+                                 const double* scale, double* out, void* stream);
+int elfi_b200_prior_logpdf_cond_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int64_t B,
+                                    int64_t p, const double* spec_host, double* out, void* stream);
 
 /* Gaussian noise model of elfi/examples/gauss.py (1-d case): priors mu ~ U(prm[0], prm[0]+prm[1]),
  * sigma ~ truncnorm(prm[2], prm[3]) (gauss.py:118-126); simulator y = mu + sigma z (gauss.py:11-35)
@@ -655,6 +682,24 @@ int elfi_b200_sim_arch_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int
 int elfi_b200_arch_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_b, int64_t ld_j,
                                  int64_t B, int64_t n, int64_t n_lags, double* S, int64_t ldS,
                                  void* stream);
+
+/* M/G/1 queue of elfi/examples/mg1.py (throughput mode, statistical parity); stream layout, thread
+ * layout and arithmetic in elfi_b200/csrc/mg1.cu and mg1.cuh.  Rows where the reference's NumPy
+ * raises (1/t3 with its sign bit set, t2 - t1 not finite) give NaN data and NaN quantiles.
+ * sim_mg1: row i has parameters (t1, t2, t3) = P[i * ldP + 0..2] (ldP >= 3) and inter-departure
+ *   times Y[i * ldY + j], j < n_obs (2 <= n_obs <= 512); S[i * ldS + k] = np.quantile(y_i, q[k])
+ *   (method 'linear'; 1 <= nq <= 32, q_host on the host, each in [0, 1]) is computed in the same
+ *   kernel.  Y or S may be NULL; row i is a pure function of (seed, offset + i).
+ * row_quantiles: S[b * ldS + k] = np.quantile(X[b, :], q[k]) of the row X[b * ld_b + j * ld_j],
+ *   j < n (2 <= n <= 512), any strides; a row with a NaN has every quantile NaN.  Bit for bit
+ *   NumPy's, and the quantiles sim_mg1 fuses are the bits of row_quantiles of its data. */
+int elfi_b200_sim_mg1_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
+                          int64_t n_obs, int64_t nq, const double* q_host, uint64_t seed,
+                          uint64_t offset, double* Y, int64_t ldY, double* S, int64_t ldS,
+                          void* stream);
+int elfi_b200_row_quantiles_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_b, int64_t ld_j,
+                                int64_t B, int64_t n, int64_t nq, const double* q_host, double* S,
+                                int64_t ldS, void* stream);
 
 /* ---- KLIEP density-ratio estimation (AdaptiveThresholdSMC) -------------------------------------
  * DensityRatioEstimation.fit + max_ratio (elfi/methods/density_ratio_estimation.py:71-207):
