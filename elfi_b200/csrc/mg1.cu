@@ -18,43 +18,19 @@
 // has as many warps (at most 4) as fit in 64 KiB.  Not measured: keeping each row's sort in the
 // simulating thread (a register or shared-memory sort of n keys per thread) instead of the warp.
 //
-// row_quantiles_kernel loads any strided row into the same registers and calls the same code.  A
-// sorted row does not depend on the order its keys came in, so the fused and the unfused quantiles
-// are the same bits by construction.
-#include "bitonic.cuh"
+// row_quantiles_kernel loads any strided row into the same registers and calls the same code
+// (rowquantiles.cuh, which svm.cu shares).  A sorted row does not depend on the order its keys came
+// in, so the fused and the unfused quantiles are the same bits by construction.
 #include "common.cuh"
 #include "mg1.cuh"
 #include "philox.cuh"
+#include "rowquantiles.cuh"
 
 namespace elfi {
 
 constexpr uint32_t SALT_MG1 = 0x4d473151u;   // "MG1Q"
 constexpr int MG1_WARPS_MAX = 4;
 constexpr size_t MG1_STRIP_BUDGET = 64 * 1024;
-
-struct QuantileLevels {
-    double q[MG1_NQ_MAX];
-};
-
-// sort a register-resident row of n keys (padding ~0) and write quantile `lane` to S_row[lane]
-// for lane < nq (pk: the lane's pick)
-template <int KPL>
-__device__ __forceinline__ void quantiles_of_keys(uint64_t (&key)[KPL], int lane, int n, int nq,
-                                                  const ToadPick& pk, bool live, double* S_row) {
-    bitonic_in_registers<KPL>(key, lane);
-    const bool has_nan = pick_reg(key, n - 1) == ~uint64_t(0);
-    const double a = u64_to_key(pick_reg_lane(key, pk.lo));
-    const double b = u64_to_key(pick_reg_lane(key, pk.hi));
-    if (live && lane < nq) S_row[lane] = has_nan ? NAN : gnk_lerp(a, b, pk.t);
-}
-
-__device__ __forceinline__ ToadPick lane_pick(int n, int nq, const QuantileLevels& Q, int lane) {
-    double q = Q.q[0];
-#pragma unroll
-    for (int k = 1; k < MG1_NQ_MAX; ++k)
-        if (k == lane && k < nq) q = Q.q[k];
-    return toad_quantile_pick(n, q);
-}
 
 // P[i * ldP + 0..2] = (t1, t2, t3).  Y and S may be NULL.  blockDim.x = 32 * warps.
 template <int KPL>
@@ -125,21 +101,6 @@ row_quantiles_kernel(const double* __restrict__ X, int64_t ld_b, int64_t ld_j, i
     }
 }
 
-static int mg1_kpl(int n) {
-    int kpl = 1;
-    while (32 * kpl < n) kpl <<= 1;
-    return kpl;
-}
-
-static bool mg1_levels(const double* q_host, int64_t nq, QuantileLevels* Q) {
-    memset(Q, 0, sizeof(*Q));
-    for (int k = 0; k < nq; ++k) {
-        if (!(q_host[k] >= 0.0 && q_host[k] <= 1.0)) return false;
-        Q->q[k] = q_host[k];
-    }
-    return true;
-}
-
 }  // namespace elfi
 
 extern "C" {
@@ -157,7 +118,8 @@ int elfi_b200_sim_mg1_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int6
                  "ldY >= n_obs; n_obs=%lld nq=%lld ldP=%lld)", MG1_NOBS_MIN, MG1_NOBS_MAX,
                  MG1_NQ_MAX, (long long)n_obs, (long long)nq, (long long)ldP);
     QuantileLevels Q;
-    ELFI_REQUIRE(S == nullptr || mg1_levels(q_host, nq, &Q), "sim_mg1: every q must lie in [0, 1]");
+    ELFI_REQUIRE(S == nullptr || quantile_levels(q_host, nq, &Q),
+                 "sim_mg1: every q must lie in [0, 1]");
     if (S == nullptr) memset(&Q, 0, sizeof(Q));
     if (B == 0) return ELFI_B200_OK;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -173,7 +135,7 @@ int elfi_b200_sim_mg1_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int6
                                       cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));    \
     sim_mg1_kernel<KPL><<<blocks, 32 * warps, smem, stream>>>(P, ldP, B, n, npad, int(nq), Q,      \
                                                               seed, offset, Y, ldY, S, ldS)
-    switch (mg1_kpl(n)) {
+    switch (quantile_kpl(n)) {
     case 1: ELFI_SIM_MG1(1); break;
     case 2: ELFI_SIM_MG1(2); break;
     case 4: ELFI_SIM_MG1(4); break;
@@ -196,7 +158,7 @@ int elfi_b200_row_quantiles_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_
                  "nq=%lld ldS=%lld)", MG1_NOBS_MIN, MG1_NOBS_MAX, MG1_NQ_MAX, (long long)n,
                  (long long)nq, (long long)ldS);
     QuantileLevels Q;
-    ELFI_REQUIRE(mg1_levels(q_host, nq, &Q), "row_quantiles: every q must lie in [0, 1]");
+    ELFI_REQUIRE(quantile_levels(q_host, nq, &Q), "row_quantiles: every q must lie in [0, 1]");
     if (B == 0) return ELFI_B200_OK;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     ELFI_CUDA_OK(cudaSetDevice(ctx->device));
@@ -205,7 +167,7 @@ int elfi_b200_row_quantiles_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_
 #define ELFI_ROW_QUANTILES(KPL)                                                                    \
     row_quantiles_kernel<KPL><<<blocks, 256, 0, stream>>>(X, ld_b, ld_j, B, int(n), int(nq), Q, S, \
                                                           ldS)
-    switch (mg1_kpl(int(n))) {
+    switch (quantile_kpl(int(n))) {
     case 1: ELFI_ROW_QUANTILES(1); break;
     case 2: ELFI_ROW_QUANTILES(2); break;
     case 4: ELFI_ROW_QUANTILES(4); break;

@@ -62,6 +62,7 @@ __device__ __forceinline__ void toad_sim_one(const ToadSim& a, int64_t row, int 
         for (int d = 0; d < a.n_days; ++d) x(d) = NAN;
         return;
     }
+    const StableRow sr = toad_stable_row(alpha, gamma);
     const Philox ph(a.seed);
     const uint64_t crow = a.offset + uint64_t(row);
     const uint32_t r0 = uint32_t(crow), r1 = uint32_t(crow >> 32);
@@ -76,7 +77,7 @@ __device__ __forceinline__ void toad_sim_one(const ToadSim& a, int64_t row, int 
             const PhiloxWords w1 = ph(r0, r1, (cell << 1) | 1u, SALT_TOAD);
             const double TH = toad_theta(u01_open_top(w1.x, w1.y));
             const double W = toad_expon(u01(w1.z, w1.w));
-            cur = __dadd_rn(cur, toad_stable_step(alpha, gamma, TH, W));
+            cur = __dadd_rn(cur, stable_draw(sr, TH, W));
         }
         x(d) = cur;
     }

@@ -5,12 +5,9 @@
 // the device and plain operators on the host, where tests/harness/toad_harness.cpp builds this
 // header with -ffp-contract=off and checks it against NumPy.
 //
-// Step (scipy/stats/_levy_stable: _rvs_Z1 with beta = 0, then vals * scale + loc and the S1 shift
-// of levy_stable_gen.rvs), from TH uniform on (-pi/2, pi/2) and W standard exponential:
-//   alpha != 1  (beta0func)   W / (cos TH / tan(aTH) + sin TH) * ((cos aTH + sin aTH tan TH) / W) ** (1 / alpha)
-//   alpha == 1  (alpha1func)  2 / pi * ((pi / 2 + bTH) tan TH - beta log((pi / 2 W cos TH) / (pi / 2 + bTH)))
-//   with aTH = alpha TH, bTH = beta TH = +-0; then X = vals * gamma + 0, and at alpha == 1
-//   X + 2 beta gamma log(gamma) / pi, which is NaN at gamma = 0 (0 * -inf).
+// Step: stable.cuh's levy_stable draw with beta = 0, loc = 0, scale gamma, in S1 (SciPy's default):
+// the beta0func branch for alpha != 1, alpha1func at alpha == 1, where the S1 shift
+// 2 beta gamma log(gamma) / pi is NaN at gamma = 0 (0 * -inf).
 //
 // Summaries of one lag (compute_summaries): the kept set is the non-NaN |displacements| >= thd,
 // sorted, n of them.  np.nanquantile (method 'linear'): vi = (n - 1) p, lo = floor(vi), hi = lo + 1,
@@ -26,6 +23,7 @@
 #include <stdint.h>
 
 #include "gnkstats.cuh"
+#include "stable.cuh"
 
 namespace elfi {
 
@@ -35,44 +33,25 @@ constexpr int TOAD_LAGS_MAX = 8;           // lags of the fused summaries
 constexpr int TOAD_MEDIAN_SMALL = 600;     // below: np.ma.median; from here: np.median
 constexpr int64_t TOAD_CELLS_MAX = int64_t(1) << 31;   // n_days * n_toads: (cell << 1) | h < 2^32
 constexpr double TOAD_GAP_FLOOR = 0x1.1b48655f37267p-29;   // np.exp(-20)
-constexpr double TOAD_PI = 3.141592653589793;           // np.pi
-constexpr double TOAD_PI_2 = 1.5707963267948966;        // np.pi / 2
 
-ELFI_HD double toad_sin(double x) { return sin(x); }
-ELFI_HD double toad_cos(double x) { return cos(x); }
-ELFI_HD double toad_tan(double x) { return tan(x); }
 ELFI_HD double toad_log(double x) { return log(x); }
-ELFI_HD double toad_pow(double x, double y) { return pow(x, y); }
 
 // the reference raises for these (levy_stable's argcheck and scale >= 0); the device gives NaN rows
 ELFI_HD bool toad_params_ok(double alpha, double gamma) {
-    return alpha > 0.0 && alpha <= 2.0 && gamma >= 0.0;
+    return stable_params_ok(alpha, 0.0, gamma);
 }
 
-// TH = uniform.rvs(loc=-pi/2, scale=pi) from u in [0, 1): u * pi + (-pi / 2)
-ELFI_HD double toad_theta(double u) { return leaf_add(leaf_mul(u, TOAD_PI), -TOAD_PI_2); }
-// W = expon.rvs() from u in (0, 1]: -log(u) * 1 + 0
-ELFI_HD double toad_expon(double u) { return leaf_add(leaf_mul(-toad_log(u), 1.0), 0.0); }
+ELFI_HD double toad_theta(double u) { return stable_theta(u); }
+ELFI_HD double toad_expon(double u) { return stable_expon(u); }
+
+// the per-toad factors of levy_stable.rvs(alpha, beta=0, scale=gamma) (S1)
+ELFI_HD StableRow toad_stable_row(double alpha, double gamma) {
+    return stable_row(alpha, 0.0, 0.0, gamma, false);
+}
 
 // levy_stable.rvs(alpha, beta=0, scale=gamma) (S1) of one (TH, W)
 ELFI_HD double toad_stable_step(double alpha, double gamma, double TH, double W) {
-    const double aTH = leaf_mul(alpha, TH);
-    const double cosTH = toad_cos(TH), tanTH = toad_tan(TH);
-    double val;
-    if (alpha == 1.0) {
-        const double bTH = leaf_mul(0.0, TH);
-        const double h = leaf_add(TOAD_PI_2, bTH);
-        const double lg = toad_log(gnk_div(leaf_mul(leaf_mul(TOAD_PI_2, W), cosTH), h));
-        val = leaf_mul(2.0 / TOAD_PI, leaf_sub(leaf_mul(h, tanTH), leaf_mul(0.0, lg)));
-    } else {
-        const double den = leaf_add(gnk_div(cosTH, toad_tan(aTH)), toad_sin(TH));
-        const double num = leaf_add(toad_cos(aTH), leaf_mul(toad_sin(aTH), tanTH));
-        val = leaf_mul(gnk_div(W, den), toad_pow(gnk_div(num, W), gnk_div(1.0, alpha)));
-    }
-    double x = leaf_add(leaf_mul(val, gamma), 0.0);
-    if (alpha == 1.0)
-        x = leaf_add(x, gnk_div(leaf_mul(leaf_mul(0.0, gamma), toad_log(gamma)), TOAD_PI));
-    return x;
+    return stable_draw(toad_stable_row(alpha, gamma), TH, W);
 }
 
 // a refuge day uniform in [0, d) from a 64-bit word: the high word of w * d (bias below d / 2^64)

@@ -1541,3 +1541,42 @@ def row_quantiles(x, q):
     _lib.call('elfi_b200_row_quantiles_f64', dev.context(), dev.ptr(x), x.stride(0), x.stride(1),
               B, n, qv.size, dev.ptr(qv), dev.ptr(S), qv.size, dev.stream_ptr())
     return S
+
+
+# ---- alpha-stable stochastic volatility model (elfi/examples/stochastic_volatility_model.py) ---------
+SVM_NPARAMS = 7               # alpha, beta, kappa, eta, mu, phi, sigma
+SVM_LEVELS = (0.05, 0.25, 0.5, 0.75, 0.95)
+
+
+def sim_svm(params, n_obs=50, seed=0, offset=0, want_data=False, want_summaries=True):
+    """Alpha-stable stochastic volatility simulator on the device
+    (elfi/examples/stochastic_volatility_model.py).  params: (batch, 7) columns alpha, beta, kappa,
+    eta, mu, phi, sigma.  Row i is a pure function of (seed, offset + i); rows where the reference
+    raises (levy_stable's argcheck, kappa < 0, sigma < 0, phi NaN) are NaN.
+
+    Returns (Y, S), each None unless asked for: Y (batch, n_obs) the observations, S (batch, 2)
+    their quantile kurtosis and skewness [kurt, skew], computed in the simulator without writing
+    Y, bit for bit :func:`svm_summaries` of Y."""
+    n_obs = _mg1_n(n_obs, 'the device stochastic volatility simulator and its summaries')
+    P = _matrix(params)
+    if P.shape[1] != SVM_NPARAMS:
+        raise ValueError('the stochastic volatility model has 7 parameters (alpha, beta, kappa, '
+                         'eta, mu, phi, sigma), got a parameter width of {}'.format(P.shape[1]))
+    B = P.shape[0]
+    Y = dev.empty((B, n_obs)) if want_data else None
+    S = dev.empty((B, 2)) if want_summaries else None
+    _lib.call('elfi_b200_sim_svm_f64', dev.context(), dev.ptr(P), _ld(P), B, n_obs, int(seed),
+              int(offset), dev.ptr(Y), n_obs, dev.ptr(S), 2, dev.stream_ptr())
+    return Y, S
+
+
+def svm_summaries(x):
+    """[kurt, skew] (batch, 2) of device data x (batch, n), any strides, without the fused kernel:
+    :func:`row_quantiles` at 0.05, 0.25, 0.5, 0.75, 0.95, then the reference's subtractions and
+    division in fp64 (IEEE, so NumPy's bits):
+    kurt = (q95 - q05) / (q75 - q25), skew = ((q95 - q50) - (q50 - q05)) / (q95 - q05)."""
+    q = row_quantiles(x, SVM_LEVELS)
+    q05, q25, q50, q75, q95 = q.unbind(1)
+    kurt = (q95 - q05) / (q75 - q25)
+    skew = ((q95 - q50) - (q50 - q05)) / (q95 - q05)
+    return torch.stack([kurt, skew], dim=1)

@@ -701,6 +701,22 @@ int elfi_b200_row_quantiles_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_
                                 int64_t B, int64_t n, int64_t nq, const double* q_host, double* S,
                                 int64_t ldS, void* stream);
 
+/* Alpha-stable stochastic volatility model of elfi/examples/stochastic_volatility_model.py
+ * (throughput mode, statistical parity); stream layout, thread layout and arithmetic in
+ * elfi_b200/csrc/svm.cu, svm.cuh and stable.cuh.
+ * sim_svm: row i has parameters (alpha, beta, kappa, eta, mu, phi, sigma) = P[i * ldP + 0..6]
+ *   (ldP >= 7) and observations Y[i * ldY + j], j < n_obs (2 <= n_obs <= 512): an AR(1)
+ *   log-volatility x_j (stationary start) times levy_stable(alpha, beta, loc=eta, scale=kappa)
+ *   shocks in the S0 parameterization.  S[i * ldS + 0..1] (ldS >= 2) = (kurt, skew) of the row's
+ *   np.quantile at 0.05, 0.25, 0.5, 0.75, 0.95, computed in the same kernel, bit for bit the
+ *   row_quantiles of its data followed by the reference's subtractions and division.  Rows where
+ *   the reference raises (0 < alpha <= 2, -1 <= beta <= 1, kappa >= 0, sigma >= 0 violated, NaN
+ *   included, or phi = NaN) give NaN data and NaN summaries.  Y or S may be NULL; row i is a pure
+ *   function of (seed, offset + i). */
+int elfi_b200_sim_svm_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
+                          int64_t n_obs, uint64_t seed, uint64_t offset, double* Y, int64_t ldY,
+                          double* S, int64_t ldS, void* stream);
+
 /* ---- KLIEP density-ratio estimation (AdaptiveThresholdSMC) -------------------------------------
  * DensityRatioEstimation.fit + max_ratio (elfi/methods/density_ratio_estimation.py:71-207):
  * basis centres = first n_basis rows of x, A = RBF(x, centres), b = weighted RBF mean over y,
