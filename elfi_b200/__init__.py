@@ -8,6 +8,7 @@ surrogate, with the arithmetic in hand-written CUDA reached through a C ABI
 __version__ = '0.1.0'
 
 from . import _lib  # noqa: F401
+from . import tools  # noqa: F401
 from .model import (AdaptiveDistance, Constant, Discrepancy, Distance, ElfiModel,  # noqa: F401
                     NodeReference, Operation, Prior, RandomVariable, Simulator, Summary,
                     get_default_model, new_model, set_default_model)

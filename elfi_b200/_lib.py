@@ -123,6 +123,10 @@ SIGNATURES = {
                                     c_i64, c_ptr],
     'elfi_b200_sim_svm_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_u64, c_u64, c_ptr, c_i64, c_ptr,
                               c_i64, c_ptr],
+    'elfi_b200_sim_scratch_assay_f64': [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_i64, c_i64, c_i64,
+                                        c_i64, c_u64, c_u64, c_ptr, c_i64, c_ptr, c_ptr],
+    'elfi_b200_scratch_assay_summaries_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64,
+                                              c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr],
     'elfi_b200_gp_padded_size': [c_i64],
     'elfi_b200_gp_fit_f64': [c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_i64, c_dbl, c_dbl, c_dbl, c_dbl,
                              c_ptr, c_ptr, c_ptr, c_i64, c_ptr, c_ptr, c_ptr],

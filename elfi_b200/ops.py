@@ -1580,3 +1580,94 @@ def svm_summaries(x):
     kurt = (q95 - q05) / (q75 - q25)
     skew = ((q95 - q50) - (q50 - q05)) / (q95 - q05)
     return torch.stack([kurt, skew], dim=1)
+
+
+# ---- scratch assay (elfi/examples/scratch_assay.py) -----------------------------------------------
+SA_SITES_MAX = 4096            # lattice sites: the snapshot list is uint16, one warp's state in smem
+SA_ITER_MAX = 2 ** 31 - 1      # iteration counters of the Philox streams
+SA_BATCH_MAX = 2 ** 31 - 1     # one warp per row
+
+
+def scratch_assay_steps(obs_period=12, obs_interval=1 / 12, tau=1 / 24):
+    """(num_iter, interval, num_obs) as the reference's cell_sim computes them:
+    int(obs_period / tau), int(obs_interval / tau) and int(num_iter / interval)."""
+    num_iter = int(obs_period / tau)
+    interval = int(obs_interval / tau)
+    if not 0 <= num_iter <= SA_ITER_MAX:
+        raise ValueError('the device scratch assay simulator takes 0 <= int(obs_period / tau) < '
+                         '2^31 iterations, got {}'.format(num_iter))
+    if interval < 1:
+        raise ValueError('the scratch assay simulator takes obs_interval >= tau (at least one '
+                         'iteration between observations), got int(obs_interval / tau) = '
+                         '{}'.format(interval))
+    return num_iter, interval, int(num_iter / interval)
+
+
+def _scratch_init(init_arr):
+    """The initial lattice as a contiguous (nrows, ncols) uint8 device tensor, checked."""
+    t = init_arr if dev.is_device_array(init_arr) else dev.to_device(
+        np.asarray(init_arr, dtype=np.float64))
+    if t.dim() != 2:
+        raise ValueError('init_arr must be a 2-d (nrows, ncols) lattice, got shape {}'.format(
+            tuple(t.shape)))
+    nrows, ncols = (int(v) for v in t.shape)
+    if not (1 <= nrows and 1 <= ncols and nrows * ncols <= SA_SITES_MAX):
+        raise ValueError('the device scratch assay simulator takes a lattice of 1 to {} sites, '
+                         'got {} x {}'.format(SA_SITES_MAX, nrows, ncols))
+    if not bool(torch.all((t == 0) | (t == 1))):
+        raise ValueError('init_arr must hold 0s and 1s only')
+    return (t != 0).to(torch.uint8).contiguous()
+
+
+def sim_scratch_assay(params, init_arr, obs_period=12, obs_interval=1 / 12, tau=1 / 24, seed=0,
+                      offset=0, want_data=False, want_summaries=True):
+    """Scratch assay simulator on the device (elfi/examples/scratch_assay.py, Johnston et al.
+    2014), its streams replayed exactly by tests/scratch_assay_replay.py.  params: (batch, 2)
+    columns pm, pp; init_arr: the (nrows, ncols) initial lattice of 0s and 1s, at most
+    SA_SITES_MAX sites.  The iteration and observation counts are the reference's
+    (:func:`scratch_assay_steps`).  Row i is a pure function of (seed, offset + i).
+
+    Returns (X, S), each None unless asked for: X (batch, nrows, ncols, num_obs + 1) bool, the
+    frames; S (batch, num_obs + 1) float64, the mismatches between consecutive frames and the
+    final cell count (the reference's cell_summaries), computed in the simulator without writing
+    X, equal to :func:`scratch_assay_summaries` of X."""
+    num_iter, interval, num_obs = scratch_assay_steps(obs_period, obs_interval, tau)
+    init = _scratch_init(init_arr)
+    nrows, ncols = (int(v) for v in init.shape)
+    P = _matrix(params)
+    if P.shape[1] != 2:
+        raise ValueError('the scratch assay model has 2 parameters (pm, pp), got a parameter width '
+                         'of {}'.format(P.shape[1]))
+    B = P.shape[0]
+    if B > SA_BATCH_MAX:
+        raise ValueError('the device scratch assay simulator takes at most {} rows per call, got '
+                         '{}'.format(SA_BATCH_MAX, B))
+    X = dev.empty((B, nrows, ncols, num_obs + 1), dtype=torch.bool) if want_data else None
+    S = dev.empty((B, num_obs + 1)) if want_summaries else None
+    _lib.call('elfi_b200_sim_scratch_assay_f64', dev.context(), dev.ptr(P), _ld(P), B,
+              dev.ptr(init), nrows, ncols, num_iter, interval, int(seed), int(offset), dev.ptr(S),
+              num_obs + 1, dev.ptr(X), dev.stream_ptr())
+    return X, S
+
+
+def scratch_assay_summaries(x):
+    """The reference's cell_summaries of data (batch, nrows, ncols, n_frames), any strides, nonzero
+    meaning a cell: a (batch, n_frames) float64 tensor of the n_frames - 1 mismatches between
+    consecutive frames, then the cells of the last frame.  On 0 / 1 data these are NumPy's values
+    exactly (they are integers)."""
+    if not dev.is_device_array(x):
+        x = dev.to_device(np.asarray(x, dtype=np.float64))
+    if x.dtype not in (torch.bool, torch.uint8):
+        x = x != 0
+    if x.dim() != 4:
+        raise ValueError('scratch_assay_summaries takes (batch, nrows, ncols, n_frames) data, got '
+                         'shape {}'.format(tuple(x.shape)))
+    B, nrows, ncols, frames = (int(v) for v in x.shape)
+    if min(nrows, ncols, frames) < 1:
+        raise ValueError('scratch_assay_summaries takes nrows, ncols, n_frames >= 1, got shape '
+                         '{}'.format(tuple(x.shape)))
+    S = dev.empty((B, frames))
+    _lib.call('elfi_b200_scratch_assay_summaries_f64', dev.context(), dev.ptr(x), x.stride(0),
+              x.stride(1), x.stride(2), x.stride(3), B, nrows, ncols, frames, dev.ptr(S), frames,
+              dev.stream_ptr())
+    return S

@@ -717,6 +717,30 @@ int elfi_b200_sim_svm_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int6
                           int64_t n_obs, uint64_t seed, uint64_t offset, double* Y, int64_t ldY,
                           double* S, int64_t ldS, void* stream);
 
+/* Scratch assay model of elfi/examples/scratch_assay.py (throughput mode, exact replay of its
+ * streams); law, stream layout and warp layout in elfi_b200/csrc/scratch_assay.cuh and
+ * scratch_assay.cu.
+ * sim_scratch_assay: row i has parameters (pm, pp) = P[i * ldP + 0..1] (ldP >= 2) and starts from
+ *   the lattice init[r * ncols + c] (device, nrows * ncols <= 4096 bytes, nonzero = a cell).  It
+ *   runs num_iter (< 2^31) iterations of motility then proliferation and observes the lattice
+ *   every obs_interval (>= 1) iterations: num_obs = num_iter / obs_interval frames after the
+ *   initial one.  S[i * ldS + k] (ldS >= num_obs + 1) gets the mismatches between frames k and
+ *   k + 1, k < num_obs, then S[i * ldS + num_obs] the cells of the last frame; X gets the frames
+ *   X[((i * nrows + r) * ncols + c) * (num_obs + 1) + k] as 0 / 1.  S and X may each be NULL; S is
+ *   computed without writing X.  Row i is a pure function of (seed, offset + i); B < 2^31.
+ * scratch_assay_summaries: the same summaries S[i * ldS + k], k < n_frames (ldS >= n_frames), of
+ *   the frames X[i * ld_b + r * ld_r + c * ld_c + k * ld_k] (uint8, nonzero = a cell), any
+ *   strides: n_frames - 1 mismatches, then the cells of the last frame. */
+int elfi_b200_sim_scratch_assay_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
+                                    const uint8_t* init, int64_t nrows, int64_t ncols,
+                                    int64_t num_iter, int64_t obs_interval, uint64_t seed,
+                                    uint64_t offset, double* S, int64_t ldS, uint8_t* X,
+                                    void* stream);
+int elfi_b200_scratch_assay_summaries_f64(elfi_b200_ctx* ctx, const uint8_t* X, int64_t ld_b,
+                                          int64_t ld_r, int64_t ld_c, int64_t ld_k, int64_t B,
+                                          int64_t nrows, int64_t ncols, int64_t n_frames,
+                                          double* S, int64_t ldS, void* stream);
+
 /* ---- KLIEP density-ratio estimation (AdaptiveThresholdSMC) -------------------------------------
  * DensityRatioEstimation.fit + max_ratio (elfi/methods/density_ratio_estimation.py:71-207):
  * basis centres = first n_basis rows of x, A = RBF(x, centres), b = weighted RBF mean over y,
