@@ -11,12 +11,15 @@
 // under 10 % of the memory time at D=128 on an H100 SXM (data-sheet rates: 34 TFLOP/s fp64,
 // 3.35 TB/s), so the kernel is bandwidth bound as long as the TMA pipeline keeps enough rows in
 // flight per SM (see rowstream.cuh).
+//
+// What every metric shares is written once: dist_record() is the acceptance epilogue of all
+// kernels (row-stream consumers and thread-per-row fallbacks), rs_streams() decides between the
+// two, dist_params() fills the kernel parameters and dist_call() is the host skeleton of the entry
+// points over a device-resident matrix.  A metric adds its per-term arithmetic and its finish:
+// a consumer, a thread-per-row kernel and a case in launch_dist() or launch_metric().
 #include <cstdlib>
 
 #include "rowstream.cuh"
-
-extern "C" int elfi_b200_colmoments_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
-                                        int64_t D, double* out, void* stream);
 
 namespace elfi {
 
@@ -42,7 +45,7 @@ struct DistParams {
 // leaves a non-negative accumulator unchanged bit for bit.
 __device__ __forceinline__ void dist_setup_shared(uint8_t* aux, const DistParams& p, int D,
                                                   bool weighted) {
-    const int Dp = ((D + RS_BOX_COLS - 1) / RS_BOX_COLS) * RS_BOX_COLS;
+    const int Dp = rs_padded_cols(D);
     double* obs_s = reinterpret_cast<double*>(aux);
     for (int j = threadIdx.x; j < Dp; j += blockDim.x) obs_s[j] = j < D ? p.obs[j] : 0.0;
     if (weighted) {
@@ -53,17 +56,23 @@ __device__ __forceinline__ void dist_setup_shared(uint8_t* aux, const DistParams
     }
 }
 
-// Epilogue shared by all consumers.  KMAX is a compile-time bound so that acc[] and thr[] are
-// indexed by constants (a runtime-indexed acc[] would be demoted to local memory).
-template <int KMAX>
-__device__ __forceinline__ void dist_finish(const DistParams& p, const double (&acc)[KMAX], int K,
-                                            int64_t row, int64_t B, int lane) {
+// The acceptance epilogue of every distance kernel: store the row's K distances, compare each
+// with its threshold, ballot, lane 0 writes the warp's mask word.  `column(k)` turns the caller's
+// accumulator k into the finished distance; it runs for rows < B only.
+// KMAX is a compile-time bound so that the caller's acc[] and thr[] are indexed by constants (a
+// runtime-indexed acc[] would be demoted to local memory); with KMAX = 0 the loop runs to K
+// instead, for a caller that computes a whole column inside `column`.
+// WHOLE_WARP: row-stream consumers run full warps over zero-filled tiles and always own their
+// mask word; a thread-per-row grid may end in a warp that starts at or beyond B and owns none.
+template <bool WHOLE_WARP, int KMAX, class Column>
+__device__ __forceinline__ void dist_record(const DistParams& p, int K, int64_t row, int64_t B,
+                                            int lane, Column column) {
     bool ok = row < B;
     if (ok) {
 #pragma unroll
-        for (int k = 0; k < KMAX; ++k) {
+        for (int k = 0; k < (KMAX ? KMAX : K); ++k) {
             if (k < K) {
-                const double d = sqrt(acc[k]);
+                const double d = column(k);
                 p.d_out[row * K + k] = d;
                 if (p.has_thr) ok = ok && (d <= p.threshold(k));
             }
@@ -71,8 +80,15 @@ __device__ __forceinline__ void dist_finish(const DistParams& p, const double (&
     }
     if (p.mask != nullptr) {
         const uint32_t bits = __ballot_sync(0xffffffffu, ok && p.has_thr);
-        if (lane == 0) p.mask[row >> 5] = bits;
+        if (lane == 0 && (WHOLE_WARP || (row - lane) < B)) p.mask[row >> 5] = bits;
     }
+}
+
+// Euclidean finish of the row-stream consumers: the root of each of the K sums.
+template <int KMAX>
+__device__ __forceinline__ void dist_finish(const DistParams& p, const double (&acc)[KMAX], int K,
+                                            int64_t row, int64_t B, int lane) {
+    dist_record<true, KMAX>(p, K, row, B, lane, [&](int k) { return sqrt(acc[k]); });
 }
 
 // K = 1, unweighted: the headline kernel (config #2: 1e6 x 128).
@@ -121,6 +137,7 @@ struct WeightedConsumer {
     }
     __device__ WeightedConsumer(const Params& p_, const uint8_t* aux, int D, int)
         : p(p_), obs_s(reinterpret_cast<const double*>(aux)), acc(0.0) {
+        // spelled out: behind rs_padded_cols() the same offset compiles to other machine code
         w_s = obs_s + ((D + RS_BOX_COLS - 1) / RS_BOX_COLS) * RS_BOX_COLS;
     }
     __device__ __forceinline__ void begin_row() { acc = 0.0; }
@@ -161,7 +178,7 @@ struct NestedConsumer {
     }
     __device__ NestedConsumer(const Params& p_, const uint8_t* aux, int D, int)
         : p(p_), obs_s(reinterpret_cast<const double*>(aux)) {
-        Dp = ((D + RS_BOX_COLS - 1) / RS_BOX_COLS) * RS_BOX_COLS;
+        Dp = rs_padded_cols(D);
         w_s = obs_s + Dp;
 #pragma unroll
         for (int k = 0; k < KMAX; ++k) acc[k] = 0.0;
@@ -224,7 +241,7 @@ struct NestedMomentsConsumer : NestedConsumer<KMAX> {
     }
     static __device__ void setup_shared(uint8_t* aux, const Params& p, int D) {
         dist_setup_shared(aux, p, D, true);
-        const int Dp = ((D + RS_BOX_COLS - 1) / RS_BOX_COLS) * RS_BOX_COLS;
+        const int Dp = rs_padded_cols(D);
         double* shift = reinterpret_cast<double*>(aux) + size_t(1 + p.K) * Dp;
         for (int j = threadIdx.x; j < Dp; j += blockDim.x) shift[j] = j < D ? p.shift_src[j] : 0.0;
         double* acc = shift + Dp;
@@ -324,7 +341,7 @@ static int fused_moments_warps(elfi_b200_ctx* ctx, int64_t Dp, int64_t K) {
 template <int KMAX>
 static int launch_nested_moments(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
                                  int64_t D, DistParams p, double* moments, cudaStream_t stream) {
-    const int64_t Dp = ((D + RS_BOX_COLS - 1) / RS_BOX_COLS) * RS_BOX_COLS;
+    const int64_t Dp = rs_padded_cols(D);
     const int warps = fused_moments_warps<KMAX>(ctx, Dp, p.K);
     const size_t aux = NestedMomentsConsumer<KMAX>::aux_bytes(Dp, p.K, warps);
     const int64_t ntiles = (B + RS_BOX_ROWS - 1) / RS_BOX_ROWS;
@@ -352,34 +369,23 @@ static int launch_nested_moments(elfi_b200_ctx* ctx, const double* S, int64_t ld
 __global__ void __launch_bounds__(256)
 dist_direct_kernel(const double* __restrict__ S, int64_t ld, int64_t B, int D, DistParams p) {
     const int64_t row = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-    const int lane = threadIdx.x & 31;
-    const int K = p.K;
-    bool ok = row < B;
-    if (ok) {
+    dist_record<false, 0>(p, p.K, row, B, threadIdx.x & 31, [&](int k) {
         const double* r = S + row * ld;
-        for (int k = 0; k < K; ++k) {
-            double acc = 0.0;
-            if (p.W != nullptr) {
-                const double* w = p.W + size_t(k) * D;
-                for (int j = 0; j < D; ++j) {
-                    const double d = __dsub_rn(__ldg(r + j), __ldg(p.obs + j));
-                    acc = __dadd_rn(acc, __dmul_rn(__ldg(w + j), __dmul_rn(d, d)));
-                }
-            } else {
-                for (int j = 0; j < D; ++j) {
-                    const double d = __dsub_rn(__ldg(r + j), __ldg(p.obs + j));
-                    acc = __dadd_rn(acc, __dmul_rn(d, d));
-                }
+        double acc = 0.0;
+        if (p.W != nullptr) {
+            const double* w = p.W + size_t(k) * D;
+            for (int j = 0; j < D; ++j) {
+                const double d = __dsub_rn(__ldg(r + j), __ldg(p.obs + j));
+                acc = __dadd_rn(acc, __dmul_rn(__ldg(w + j), __dmul_rn(d, d)));
             }
-            const double dist = sqrt(acc);
-            p.d_out[row * K + k] = dist;
-            if (p.has_thr) ok = ok && (dist <= p.threshold(k));
+        } else {
+            for (int j = 0; j < D; ++j) {
+                const double d = __dsub_rn(__ldg(r + j), __ldg(p.obs + j));
+                acc = __dadd_rn(acc, __dmul_rn(d, d));
+            }
         }
-    }
-    if (p.mask != nullptr) {
-        const uint32_t bits = __ballot_sync(0xffffffffu, ok && p.has_thr);
-        if (lane == 0 && (row - lane) < B) p.mask[row >> 5] = bits;
-    }
+        return sqrt(acc);
+    });
 }
 
 // Mask words -> ascending accepted row indices.  CTA b owns words [b*1024, (b+1)*1024):
@@ -454,13 +460,12 @@ int launch_compact_mask(const uint32_t* mask, int64_t B, int32_t* idx, int64_t* 
     return ELFI_B200_OK;
 }
 
-// Distances (+ mask when thresholds are given) for a device-resident matrix.
-int launch_dist(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B, int64_t D,
-                const double* obs, const double* W, int64_t K, const double* thr_host,
-                double* d_out, uint32_t* mask, cudaStream_t stream,
-                const double* thr_dev = nullptr) {
-    DistParams p;
-    memset(&p, 0, sizeof(p));
+// The kernel parameters of one call.  Thresholds come from the host (copied into thr[]), stay on
+// the device, or there are none.
+static DistParams dist_params(const double* obs, const double* W, int64_t K,
+                              const double* thr_host, const double* thr_dev, double* d_out,
+                              uint32_t* mask) {
+    DistParams p = {};
     p.obs = obs;
     p.W = W;
     p.d_out = d_out;
@@ -470,24 +475,27 @@ int launch_dist(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B, int
     p.thr_dev = thr_dev;
     if (thr_host)
         for (int k = 0; k < K; ++k) p.thr[k] = thr_host[k];
-    if (B == 0) return ELFI_B200_OK;
+    return p;
+}
 
-    const int64_t Dp = ((D + RS_BOX_COLS - 1) / RS_BOX_COLS) * RS_BOX_COLS;
-    const bool use_tma = D >= RS_BOX_COLS && tma_compatible(S, ldS);
-    if (use_tma) {
-        const size_t aux = size_t(Dp) * 8 * (W ? (1 + K) : 1);
-        if (rs_pick_stages(ctx->smem_optin, aux) >= 2) {
-            if (W == nullptr) return rowstream_launch<EuclidConsumer>(ctx, S, ldS, B, D, aux, p, stream);
-            if (K == 1) return rowstream_launch<WeightedConsumer>(ctx, S, ldS, B, D, aux, p, stream);
-            if (K <= 2) return rowstream_launch<NestedConsumer<2>>(ctx, S, ldS, B, D, aux, p, stream);
-            if (K <= 3) return rowstream_launch<NestedConsumer<3>>(ctx, S, ldS, B, D, aux, p, stream);
-            if (K <= 4) return rowstream_launch<NestedConsumer<4>>(ctx, S, ldS, B, D, aux, p, stream);
-            if (K <= 5) return rowstream_launch<NestedConsumer<5>>(ctx, S, ldS, B, D, aux, p, stream);
-            if (K <= 6) return rowstream_launch<NestedConsumer<6>>(ctx, S, ldS, B, D, aux, p, stream);
-            if (K <= 8) return rowstream_launch<NestedConsumer<8>>(ctx, S, ldS, B, D, aux, p, stream);
-            if (K <= 16) return rowstream_launch<NestedConsumer<16>>(ctx, S, ldS, B, D, aux, p, stream);
-            return rowstream_launch<NestedConsumer<32>>(ctx, S, ldS, B, D, aux, p, stream);
-        }
+// Distances (+ mask when thresholds are given) for a device-resident matrix.
+int launch_dist(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B, int64_t D,
+                const DistParams& p, cudaStream_t stream) {
+    if (B == 0) return ELFI_B200_OK;
+    const double* W = p.W;
+    const int K = p.K;
+    const size_t aux = size_t(rs_padded_cols(D)) * 8 * (W ? (1 + K) : 1);
+    if (rs_streams(ctx, S, ldS, D, aux)) {
+        if (W == nullptr) return rowstream_launch<EuclidConsumer>(ctx, S, ldS, B, D, aux, p, stream);
+        if (K == 1) return rowstream_launch<WeightedConsumer>(ctx, S, ldS, B, D, aux, p, stream);
+        if (K <= 2) return rowstream_launch<NestedConsumer<2>>(ctx, S, ldS, B, D, aux, p, stream);
+        if (K <= 3) return rowstream_launch<NestedConsumer<3>>(ctx, S, ldS, B, D, aux, p, stream);
+        if (K <= 4) return rowstream_launch<NestedConsumer<4>>(ctx, S, ldS, B, D, aux, p, stream);
+        if (K <= 5) return rowstream_launch<NestedConsumer<5>>(ctx, S, ldS, B, D, aux, p, stream);
+        if (K <= 6) return rowstream_launch<NestedConsumer<6>>(ctx, S, ldS, B, D, aux, p, stream);
+        if (K <= 8) return rowstream_launch<NestedConsumer<8>>(ctx, S, ldS, B, D, aux, p, stream);
+        if (K <= 16) return rowstream_launch<NestedConsumer<16>>(ctx, S, ldS, B, D, aux, p, stream);
+        return rowstream_launch<NestedConsumer<32>>(ctx, S, ldS, B, D, aux, p, stream);
     }
     const unsigned blocks = unsigned((B + 255) / 256);
     dist_direct_kernel<<<blocks, 256, 0, stream>>>(S, ldS, B, int(D), p);
@@ -506,6 +514,11 @@ struct MetricParams : DistParams {
     const double* V;   // (D) component variances of 'seuclidean', else nullptr
 };
 
+// 'seuclidean' is a fifth metric inside this file only: it has an entry point of its own
+// (elfi_b200_dist_seuclidean_thr_f64, because of V), and elfi_b200_dist_metric_thr_f64 keeps
+// rejecting every code beyond ELFI_B200_METRIC_MINKOWSKI.
+constexpr int METRIC_SEUCLIDEAN = ELFI_B200_METRIC_MINKOWSKI + 1;
+
 template <int METRIC>
 __device__ __forceinline__ double metric_term(double acc, double d, double pexp) {
     if (METRIC == ELFI_B200_METRIC_SQEUCLIDEAN) return __dadd_rn(acc, __dmul_rn(d, d));
@@ -520,24 +533,10 @@ __device__ __forceinline__ double metric_value(double acc, double pexp) {
 }
 
 template <int METRIC>
-__device__ __forceinline__ void metric_finish(const MetricParams& p, double acc, int64_t row,
-                                              int64_t B, int lane, bool whole_warp) {
-    bool ok = row < B;
-    if (ok) {
-        const double d = metric_value<METRIC>(acc, p.pexp);
-        p.d_out[row] = d;
-        if (p.has_thr) ok = d <= p.threshold(0);
-    }
-    if (p.mask != nullptr) {
-        const uint32_t bits = __ballot_sync(0xffffffffu, ok && p.has_thr);
-        if (lane == 0 && (whole_warp || (row - lane) < B)) p.mask[row >> 5] = bits;
-    }
-}
-
-template <int METRIC>
 struct MetricConsumer {
     typedef MetricParams Params;
     static constexpr int PASSES = 1;
+    static constexpr int AUX_ROWS = 1;   // padded rows of shared memory: obs
     const Params& p;
     const double* obs_s;
     double acc;
@@ -559,7 +558,8 @@ struct MetricConsumer {
         }
     }
     __device__ __forceinline__ void end_row(int64_t row, int64_t B, int lane) {
-        metric_finish<METRIC>(p, acc, row, B, lane, true);
+        dist_record<true, 1>(p, 1, row, B, lane,
+                             [&](int) { return metric_value<METRIC>(acc, p.pexp); });
     }
 };
 
@@ -567,50 +567,13 @@ template <int METRIC>
 __global__ void __launch_bounds__(256)
 metric_direct_kernel(const double* __restrict__ S, int64_t ld, int64_t B, int D, MetricParams p) {
     const int64_t row = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-    double acc = 0.0;
-    if (row < B) {
+    dist_record<false, 1>(p, 1, row, B, threadIdx.x & 31, [&](int) {
         const double* r = S + row * ld;
+        double acc = 0.0;
         for (int j = 0; j < D; ++j)
             acc = metric_term<METRIC>(acc, __dsub_rn(__ldg(r + j), __ldg(p.obs + j)), p.pexp);
-    }
-    metric_finish<METRIC>(p, acc, row, B, threadIdx.x & 31, false);
-}
-
-template <int METRIC>
-static int launch_metric_t(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B, int64_t D,
-                           const MetricParams& p, cudaStream_t stream) {
-    const int64_t Dp = ((D + RS_BOX_COLS - 1) / RS_BOX_COLS) * RS_BOX_COLS;
-    const size_t aux = size_t(Dp) * 8;
-    if (D >= RS_BOX_COLS && tma_compatible(S, ldS) && rs_pick_stages(ctx->smem_optin, aux) >= 2)
-        return rowstream_launch<MetricConsumer<METRIC>>(ctx, S, ldS, B, D, aux, p, stream);
-    metric_direct_kernel<METRIC><<<unsigned((B + 255) / 256), 256, 0, stream>>>(S, ldS, B, int(D), p);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
-}
-
-static int launch_metric(elfi_b200_ctx* ctx, int metric, double pexp, const double* S, int64_t ldS,
-                         int64_t B, int64_t D, const double* obs, const double* thr_host,
-                         double* d_out, uint32_t* mask, cudaStream_t stream) {
-    MetricParams p;
-    memset(&p, 0, sizeof(p));
-    p.obs = obs;
-    p.d_out = d_out;
-    p.mask = mask;
-    p.K = 1;
-    p.has_thr = thr_host != nullptr;
-    if (thr_host) p.thr[0] = thr_host[0];
-    p.pexp = pexp;
-    if (B == 0) return ELFI_B200_OK;
-    switch (metric) {
-        case ELFI_B200_METRIC_SQEUCLIDEAN:
-            return launch_metric_t<ELFI_B200_METRIC_SQEUCLIDEAN>(ctx, S, ldS, B, D, p, stream);
-        case ELFI_B200_METRIC_CITYBLOCK:
-            return launch_metric_t<ELFI_B200_METRIC_CITYBLOCK>(ctx, S, ldS, B, D, p, stream);
-        case ELFI_B200_METRIC_CHEBYSHEV:
-            return launch_metric_t<ELFI_B200_METRIC_CHEBYSHEV>(ctx, S, ldS, B, D, p, stream);
-        default:
-            return launch_metric_t<ELFI_B200_METRIC_MINKOWSKI>(ctx, S, ldS, B, D, p, stream);
-    }
+        return metric_value<METRIC>(acc, p.pexp);
+    });
 }
 
 // 'seuclidean' (cdist(..., 'seuclidean', V=V)): SciPy 1.18's compiled loop keeps TWO running sums,
@@ -649,22 +612,11 @@ __device__ __forceinline__ double seuclid_term(double x, double o, double v) {
     return __ddiv_rn(__dmul_rn(d, d), v);
 }
 
-__device__ __forceinline__ void seuclid_finish(const MetricParams& p, double dist, int64_t row,
-                                               int64_t B, int lane, bool whole_warp) {
-    bool ok = row < B;
-    if (ok) {
-        p.d_out[row] = dist;
-        if (p.has_thr) ok = dist <= p.threshold(0);
-    }
-    if (p.mask != nullptr) {
-        const uint32_t bits = __ballot_sync(0xffffffffu, ok && p.has_thr);
-        if (lane == 0 && (whole_warp || (row - lane) < B)) p.mask[row >> 5] = bits;
-    }
-}
-
-struct SeuclidConsumer {
+template <>
+struct MetricConsumer<METRIC_SEUCLIDEAN> {
     typedef MetricParams Params;
     static constexpr int PASSES = 1;
+    static constexpr int AUX_ROWS = 2;   // obs, V
     const Params& p;
     const double* obs_s;
     const double* v_s;
@@ -672,16 +624,16 @@ struct SeuclidConsumer {
     SeuclidTerm acc;
 
     static __device__ void setup_shared(uint8_t* aux, const Params& p, int D) {
-        const int Dp = ((D + RS_BOX_COLS - 1) / RS_BOX_COLS) * RS_BOX_COLS;
+        const int Dp = rs_padded_cols(D);
         double* obs_s = reinterpret_cast<double*>(aux);
         for (int j = threadIdx.x; j < Dp; j += blockDim.x) {
             obs_s[j] = j < D ? p.obs[j] : 0.0;
             obs_s[Dp + j] = j < D ? p.V[j] : 1.0;
         }
     }
-    __device__ SeuclidConsumer(const Params& p_, const uint8_t* aux, int D_, int)
+    __device__ MetricConsumer(const Params& p_, const uint8_t* aux, int D_, int)
         : p(p_), obs_s(reinterpret_cast<const double*>(aux)), D(D_) {
-        v_s = obs_s + ((D + RS_BOX_COLS - 1) / RS_BOX_COLS) * RS_BOX_COLS;
+        v_s = obs_s + rs_padded_cols(D);
         acc.begin(D);
     }
     __device__ __forceinline__ void begin_row() { acc.begin(D); }
@@ -698,47 +650,57 @@ struct SeuclidConsumer {
         }
     }
     __device__ __forceinline__ void end_row(int64_t row, int64_t B, int lane) {
-        seuclid_finish(p, acc.value(), row, B, lane, true);
+        dist_record<true, 1>(p, 1, row, B, lane, [&](int) { return acc.value(); });
     }
 };
 
+template <>
 __global__ void __launch_bounds__(256)
-seuclid_direct_kernel(const double* __restrict__ S, int64_t ld, int64_t B, int D, MetricParams p) {
+metric_direct_kernel<METRIC_SEUCLIDEAN>(const double* __restrict__ S, int64_t ld, int64_t B, int D,
+                                        MetricParams p) {
     const int64_t row = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-    SeuclidTerm acc;
-    acc.begin(D);
-    if (row < B) {
+    dist_record<false, 1>(p, 1, row, B, threadIdx.x & 31, [&](int) {
         const double* r = S + row * ld;
+        SeuclidTerm acc;
+        acc.begin(D);
         for (int j = 0; j < D; j += 2) {
             const double t0 = seuclid_term(__ldg(r + j), __ldg(p.obs + j), __ldg(p.V + j));
             const double t1 = j + 1 < D
                 ? seuclid_term(__ldg(r + j + 1), __ldg(p.obs + j + 1), __ldg(p.V + j + 1)) : 0.0;
             acc.pair(j, t0, t1);
         }
-    }
-    seuclid_finish(p, acc.value(), row, B, threadIdx.x & 31, false);
+        return acc.value();
+    });
 }
 
-static int launch_seuclid(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B, int64_t D,
-                          const double* obs, const double* V, const double* thr_host,
-                          double* d_out, uint32_t* mask, cudaStream_t stream) {
-    MetricParams p;
-    memset(&p, 0, sizeof(p));
-    p.obs = obs;
-    p.V = V;
-    p.d_out = d_out;
-    p.mask = mask;
-    p.K = 1;
-    p.has_thr = thr_host != nullptr;
-    if (thr_host) p.thr[0] = thr_host[0];
-    if (B == 0) return ELFI_B200_OK;
-    const int64_t Dp = ((D + RS_BOX_COLS - 1) / RS_BOX_COLS) * RS_BOX_COLS;
-    const size_t aux = size_t(Dp) * 8 * 2;
-    if (D >= RS_BOX_COLS && tma_compatible(S, ldS) && rs_pick_stages(ctx->smem_optin, aux) >= 2)
-        return rowstream_launch<SeuclidConsumer>(ctx, S, ldS, B, D, aux, p, stream);
-    seuclid_direct_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(S, ldS, B, int(D), p);
+// One column of any metric: the row stream when the matrix takes it, else a thread per row.
+template <int METRIC>
+static int launch_metric_t(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B, int64_t D,
+                           const MetricParams& p, cudaStream_t stream) {
+    typedef MetricConsumer<METRIC> Consumer;
+    const size_t aux = size_t(rs_padded_cols(D)) * 8 * Consumer::AUX_ROWS;
+    if (rs_streams(ctx, S, ldS, D, aux))
+        return rowstream_launch<Consumer>(ctx, S, ldS, B, D, aux, p, stream);
+    metric_direct_kernel<METRIC><<<unsigned((B + 255) / 256), 256, 0, stream>>>(S, ldS, B, int(D), p);
     ELFI_CUDA_OK(cudaGetLastError());
     return ELFI_B200_OK;
+}
+
+static int launch_metric(elfi_b200_ctx* ctx, int metric, const double* S, int64_t ldS, int64_t B,
+                         int64_t D, const MetricParams& p, cudaStream_t stream) {
+    if (B == 0) return ELFI_B200_OK;
+    switch (metric) {
+        case ELFI_B200_METRIC_SQEUCLIDEAN:
+            return launch_metric_t<ELFI_B200_METRIC_SQEUCLIDEAN>(ctx, S, ldS, B, D, p, stream);
+        case ELFI_B200_METRIC_CITYBLOCK:
+            return launch_metric_t<ELFI_B200_METRIC_CITYBLOCK>(ctx, S, ldS, B, D, p, stream);
+        case ELFI_B200_METRIC_CHEBYSHEV:
+            return launch_metric_t<ELFI_B200_METRIC_CHEBYSHEV>(ctx, S, ldS, B, D, p, stream);
+        case ELFI_B200_METRIC_MINKOWSKI:
+            return launch_metric_t<ELFI_B200_METRIC_MINKOWSKI>(ctx, S, ldS, B, D, p, stream);
+        default:
+            return launch_metric_t<METRIC_SEUCLIDEAN>(ctx, S, ldS, B, D, p, stream);
+    }
 }
 
 static int check_dist_args(const void* S, int64_t ldS, int64_t B, int64_t D, const void* obs,
@@ -755,6 +717,33 @@ static int check_dist_args(const void* S, int64_t ldS, int64_t B, int64_t D, con
     return ELFI_B200_OK;
 }
 
+// The skeleton of the entry points over a device-resident matrix: check the arguments, take the
+// mask from the scratch arena when there are thresholds (on the host or on the device),
+// `launch(params, stream)` the distance kernel, compact the mask when indices or their count
+// are asked for.  `who` names the entry point in its own messages.
+template <class Launch>
+static int dist_call(const char* who, elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
+                     int64_t D, const double* obs, const double* W, int64_t K,
+                     const double* thr_host, const double* thr_dev, double* d_out,
+                     int32_t* acc_idx, int64_t* n_acc, void* stream_, Launch launch) {
+    const double* thr = thr_host ? thr_host : thr_dev;
+    int rc = check_dist_args(S, ldS, B, D, obs, W, K, thr, acc_idx);
+    if (rc) return rc;
+    ELFI_REQUIRE(B == 0 || d_out != nullptr, "%s: d_out is NULL", who);
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
+    uint32_t* mask = nullptr;
+    if (thr != nullptr) {
+        mask = static_cast<uint32_t*>(ctx_scratch(ctx, size_t((B + 31) / 32) * 4 + 256));
+        if (!mask) return ELFI_B200_ERR_NOMEM;
+    }
+    rc = launch(dist_params(obs, W, K, thr_host, thr_dev, d_out, mask), stream);
+    if (rc) return rc;
+    if (thr != nullptr && (acc_idx != nullptr || n_acc != nullptr))
+        return launch_compact_mask(mask, B, acc_idx, n_acc, stream);
+    return ELFI_B200_OK;
+}
+
 }  // namespace elfi
 
 extern "C" {
@@ -765,22 +754,10 @@ int elfi_b200_dist_euclid_thr_f64(elfi_b200_ctx* ctx, const double* S, int64_t l
                                   int64_t* n_acc, void* stream_) {
     using namespace elfi;
     ELFI_REQUIRE(ctx != nullptr, "dist: ctx is NULL");
-    int rc = check_dist_args(S, ldS, B, D, obs, W, K, thr_host, acc_idx);
-    if (rc) return rc;
-    ELFI_REQUIRE(B == 0 || d_out != nullptr, "dist: d_out is NULL");
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    uint32_t* mask = nullptr;
-    if (thr_host != nullptr) {
-        const size_t nwords = size_t((B + 31) / 32);
-        mask = static_cast<uint32_t*>(ctx_scratch(ctx, nwords * 4 + 256));
-        if (!mask) return ELFI_B200_ERR_NOMEM;
-    }
-    rc = launch_dist(ctx, S, ldS, B, D, obs, W, K, thr_host, d_out, mask, stream);
-    if (rc) return rc;
-    if (thr_host != nullptr && (acc_idx != nullptr || n_acc != nullptr))
-        return launch_compact_mask(mask, B, acc_idx, n_acc, stream);
-    return ELFI_B200_OK;
+    return dist_call("dist", ctx, S, ldS, B, D, obs, W, K, thr_host, nullptr, d_out, acc_idx, n_acc,
+                     stream_, [&](const DistParams& p, cudaStream_t stream) {
+                         return launch_dist(ctx, S, ldS, B, D, p, stream);
+                     });
 }
 
 int elfi_b200_dist_euclid_thr_dev_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
@@ -789,19 +766,10 @@ int elfi_b200_dist_euclid_thr_dev_f64(elfi_b200_ctx* ctx, const double* S, int64
                                       int64_t* n_acc, void* stream_) {
     using namespace elfi;
     ELFI_REQUIRE(ctx != nullptr && thr_dev != nullptr, "dist: ctx or thr_dev is NULL");
-    int rc = check_dist_args(S, ldS, B, D, obs, W, K, thr_dev, acc_idx);
-    if (rc) return rc;
-    ELFI_REQUIRE(B == 0 || d_out != nullptr, "dist: d_out is NULL");
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    const size_t nwords = size_t((B + 31) / 32);
-    uint32_t* mask = static_cast<uint32_t*>(ctx_scratch(ctx, nwords * 4 + 256));
-    if (!mask) return ELFI_B200_ERR_NOMEM;
-    rc = launch_dist(ctx, S, ldS, B, D, obs, W, K, nullptr, d_out, mask, stream, thr_dev);
-    if (rc) return rc;
-    if (acc_idx != nullptr || n_acc != nullptr)
-        return launch_compact_mask(mask, B, acc_idx, n_acc, stream);
-    return ELFI_B200_OK;
+    return dist_call("dist", ctx, S, ldS, B, D, obs, W, K, nullptr, thr_dev, d_out, acc_idx, n_acc,
+                     stream_, [&](const DistParams& p, cudaStream_t stream) {
+                         return launch_dist(ctx, S, ldS, B, D, p, stream);
+                     });
 }
 
 int elfi_b200_dist_euclid_mom_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
@@ -818,48 +786,35 @@ int elfi_b200_dist_euclid_mom_f64(elfi_b200_ctx* ctx, const double* S, int64_t l
     ELFI_REQUIRE(B >= 1 && d_out != nullptr, "dist_mom: needs at least one row and d_out");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    const int64_t Dp = ((D + RS_BOX_COLS - 1) / RS_BOX_COLS) * RS_BOX_COLS;
-    const size_t aux = NestedMomentsConsumer<2>::aux_bytes(Dp, K);
-    const bool fused = W != nullptr && D >= RS_BOX_COLS && tma_compatible(S, ldS) &&
-                       rs_pick_stages(ctx->smem_optin, aux) >= 2;
+    const size_t aux = NestedMomentsConsumer<2>::aux_bytes(rs_padded_cols(D), K);
+    const bool fused = W != nullptr && rs_streams(ctx, S, ldS, D, aux);
+    // the mask and the per-warp partial sums in ONE request: a second one may grow the arena and
+    // move the first
     const size_t mask_bytes = (size_t((B + 31) / 32) * 4 + 255) & ~size_t(255);
     const size_t part_bytes = fused ? size_t(ctx->sm_count) * 16 * 2 * D * 8 : 0;   // <= 16 warps
     uint8_t* base = static_cast<uint8_t*>(ctx_scratch(ctx, mask_bytes + part_bytes + 256));
     if (!base) return ELFI_B200_ERR_NOMEM;
     uint32_t* mask = thr ? reinterpret_cast<uint32_t*>(base) : nullptr;
-    if (!fused) {
-        // narrow / unaligned / unweighted matrices: distances, then the stand-alone moments pass
-        rc = launch_dist(ctx, S, ldS, B, D, obs, W, K, thr_host, d_out, mask, stream, thr_dev);
-        if (rc) return rc;
-        if (thr && (acc_idx != nullptr || n_acc != nullptr)) {
-            rc = launch_compact_mask(mask, B, acc_idx, n_acc, stream);
-            if (rc) return rc;
-        }
-        return elfi_b200_colmoments_f64(ctx, S, ldS, B, D, moments, stream_);
+    DistParams p = dist_params(obs, W, K, thr_host, thr_dev, d_out, mask);
+    if (fused) {
+        p.shift_src = S;
+        p.mom_partial = reinterpret_cast<double*>(base + mask_bytes);
+        if (K <= 2) rc = launch_nested_moments<2>(ctx, S, ldS, B, D, p, moments, stream);
+        else if (K <= 4) rc = launch_nested_moments<4>(ctx, S, ldS, B, D, p, moments, stream);
+        else if (K <= 6) rc = launch_nested_moments<6>(ctx, S, ldS, B, D, p, moments, stream);
+        else if (K <= 8) rc = launch_nested_moments<8>(ctx, S, ldS, B, D, p, moments, stream);
+        else if (K <= 16) rc = launch_nested_moments<16>(ctx, S, ldS, B, D, p, moments, stream);
+        else rc = launch_nested_moments<32>(ctx, S, ldS, B, D, p, moments, stream);
+    } else {
+        rc = launch_dist(ctx, S, ldS, B, D, p, stream);
     }
-    DistParams p;
-    memset(&p, 0, sizeof(p));
-    p.obs = obs;
-    p.W = W;
-    p.d_out = d_out;
-    p.mask = mask;
-    p.K = int(K);
-    p.has_thr = thr != nullptr;
-    p.thr_dev = thr_dev;
-    if (thr_host)
-        for (int k = 0; k < K; ++k) p.thr[k] = thr_host[k];
-    p.shift_src = S;
-    p.mom_partial = reinterpret_cast<double*>(base + mask_bytes);
-    if (K <= 2) rc = launch_nested_moments<2>(ctx, S, ldS, B, D, p, moments, stream);
-    else if (K <= 4) rc = launch_nested_moments<4>(ctx, S, ldS, B, D, p, moments, stream);
-    else if (K <= 6) rc = launch_nested_moments<6>(ctx, S, ldS, B, D, p, moments, stream);
-    else if (K <= 8) rc = launch_nested_moments<8>(ctx, S, ldS, B, D, p, moments, stream);
-    else if (K <= 16) rc = launch_nested_moments<16>(ctx, S, ldS, B, D, p, moments, stream);
-    else rc = launch_nested_moments<32>(ctx, S, ldS, B, D, p, moments, stream);
     if (rc) return rc;
-    if (thr && (acc_idx != nullptr || n_acc != nullptr))
-        return launch_compact_mask(mask, B, acc_idx, n_acc, stream);
-    return ELFI_B200_OK;
+    if (thr && (acc_idx != nullptr || n_acc != nullptr)) {
+        rc = launch_compact_mask(mask, B, acc_idx, n_acc, stream);
+        if (rc) return rc;
+    }
+    // narrow / unaligned / unweighted matrices: the stand-alone moments pass after the distances
+    return fused ? ELFI_B200_OK : elfi_b200_colmoments_f64(ctx, S, ldS, B, D, moments, stream_);
 }
 
 int elfi_b200_dist_euclid_thr_f64_host(elfi_b200_ctx* ctx, const double* S_host, int64_t ldS,
@@ -926,8 +881,9 @@ int elfi_b200_dist_euclid_thr_f64_host(elfi_b200_ctx* ctx, const double* S_host,
                                            size_t(ldS) * 8, size_t(row_bytes), size_t(rows),
                                            cudaMemcpyHostToDevice, st));
         }
-        rc = launch_dist(ctx, chunk[which], D, rows, D, obs_d, w_d, K, thr_host, d_d + r0 * K,
-                         mask_d ? mask_d + r0 / 32 : nullptr, st);
+        rc = launch_dist(ctx, chunk[which], D, rows, D,
+                         dist_params(obs_d, w_d, K, thr_host, nullptr, d_d + r0 * K,
+                                     mask_d ? mask_d + r0 / 32 : nullptr), st);
         if (rc) return rc;
     }
     // join s1 into s0, compact, copy back
@@ -963,21 +919,11 @@ int elfi_b200_dist_metric_thr_f64(elfi_b200_ctx* ctx, int32_t metric, double pex
                  "dist_metric: unknown metric code %d", int(metric));
     ELFI_REQUIRE(metric != ELFI_B200_METRIC_MINKOWSKI || (pexp > 0.0 && pexp < 1e308),
                  "dist_metric: Minkowski exponent must be positive and finite");
-    int rc = check_dist_args(S, ldS, B, D, obs, nullptr, 1, thr_host, acc_idx);
-    if (rc) return rc;
-    ELFI_REQUIRE(B == 0 || d_out != nullptr, "dist_metric: d_out is NULL");
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    uint32_t* mask = nullptr;
-    if (thr_host != nullptr) {
-        mask = static_cast<uint32_t*>(ctx_scratch(ctx, size_t((B + 31) / 32) * 4 + 256));
-        if (!mask) return ELFI_B200_ERR_NOMEM;
-    }
-    rc = launch_metric(ctx, int(metric), pexp, S, ldS, B, D, obs, thr_host, d_out, mask, stream);
-    if (rc) return rc;
-    if (thr_host != nullptr && (acc_idx != nullptr || n_acc != nullptr))
-        return launch_compact_mask(mask, B, acc_idx, n_acc, stream);
-    return ELFI_B200_OK;
+    return dist_call("dist_metric", ctx, S, ldS, B, D, obs, nullptr, 1, thr_host, nullptr, d_out,
+                     acc_idx, n_acc, stream_, [&](const DistParams& p, cudaStream_t stream) {
+                         return launch_metric(ctx, int(metric), S, ldS, B, D,
+                                              MetricParams{p, pexp, nullptr}, stream);
+                     });
 }
 
 int elfi_b200_dist_seuclidean_thr_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
@@ -987,21 +933,11 @@ int elfi_b200_dist_seuclidean_thr_f64(elfi_b200_ctx* ctx, const double* S, int64
     using namespace elfi;
     ELFI_REQUIRE(ctx != nullptr, "dist_seuclidean: ctx is NULL");
     ELFI_REQUIRE(V != nullptr, "dist_seuclidean: V is NULL");
-    int rc = check_dist_args(S, ldS, B, D, obs, nullptr, 1, thr_host, acc_idx);
-    if (rc) return rc;
-    ELFI_REQUIRE(B == 0 || d_out != nullptr, "dist_seuclidean: d_out is NULL");
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    uint32_t* mask = nullptr;
-    if (thr_host != nullptr) {
-        mask = static_cast<uint32_t*>(ctx_scratch(ctx, size_t((B + 31) / 32) * 4 + 256));
-        if (!mask) return ELFI_B200_ERR_NOMEM;
-    }
-    rc = launch_seuclid(ctx, S, ldS, B, D, obs, V, thr_host, d_out, mask, stream);
-    if (rc) return rc;
-    if (thr_host != nullptr && (acc_idx != nullptr || n_acc != nullptr))
-        return launch_compact_mask(mask, B, acc_idx, n_acc, stream);
-    return ELFI_B200_OK;
+    return dist_call("dist_seuclidean", ctx, S, ldS, B, D, obs, nullptr, 1, thr_host, nullptr,
+                     d_out, acc_idx, n_acc, stream_, [&](const DistParams& p, cudaStream_t stream) {
+                         return launch_metric(ctx, METRIC_SEUCLIDEAN, S, ldS, B, D,
+                                              MetricParams{p, 0.0, V}, stream);
+                     });
 }
 
 }  // extern "C"

@@ -52,6 +52,13 @@ constexpr int RS_BOX_COLS = 16;      // fp64 columns per box (128 bytes)
 constexpr int RS_BOX_BYTES = RS_BOX_ROWS * RS_BOX_COLS * 8;
 constexpr int RS_MAX_STAGES = 6;
 
+// D rounded up to whole boxes: the row length of everything a consumer keeps per column in
+// shared memory (TMA zero-fills the columns >= D of the last box).
+template <class Int>
+__host__ __device__ constexpr Int rs_padded_cols(Int D) {
+    return ((D + RS_BOX_COLS - 1) / RS_BOX_COLS) * RS_BOX_COLS;
+}
+
 // Shared-memory layout (dynamic, 1024-byte aligned):
 //   [RS_WARPS][ns][4096]  boxes
 //   [RS_WARPS][ns] u64    mbarriers
@@ -71,6 +78,15 @@ inline int rs_pick_stages(size_t smem_optin, size_t aux_bytes, int warps = RS_WA
     for (int ns = RS_MAX_STAGES; ns >= 2; --ns)
         if (rs_aux_offset(ns, warps) + aux_bytes + 1024 <= smem_optin) return ns;
     return 0;
+}
+
+// Does the (.., D) matrix M take the row stream with `aux_bytes` of consumer shared memory?  It
+// needs one whole box of columns, a TMA-addressable base and stride, and room for a 2-slot ring;
+// callers send every other matrix to their thread-per-row kernel.
+inline bool rs_streams(const elfi_b200_ctx* ctx, const void* M, int64_t ld, int64_t D,
+                       size_t aux_bytes) {
+    return D >= RS_BOX_COLS && tma_compatible(M, ld) &&
+           rs_pick_stages(ctx->smem_optin, aux_bytes) >= 2;
 }
 
 // The Consumer concept (all members are per lane):

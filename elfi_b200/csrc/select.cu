@@ -808,13 +808,6 @@ int elfi_b200_accept_append_f64(elfi_b200_ctx* ctx, const int32_t* acc_idx, cons
 // One batch of a threshold-mode rejection round in ONE call: distances + acceptance + compaction
 // (elfi_b200_dist_euclid_thr[_dev]_f64) and the append of the accepted rows [d | extra sources]
 // to the candidate buffer (elfi_b200_accept_append_f64); four launches, no synchronisation.
-extern "C" int elfi_b200_dist_euclid_thr_f64(elfi_b200_ctx*, const double*, int64_t, int64_t, int64_t,
-                                             const double*, const double*, int64_t, const double*,
-                                             double*, int32_t*, int64_t*, void*);
-extern "C" int elfi_b200_dist_euclid_thr_dev_f64(elfi_b200_ctx*, const double*, int64_t, int64_t,
-                                                 int64_t, const double*, const double*, int64_t,
-                                                 const double*, double*, int32_t*, int64_t*, void*);
-
 int elfi_b200_rejection_batch_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
                                   int64_t D, const double* obs, const double* W, int64_t K,
                                   const double* thr_host, const double* thr_dev, double* d_out,

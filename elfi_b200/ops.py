@@ -28,6 +28,52 @@ def _matrix(S):
     return S
 
 
+def _ld(t):
+    return t.stride(0) if t.shape[0] > 1 else t.shape[1]
+
+
+def _dist_prepare(S, obs, thresholds, K=1, want_indices=True, device_thresholds=False):
+    """What the device distance wrappers share: the matrix, ``obs`` flattened and checked against
+    its width, the K thresholds as a host float64 array (or None) -- or left as a device tensor
+    where the entry point reads them there (``device_thresholds``) -- and the outputs d (B, K),
+    acc_idx and n_acc (both None without thresholds)."""
+    S = _matrix(S)
+    B, D = S.shape
+    obs_t = dev.to_device(obs).reshape(-1)
+    if obs_t.numel() != D:
+        raise ValueError('XA and XB must have the same number of columns '
+                         '(i.e. feature dimension.)')
+    thr = None
+    if device_thresholds and dev.is_device_array(thresholds):
+        thr = thresholds.reshape(-1)
+        if thr.dtype != torch.float64 or not thr.is_contiguous():
+            thr = thr.to(torch.float64).contiguous()
+    elif thresholds is not None:
+        thr = np.ascontiguousarray(np.atleast_1d(thresholds), dtype=np.float64)
+    if thr is not None and thr.shape[0] != K:
+        raise ValueError('need one threshold per distance column ({} != {})'.format(
+            thr.shape[0], K))
+    d = dev.empty((B, K))
+    acc_idx = n_acc = None
+    if thr is not None:
+        n_acc = dev.zeros((1,), dtype=torch.int64)
+        if want_indices:
+            acc_idx = dev.empty((max(B, 1),), dtype=torch.int32)
+    return S, obs_t, thr, d, acc_idx, n_acc
+
+
+def _dist_accepted(acc_idx, n_acc, want_indices=True, sync=True):
+    """What a distance wrapper returns next to d: None without thresholds, the pair
+    (acc_idx, n_acc) left on the device when ``sync`` is False, else the accepted indices, or
+    their number when the caller did not want indices."""
+    if n_acc is None:
+        return None
+    if not sync:
+        return acc_idx, n_acc
+    n = int(n_acc.item())
+    return acc_idx[:n] if want_indices else n
+
+
 def dist_euclid(S, obs, w=None, thresholds=None, want_indices=True, sync=True, moments=False):
     """Euclidean / nested weighted distances of the rows of S to ``obs`` + acceptance.
 
@@ -52,12 +98,6 @@ def dist_euclid(S, obs, w=None, thresholds=None, want_indices=True, sync=True, m
     d : (B,) tensor if K == 1 and w was not 2-d, else (B, K)
     acc_idx : int32 tensor of accepted row indices, ascending (None without thresholds)
     """
-    S = _matrix(S)
-    B, D = S.shape
-    obs_t = dev.to_device(obs).reshape(-1)
-    if obs_t.numel() != D:
-        raise ValueError('XA and XB must have the same number of columns '
-                         '(i.e. feature dimension.)')
     squeeze = True
     W = None
     K = 1
@@ -68,45 +108,28 @@ def dist_euclid(S, obs, w=None, thresholds=None, want_indices=True, sync=True, m
         else:
             squeeze = False
         K = W.shape[0]
+    S, obs_t, thr, d, acc_idx, n_acc = _dist_prepare(S, obs, thresholds, K, want_indices,
+                                                     device_thresholds=True)
+    B, D = S.shape
+    if W is not None:
         if W.shape[1] != D:
             raise ValueError('weights must have {} columns'.format(D))
         if K > MAX_NESTED:
             raise ValueError('at most {} nested distances are supported'.format(MAX_NESTED))
-    thr = None
-    thr_on_device = dev.is_device_array(thresholds)
-    if thr_on_device:
-        thr = thresholds.reshape(-1)
-        if thr.dtype != torch.float64 or not thr.is_contiguous():
-            thr = thr.to(torch.float64).contiguous()
-    elif thresholds is not None:
-        thr = np.ascontiguousarray(np.atleast_1d(thresholds), dtype=np.float64)
-    if thr is not None and thr.shape[0] != K:
-        raise ValueError('need one threshold per distance column ({} != {})'.format(
-            thr.shape[0], K))
-    d = dev.empty((B, K))
-    acc_idx = n_acc = None
-    if thr is not None:
-        n_acc = dev.zeros((1,), dtype=torch.int64)
-        if want_indices:
-            acc_idx = dev.empty((max(B, 1),), dtype=torch.int32)
+    thr_on_device = dev.is_device_array(thr)
     mom = None
     if moments:
         mom = dev.empty((2, D))
-        _lib.call('elfi_b200_dist_euclid_mom_f64', dev.context(), dev.ptr(S),
-                  S.stride(0) if B > 1 else D, B, D, dev.ptr(obs_t), dev.ptr(W), K,
-                  None if thr_on_device else dev.ptr(thr), dev.ptr(thr) if thr_on_device else None,
-                  dev.ptr(d), dev.ptr(acc_idx), dev.ptr(n_acc), dev.ptr(mom), dev.stream_ptr())
+        _lib.call('elfi_b200_dist_euclid_mom_f64', dev.context(), dev.ptr(S), _ld(S), B, D,
+                  dev.ptr(obs_t), dev.ptr(W), K, None if thr_on_device else dev.ptr(thr),
+                  dev.ptr(thr) if thr_on_device else None, dev.ptr(d), dev.ptr(acc_idx),
+                  dev.ptr(n_acc), dev.ptr(mom), dev.stream_ptr())
     else:
         _lib.call('elfi_b200_dist_euclid_thr_dev_f64' if thr_on_device else
-                  'elfi_b200_dist_euclid_thr_f64', dev.context(), dev.ptr(S),
-                  S.stride(0) if B > 1 else D, B, D, dev.ptr(obs_t), dev.ptr(W), K, dev.ptr(thr),
-                  dev.ptr(d), dev.ptr(acc_idx), dev.ptr(n_acc), dev.stream_ptr())
-    if thr is not None:
-        if not sync:
-            acc_idx = (acc_idx, n_acc)
-        else:
-            n = int(n_acc.item())
-            acc_idx = acc_idx[:n] if want_indices else n
+                  'elfi_b200_dist_euclid_thr_f64', dev.context(), dev.ptr(S), _ld(S), B, D,
+                  dev.ptr(obs_t), dev.ptr(W), K, dev.ptr(thr), dev.ptr(d), dev.ptr(acc_idx),
+                  dev.ptr(n_acc), dev.stream_ptr())
+    acc_idx = _dist_accepted(acc_idx, n_acc, want_indices, sync)
     if squeeze:
         d = d.reshape(B)
     return (d, acc_idx, mom) if moments else (d, acc_idx)
@@ -131,64 +154,28 @@ def dist_metric(S, obs, metric, p=2.0, threshold=None, want_indices=True):
             raise ValueError('p must be greater than 0')
     if metric not in METRIC_CODES:
         raise ValueError('Unknown Distance Metric: {}'.format(metric))
-    S = _matrix(S)
+    S, obs_t, thr, d, acc_idx, n_acc = _dist_prepare(S, obs, threshold, 1, want_indices)
     B, D = S.shape
-    obs_t = dev.to_device(obs).reshape(-1)
-    if obs_t.numel() != D:
-        raise ValueError('XA and XB must have the same number of columns '
-                         '(i.e. feature dimension.)')
-    thr = None
-    if threshold is not None:
-        thr = np.ascontiguousarray(np.atleast_1d(threshold), dtype=np.float64)
-        if thr.shape[0] != 1:
-            raise ValueError('need one threshold per distance column ({} != 1)'.format(thr.shape[0]))
-    d = dev.empty((B,))
-    acc_idx = n_acc = None
-    if thr is not None:
-        n_acc = dev.zeros((1,), dtype=torch.int64)
-        if want_indices:
-            acc_idx = dev.empty((max(B, 1),), dtype=torch.int32)
     _lib.call('elfi_b200_dist_metric_thr_f64', dev.context(), METRIC_CODES[metric], float(p),
-              dev.ptr(S), S.stride(0) if B > 1 else D, B, D, dev.ptr(obs_t), dev.ptr(thr),
-              dev.ptr(d), dev.ptr(acc_idx), dev.ptr(n_acc), dev.stream_ptr())
-    if thr is not None:
-        n = int(n_acc.item())
-        acc_idx = acc_idx[:n] if want_indices else n
-    return d, acc_idx
+              dev.ptr(S), _ld(S), B, D, dev.ptr(obs_t), dev.ptr(thr), dev.ptr(d), dev.ptr(acc_idx),
+              dev.ptr(n_acc), dev.stream_ptr())
+    return d.reshape(B), _dist_accepted(acc_idx, n_acc, want_indices)
 
 
 def dist_seuclidean(S, obs, V, threshold=None, want_indices=True):
     """cdist(S, obs, 'seuclidean', V=V) + acceptance on the device, bit-identical to SciPy (two
     running sums and an IEEE division per term; elfi/model/elfi_model.py:1016-1037 forwards the
     metric string and V to cdist).  Returns (d (B,), acc_idx or None)."""
-    S = _matrix(S)
+    S, obs_t, thr, d, acc_idx, n_acc = _dist_prepare(S, obs, threshold, 1, want_indices)
     B, D = S.shape
-    obs_t = dev.to_device(obs).reshape(-1)
-    if obs_t.numel() != D:
-        raise ValueError('XA and XB must have the same number of columns '
-                         '(i.e. feature dimension.)')
     V_t = dev.to_device(V)
     if V_t.dim() != 1 or V_t.shape[0] != D:
         raise ValueError('Variance vector V must be of the same dimension as the vectors on '
                          'which the distances are computed.')
-    thr = None
-    if threshold is not None:
-        thr = np.ascontiguousarray(np.atleast_1d(threshold), dtype=np.float64)
-        if thr.shape[0] != 1:
-            raise ValueError('need one threshold per distance column ({} != 1)'.format(thr.shape[0]))
-    d = dev.empty((B,))
-    acc_idx = n_acc = None
-    if thr is not None:
-        n_acc = dev.zeros((1,), dtype=torch.int64)
-        if want_indices:
-            acc_idx = dev.empty((max(B, 1),), dtype=torch.int32)
-    _lib.call('elfi_b200_dist_seuclidean_thr_f64', dev.context(), dev.ptr(S),
-              S.stride(0) if B > 1 else D, B, D, dev.ptr(obs_t), dev.ptr(V_t), dev.ptr(thr),
-              dev.ptr(d), dev.ptr(acc_idx), dev.ptr(n_acc), dev.stream_ptr())
-    if thr is not None:
-        n = int(n_acc.item())
-        acc_idx = acc_idx[:n] if want_indices else n
-    return d, acc_idx
+    _lib.call('elfi_b200_dist_seuclidean_thr_f64', dev.context(), dev.ptr(S), _ld(S), B, D,
+              dev.ptr(obs_t), dev.ptr(V_t), dev.ptr(thr), dev.ptr(d), dev.ptr(acc_idx),
+              dev.ptr(n_acc), dev.stream_ptr())
+    return d.reshape(B), _dist_accepted(acc_idx, n_acc, want_indices)
 
 
 def dist_euclid_host(S, obs, w=None, thresholds=None, return_distances=True):
@@ -217,10 +204,6 @@ def dist_euclid_host(S, obs, w=None, thresholds=None, return_distances=True):
     if d is not None and K == 1 and (w is None or np.ndim(w) == 1):
         d = d.reshape(B)
     return d, (idx[:n.value] if idx is not None else None)
-
-
-def _ld(t):
-    return t.stride(0) if t.shape[0] > 1 else t.shape[1]
 
 
 def autocov(x, lags=(1,), out=None):
