@@ -99,16 +99,16 @@ int elfi_b200_sim_arch_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int
     ELFI_REQUIRE((Y == nullptr || ldY >= n_obs) && (S == nullptr || ldS >= arch_nsumm(int(n_lags))),
                  "sim_arch: bad leading dimension of Y or S");
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     const size_t smem = S ? arch_strip_bytes(int(n_obs)) : 0;
-    ELFI_CUDA_OK(cudaFuncSetAttribute(sim_arch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      int(arch_strip_bytes(ARCH_NOBS_MAX))));
     const unsigned blocks = unsigned((B + ARCH_THREADS - 1) / ARCH_THREADS);
-    sim_arch_kernel<<<blocks, ARCH_THREADS, smem, stream>>>(P, ldP, B, int(n_obs), int(n_lags),
-                                                            seed, offset, Y, ldY, S, ldS);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        ELFI_CUDA_OK(cudaFuncSetAttribute(sim_arch_kernel,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          int(arch_strip_bytes(ARCH_NOBS_MAX))));
+        sim_arch_kernel<<<blocks, ARCH_THREADS, smem, stream>>>(P, ldP, B, int(n_obs), int(n_lags),
+                                                                seed, offset, Y, ldY, S, ldS);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_arch_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_b, int64_t ld_j,
@@ -122,16 +122,15 @@ int elfi_b200_arch_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld
                  "ldS >= 2 + L + L(L-1)/2; n=%lld n_lags=%lld ldS=%lld)", ARCH_NOBS_MIN,
                  ARCH_NOBS_MAX, ARCH_LAGS_MAX, (long long)n, (long long)n_lags, (long long)ldS);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    ELFI_CUDA_OK(cudaFuncSetAttribute(arch_summaries_kernel,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      int(arch_strip_bytes(ARCH_NOBS_MAX))));
     const unsigned blocks = unsigned((B + ARCH_THREADS - 1) / ARCH_THREADS);
-    arch_summaries_kernel<<<blocks, ARCH_THREADS, arch_strip_bytes(int(n)), stream>>>(
-        X, ld_b, ld_j, B, int(n), int(n_lags), S, ldS);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        ELFI_CUDA_OK(cudaFuncSetAttribute(arch_summaries_kernel,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          int(arch_strip_bytes(ARCH_NOBS_MAX))));
+        arch_summaries_kernel<<<blocks, ARCH_THREADS, arch_strip_bytes(int(n)), stream>>>(
+            X, ld_b, ld_j, B, int(n), int(n_lags), S, ldS);
+        return ELFI_B200_OK;
+    });
 }
 
 }  // extern "C"

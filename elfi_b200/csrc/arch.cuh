@@ -17,6 +17,7 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "hd.cuh"
 #include "leafsum.cuh"
 
 namespace elfi {

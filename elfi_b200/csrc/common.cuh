@@ -12,6 +12,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <type_traits>
 
 #include "../../include/elfi_b200.h"
 
@@ -78,6 +79,38 @@ int make_rowmajor_f64_map(elfi_b200_ctx* ctx, const double* base, int64_t rows, 
 
 inline bool tma_compatible(const void* base, int64_t ld) {
     return (reinterpret_cast<uintptr_t>(base) % 16 == 0) && ((ld * 8) % 16 == 0);
+}
+
+// The body of a device entry point, after its argument checks: make the context's device current,
+// run body(stream), which returns ELFI_B200_OK or an error code (so ELFI_CUDA_OK and ELFI_REQUIRE
+// work inside it), then report an error of the launches it made.
+template <class Body>
+int run_on_device(elfi_b200_ctx* ctx, void* stream, Body&& body) {
+    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
+    const int rc = body(static_cast<cudaStream_t>(stream));
+    if (rc != ELFI_B200_OK) return rc;
+    ELFI_CUDA_OK(cudaGetLastError());
+    return ELFI_B200_OK;
+}
+
+// f(std::integral_constant<int, K>{}) for the power of two K in [LO, HI] that k selects (LO below
+// the range, HI above it); instantiates f for exactly LO, 2 LO, ..., HI.  Returns what f returns.
+template <int LO, int HI, class F>
+auto with_pow2(int k, F&& f) {
+    if constexpr (LO == HI) {
+        return f(std::integral_constant<int, LO>{});
+    } else {
+        if (k <= LO) return f(std::integral_constant<int, LO>{});
+        return with_pow2<2 * LO, HI>(k, f);
+    }
+}
+
+// ceil(work / per_block) blocks, at most ctas_per_sm per SM: the kernels behind it grid-stride
+inline unsigned capped_grid(const elfi_b200_ctx* ctx, int64_t work, int64_t per_block,
+                            int ctas_per_sm) {
+    const int64_t blocks = (work + per_block - 1) / per_block;
+    const int64_t cap = int64_t(ctx->sm_count) * ctas_per_sm;
+    return unsigned(blocks < cap ? blocks : cap);
 }
 
 // ------------------------------------------------------------------------------------

@@ -176,8 +176,6 @@ int elfi_b200_sim_daycare_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, 
     ELFI_REQUIRE(time_end > 0.0 && time_end < INFINITY,
                  "sim_daycare: time_end must be finite and > 0");
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     DcSim a;
     a.P = P;
     a.ldP = ldP;
@@ -196,9 +194,10 @@ int elfi_b200_sim_daycare_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, 
     a.X = X;
     a.K = K;
     const size_t smem = 32 * (8 * size_t(n_ind) + 12 * size_t(n_strains));
-    sim_daycare_kernel<<<unsigned(B), 32, smem, stream>>>(a);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        sim_daycare_kernel<<<unsigned(B), 32, smem, stream>>>(a);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_daycare_summaries_f64(elfi_b200_ctx* ctx, const uint8_t* X, int64_t ld_b,
@@ -213,14 +212,12 @@ int elfi_b200_daycare_summaries_f64(elfi_b200_ctx* ctx, const uint8_t* X, int64_
                  "ldS >= 4 n_dcc; n_dcc=%lld n_obs=%lld n_strains=%lld ldS=%lld)",
                  (long long)n_dcc, (long long)n_obs, (long long)n_strains, (long long)ldS);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    int64_t blocks = (B * n_dcc + DC_SUMM_THREADS - 1) / DC_SUMM_THREADS;
-    if (blocks > int64_t(ctx->sm_count) * 32) blocks = int64_t(ctx->sm_count) * 32;
-    daycare_summaries_kernel<<<unsigned(blocks), DC_SUMM_THREADS, 0, stream>>>(
-        X, ld_b, ld_c, ld_i, ld_s, B, int(n_dcc), int(n_obs), int(n_strains), S, ldS);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        const unsigned blocks = capped_grid(ctx, B * n_dcc, DC_SUMM_THREADS, 32);
+        daycare_summaries_kernel<<<blocks, DC_SUMM_THREADS, 0, stream>>>(
+            X, ld_b, ld_c, ld_i, ld_s, B, int(n_dcc), int(n_obs), int(n_strains), S, ldS);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_daycare_distance_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
@@ -234,14 +231,12 @@ int elfi_b200_daycare_distance_f64(elfi_b200_ctx* ctx, const double* S, int64_t 
                  "n_dcc=%lld ldS=%lld)", DC_DIST_TERMS_MAX, (long long)n_ss, (long long)n_dcc,
                  (long long)ldS);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    int64_t blocks = (B + DC_DIST_THREADS - 1) / DC_DIST_THREADS;
-    if (blocks > int64_t(ctx->sm_count) * 32) blocks = int64_t(ctx->sm_count) * 32;
-    daycare_distance_kernel<<<unsigned(blocks), DC_DIST_THREADS, 0, stream>>>(
-        S, ldS, B, int(n_ss), int(n_dcc), obs_max, y, d);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        const unsigned blocks = capped_grid(ctx, B, DC_DIST_THREADS, 32);
+        daycare_distance_kernel<<<blocks, DC_DIST_THREADS, 0, stream>>>(
+            S, ldS, B, int(n_ss), int(n_dcc), obs_max, y, d);
+        return ELFI_B200_OK;
+    });
 }
 
 }  // extern "C"

@@ -27,6 +27,7 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "hd.cuh"
 #include "lotka_volterra.cuh"   // lv_leaf_sum: NumPy's pairwise order for <= 128 terms
 
 namespace elfi {

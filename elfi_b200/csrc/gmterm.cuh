@@ -10,11 +10,7 @@
 // (and so does a zero weight, whose nt is +inf; a NaN nt fails the compare and gives 0 too).
 #pragma once
 
-#if defined(__CUDACC__)
-#define ELFI_GM_HD __host__ __device__ __forceinline__
-#else
-#define ELFI_GM_HD inline
-#endif
+#include "hd.cuh"
 
 #if !defined(__CUDA_ARCH__)
 #include <math.h>
@@ -47,7 +43,7 @@ inline double gm_hilo(int hi, int lo) {
 }
 #endif
 
-ELFI_GM_HD double exp2_neg(double nt) {
+ELFI_HD double exp2_neg(double nt) {
     const double magic = 6755399441055744.0;  // 1.5 * 2^52
     const double tm = magic - nt;
     const double kd = tm - magic;             // rint(-nt)

@@ -6,15 +6,11 @@
 
 #include <math.h>
 
-#if defined(__CUDACC__)
-#define ELFI_GNK_HD __host__ __device__ __forceinline__
-#else
-#define ELFI_GNK_HD inline
-#endif
+#include "hd.cuh"
 
 namespace elfi {
 
-ELFI_GNK_HD double gnk_quantile(double A, double B, double g, double k, double c, double z) {
+ELFI_HD double gnk_quantile(double A, double B, double g, double k, double c, double z) {
     const double e = exp(-g * z);
     const double skew = 1.0 + c * ((1.0 - e) / (1.0 + e));
     const double kurt = pow(1.0 + z * z, k);

@@ -17,6 +17,7 @@
 #include "gnkstats.cuh"
 #include "leafsum.cuh"
 #include "philox.cuh"
+#include "rowquantiles.cuh"
 
 namespace elfi {
 
@@ -239,15 +240,9 @@ euclidean_multiss_kernel(const double* __restrict__ S, int64_t ldS, int64_t B, i
     }
 }
 
-static int kpl_for(int n, int min_kpl) {
-    int kpl = min_kpl;
-    while (kpl * 32 < n) kpl <<= 1;
-    return kpl;
-}
-
-static int64_t warp_blocks(int64_t warps, int sm_count) {
-    int64_t blocks = (warps + 7) / 8;
-    if (blocks > int64_t(sm_count) * 8) blocks = int64_t(sm_count) * 8;
+// blocks of 8 warps, at most 8 per SM and at least one
+static unsigned warp_blocks(const elfi_b200_ctx* ctx, int64_t warps) {
+    const unsigned blocks = capped_grid(ctx, warps, 8, 8);
     return blocks < 1 ? 1 : blocks;
 }
 
@@ -285,28 +280,26 @@ int elfi_b200_gnk_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_
     int rc = read_picks(picks_host, n, &p);
     if (rc) return rc;
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    const unsigned blocks = unsigned(warp_blocks(B * d, ctx->sm_count));
+    const unsigned blocks = warp_blocks(ctx, B * d);
     const int ni = int(n), di = int(d);
-    if (n <= GNK_REGS_MAX) {
-        switch (kpl_for(ni, 1)) {
-#define ELFI_GNK_SUMM(KPL) \
-    case KPL: gnk_summaries_regs_kernel<KPL><<<blocks, 256, 0, stream>>>(X, ld_row, ld_obs, B, ni, di, kind, p, out, ld_out); break
-            ELFI_GNK_SUMM(1); ELFI_GNK_SUMM(2); ELFI_GNK_SUMM(4); ELFI_GNK_SUMM(8); ELFI_GNK_SUMM(16);
-#undef ELFI_GNK_SUMM
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        if (n <= GNK_REGS_MAX) {
+            with_pow2<1, 16>(kpl_for(ni, 1), [&](auto K) {
+                gnk_summaries_regs_kernel<decltype(K)::value><<<blocks, 256, 0, stream>>>(
+                    X, ld_row, ld_obs, B, ni, di, kind, p, out, ld_out);
+            });
+        } else {
+            int npow2 = 2;
+            while (npow2 < n) npow2 <<= 1;
+            const size_t smem = size_t(8) * npow2 * 8;
+            ELFI_CUDA_OK(cudaFuncSetAttribute(gnk_summaries_smem_kernel,
+                                              cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              int(smem)));
+            gnk_summaries_smem_kernel<<<blocks, 256, smem, stream>>>(X, ld_row, ld_obs, B, ni, npow2,
+                                                                     di, kind, p, out, ld_out);
         }
-    } else {
-        int npow2 = 2;
-        while (npow2 < n) npow2 <<= 1;
-        const size_t smem = size_t(8) * npow2 * 8;
-        ELFI_CUDA_OK(cudaFuncSetAttribute(gnk_summaries_smem_kernel,
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-        gnk_summaries_smem_kernel<<<blocks, 256, smem, stream>>>(X, ld_row, ld_obs, B, ni, npow2, di, kind,
-                                                                 p, out, ld_out);
-    }
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_sim_gnk_summaries_f64(elfi_b200_ctx* ctx, const double* A, const double* Bs,
@@ -325,18 +318,15 @@ int elfi_b200_sim_gnk_summaries_f64(elfi_b200_ctx* ctx, const double* A, const d
     int rc = read_picks(picks_host, n_obs, &p);
     if (rc) return rc;
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    const unsigned blocks = unsigned(warp_blocks(B, ctx->sm_count));
+    const unsigned blocks = warp_blocks(ctx, B);
     const int n = int(n_obs);
-    switch (kpl_for(n, 2)) {
-#define ELFI_GNK_FUSED(KPL) \
-    case KPL: sim_gnk_summaries_kernel<KPL><<<blocks, 256, 0, stream>>>(A, Bs, g, k, c, B, n, seed, offset, kind, p, out, ld_out); break
-        ELFI_GNK_FUSED(2); ELFI_GNK_FUSED(4); ELFI_GNK_FUSED(8); ELFI_GNK_FUSED(16);
-#undef ELFI_GNK_FUSED
-    }
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        with_pow2<2, 16>(kpl_for(n, 2), [&](auto K) {
+            sim_gnk_summaries_kernel<decltype(K)::value><<<blocks, 256, 0, stream>>>(
+                A, Bs, g, k, c, B, n, seed, offset, kind, p, out, ld_out);
+        });
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_sim_bignk_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, double c, int64_t B,
@@ -359,27 +349,20 @@ int elfi_b200_sim_bignk_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, do
         if (rc) return rc;
     }
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     const int n = int(n_obs);
-    if (Y) {
-        int64_t blocks = (B * n_obs + 255) / 256;
-        const int64_t cap = int64_t(ctx->sm_count) * 64;
-        if (blocks > cap) blocks = cap;
-        sim_bignk_kernel<<<unsigned(blocks), 256, 0, stream>>>(P, ldP, c, B, n, seed, offset, Y, ldY);
-    }
-    if (S) {
-        const unsigned blocks = unsigned(warp_blocks(B, ctx->sm_count));
-        switch (kpl_for(n, 1)) {
-#define ELFI_BIGNK_FUSED(KPL) \
-    case KPL: sim_bignk_summaries_kernel<KPL><<<blocks, 256, 0, stream>>>(P, ldP, c, B, n, seed, offset, kind, p, S, ldS); break
-            ELFI_BIGNK_FUSED(1); ELFI_BIGNK_FUSED(2); ELFI_BIGNK_FUSED(4); ELFI_BIGNK_FUSED(8);
-            ELFI_BIGNK_FUSED(16);
-#undef ELFI_BIGNK_FUSED
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        if (Y)
+            sim_bignk_kernel<<<capped_grid(ctx, B * n_obs, 256, 64), 256, 0, stream>>>(
+                P, ldP, c, B, n, seed, offset, Y, ldY);
+        if (S) {
+            const unsigned blocks = warp_blocks(ctx, B);
+            with_pow2<1, 16>(kpl_for(n, 1), [&](auto K) {
+                sim_bignk_summaries_kernel<decltype(K)::value><<<blocks, 256, 0, stream>>>(
+                    P, ldP, c, B, n, seed, offset, kind, p, S, ldS);
+            });
         }
-    }
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_euclidean_multiss_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
@@ -389,13 +372,11 @@ int elfi_b200_euclidean_multiss_f64(elfi_b200_ctx* ctx, const double* S, int64_t
     ELFI_REQUIRE(B >= 0 && K >= 1 && K <= LEAF_MAX_TERMS && ldS >= K,
                  "euclidean_multiss: bad shape (1 <= K <= %d; K=%lld)", LEAF_MAX_TERMS, (long long)K);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    int64_t blocks = (B + 255) / 256;
-    if (blocks > int64_t(ctx->sm_count) * 16) blocks = int64_t(ctx->sm_count) * 16;
-    euclidean_multiss_kernel<<<unsigned(blocks), 256, 0, stream>>>(S, ldS, B, int(K), obs, out);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        euclidean_multiss_kernel<<<capped_grid(ctx, B, 256, 16), 256, 0, stream>>>(S, ldS, B, int(K),
+                                                                                  obs, out);
+        return ELFI_B200_OK;
+    });
 }
 
 }  // extern "C"

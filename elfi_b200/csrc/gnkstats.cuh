@@ -19,6 +19,7 @@
 
 #include <math.h>
 
+#include "hd.cuh"
 #include "leafsum.cuh"
 
 namespace elfi {

@@ -14,13 +14,7 @@
 // kernels in summaries.cu only add the shared-memory read of the 16 columns.
 #pragma once
 
-#if defined(__CUDACC__)
-#define ELFI_HD __host__ __device__ __forceinline__
-#define ELFI_UNROLL _Pragma("unroll")
-#else
-#define ELFI_HD inline
-#define ELFI_UNROLL
-#endif
+#include "hd.cuh"
 
 namespace elfi {
 

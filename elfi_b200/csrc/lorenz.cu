@@ -358,21 +358,17 @@ static int launch_sim_lorenz(elfi_b200_ctx* ctx, const LorenzSim& a, double* X, 
         sim_lorenz_kernel<V><<<unsigned(blocks), LORENZ_THREADS, 0, stream>>>(a, L, R, n_groups, X);
         ELFI_CUDA_OK(cudaGetLastError());
         if (S) {
-            int64_t sb = (a.B + LORENZ_WARPS - 1) / LORENZ_WARPS;
-            if (sb > int64_t(ctx->sm_count) * 16) sb = int64_t(ctx->sm_count) * 16;
+            const unsigned sb = capped_grid(ctx, a.B, LORENZ_WARPS, 16);
             const int64_t tm = int64_t(a.T) * a.m;
-            lorenz_summaries_kernel<<<unsigned(sb), LORENZ_THREADS, 0, stream>>>(
+            lorenz_summaries_kernel<<<sb, LORENZ_THREADS, 0, stream>>>(
                 X, tm, a.m, 1, a.B, a.T, a.m, S, ldS);
         }
         return ELFI_B200_OK;
     }
     const size_t slab_bytes = size_t(R) * size_t(a.T) * size_t(a.m) * sizeof(double);
-    int64_t blocks = (n_groups + LORENZ_WARPS - 1) / LORENZ_WARPS;
-    int64_t cap = int64_t(ctx->sm_count) * LORENZ_FUSED_BLOCKS_PER_SM;
+    int64_t blocks = capped_grid(ctx, n_groups, LORENZ_WARPS, LORENZ_FUSED_BLOCKS_PER_SM);
     const int64_t by_budget = int64_t(LORENZ_SLAB_BUDGET / (slab_bytes * LORENZ_WARPS));
-    if (cap > by_budget) cap = by_budget;
-    if (cap < 1) cap = 1;
-    if (blocks > cap) blocks = cap;
+    if (blocks > by_budget) blocks = by_budget < 1 ? 1 : by_budget;
     double* slab = static_cast<double*>(
         ctx_scratch(ctx, size_t(blocks) * LORENZ_WARPS * slab_bytes));
     if (!slab) return ELFI_B200_ERR_CUDA;
@@ -403,8 +399,6 @@ int elfi_b200_sim_lorenz_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, i
                  "sim_lorenz: summaries need n_timestep * n_obs <= %lld and ldS >= 6",
                  (long long)LORENZ_SUMM_MAX_TERMS);
     if (B == 0 || (X == nullptr && S == nullptr)) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     LorenzSim a;
     a.P = P;
     a.ldP = ldP;
@@ -419,12 +413,11 @@ int elfi_b200_sim_lorenz_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, i
     a.seed = seed;
     a.offset = offset;
     const int V = lorenz_vars_per_lane(a.m);
-    const int rc = V == 1   ? launch_sim_lorenz<1>(ctx, a, X, S, ldS, stream)
-                   : V == 2 ? launch_sim_lorenz<2>(ctx, a, X, S, ldS, stream)
-                            : launch_sim_lorenz<4>(ctx, a, X, S, ldS, stream);
-    if (rc) return rc;
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        return V == 1   ? launch_sim_lorenz<1>(ctx, a, X, S, ldS, stream)
+               : V == 2 ? launch_sim_lorenz<2>(ctx, a, X, S, ldS, stream)
+                        : launch_sim_lorenz<4>(ctx, a, X, S, ldS, stream);
+    });
 }
 
 int elfi_b200_lorenz_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_row,
@@ -439,14 +432,12 @@ int elfi_b200_lorenz_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t 
                  LORENZ_M_MAX, (long long)LORENZ_SUMM_MAX_TERMS, (long long)n_timestep,
                  (long long)n_obs);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    int64_t blocks = (B + LORENZ_WARPS - 1) / LORENZ_WARPS;
-    if (blocks > int64_t(ctx->sm_count) * 16) blocks = int64_t(ctx->sm_count) * 16;
-    lorenz_summaries_kernel<<<unsigned(blocks), LORENZ_THREADS, 0, stream>>>(
-        X, ld_row, ld_t, ld_k, B, int(n_timestep), int(n_obs), S, ldS);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        const unsigned blocks = capped_grid(ctx, B, LORENZ_WARPS, 16);
+        lorenz_summaries_kernel<<<blocks, LORENZ_THREADS, 0, stream>>>(
+            X, ld_row, ld_t, ld_k, B, int(n_timestep), int(n_obs), S, ldS);
+        return ELFI_B200_OK;
+    });
 }
 
 }  // extern "C"

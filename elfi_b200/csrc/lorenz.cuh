@@ -19,6 +19,7 @@
 
 #include <stdint.h>
 
+#include "hd.cuh"
 #include "leafsum.cuh"
 
 namespace elfi {

@@ -169,17 +169,6 @@ int elfi_b200_sim_lotka_volterra_f64(elfi_b200_ctx* ctx, const double* P, int64_
                  "sim_lotka_volterra: 1 <= max_events <= 2^32 - 1 (the event is one Philox word), "
                  "got %lld", (long long)max_events);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    auto* counter = static_cast<unsigned long long*>(ctx_scratch(ctx, 256));
-    if (!counter) return ELFI_B200_ERR_CUDA;
-    ELFI_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(unsigned long long), stream));
-    int per_sm = 0;
-    ELFI_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sim_lv_kernel, LV_THREADS, 0));
-    if (per_sm < 1) per_sm = 1;
-    int64_t blocks = int64_t(ctx->sm_count) * per_sm;
-    const int64_t need = (B + LV_THREADS - 1) / LV_THREADS;
-    if (blocks > need) blocks = need;
     LvSim a;
     a.P = P;
     a.ldP = ldP;
@@ -192,10 +181,18 @@ int elfi_b200_sim_lotka_volterra_f64(elfi_b200_ctx* ctx, const double* P, int64_
     a.offset = offset;
     a.X = X;
     a.n_events = n_events;
-    a.next_row = counter;
-    sim_lv_kernel<<<unsigned(blocks), LV_THREADS, 0, stream>>>(a);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        auto* counter = static_cast<unsigned long long*>(ctx_scratch(ctx, 256));
+        if (!counter) return ELFI_B200_ERR_CUDA;
+        ELFI_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(unsigned long long), stream));
+        a.next_row = counter;
+        int per_sm = 0;
+        ELFI_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sim_lv_kernel,
+                                                                   LV_THREADS, 0));
+        if (per_sm < 1) per_sm = 1;
+        sim_lv_kernel<<<capped_grid(ctx, B, LV_THREADS, per_sm), LV_THREADS, 0, stream>>>(a);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_lv_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_row, int64_t ld_obs,
@@ -208,14 +205,12 @@ int elfi_b200_lv_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_r
                  "lv_summaries: bad shape (%d <= n_obs <= %d, ldS >= %d; n_obs=%lld ldS=%lld)",
                  LV_SUMM_NOBS_MIN, LV_SUMM_NOBS_MAX, LV_NSUMM, (long long)n_obs, (long long)ldS);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    int64_t blocks = (B + LV_SUMM_THREADS - 1) / LV_SUMM_THREADS;
-    if (blocks > int64_t(ctx->sm_count) * 32) blocks = int64_t(ctx->sm_count) * 32;
-    lv_summaries_kernel<<<unsigned(blocks), LV_SUMM_THREADS, 0, stream>>>(
-        X, ld_row, ld_obs, ld_species, B, int(n_obs), S, ldS);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        const unsigned blocks = capped_grid(ctx, B, LV_SUMM_THREADS, 32);
+        lv_summaries_kernel<<<blocks, LV_SUMM_THREADS, 0, stream>>>(
+            X, ld_row, ld_obs, ld_species, B, int(n_obs), S, ldS);
+        return ELFI_B200_OK;
+    });
 }
 
 }  // extern "C"

@@ -31,6 +31,7 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "hd.cuh"
 #include "gnkstats.cuh"
 
 namespace elfi {

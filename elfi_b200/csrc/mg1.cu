@@ -10,13 +10,15 @@
 //
 // Layout.  The recurrence is sequential in j, so one thread simulates one row; the quantiles need
 // the whole row sorted, which one warp does in registers (bitonic_in_registers).  A warp's 32 rows
-// therefore go through a per-warp shared-memory strip: thread r writes its row to strip[r * npad +
-// j] (npad = n | 1, an odd stride: no bank conflicts), then the warp loads each row in turn, lane
-// L taking elements k * 32 + L (conflict-free; the order of the keys before the sort does not
-// matter), sorts it and lane k < nq writes quantile k.  The data reaches HBM only when asked for,
-// copied out of the strip row by row (coalesced).  A strip takes 256 npad bytes per warp; a block
-// has as many warps (at most 4) as fit in 64 KiB.  Not measured: keeping each row's sort in the
-// simulating thread (a register or shared-memory sort of n keys per thread) instead of the warp.
+// therefore go through a per-warp shared-memory strip (rowquantiles.cuh's warp_strips, which
+// svm.cu shares): thread r writes its row to strip[r * npad + j] (npad = n | 1, an odd stride: no
+// bank conflicts), then the warp loads each row in turn, lane L taking elements k * 32 + L
+// (conflict-free; the order of the keys before the sort does not matter), sorts it and lane k < nq
+// writes quantile k.  The data reaches HBM only when asked for, copied out of the strip row by row
+// (coalesced).  A strip takes 256 npad bytes per warp; a block has as many warps (at most
+// MG1_WARPS_MAX = 4) as fit in MG1_STRIP_BUDGET = 64 KiB.  Not measured: keeping each row's sort
+// in the simulating thread (a register or shared-memory sort of n keys per thread) instead of the
+// warp.
 //
 // row_quantiles_kernel loads any strided row into the same registers and calls the same code
 // (rowquantiles.cuh, which svm.cu shares).  A sorted row does not depend on the order its keys came
@@ -122,29 +124,18 @@ int elfi_b200_sim_mg1_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int6
                  "sim_mg1: every q must lie in [0, 1]");
     if (S == nullptr) memset(&Q, 0, sizeof(Q));
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    const int n = int(n_obs), npad = n | 1;
-    const size_t warp_bytes = size_t(32) * npad * sizeof(double);
-    int warps = int(MG1_STRIP_BUDGET / warp_bytes);
-    warps = warps < 1 ? 1 : (warps > MG1_WARPS_MAX ? MG1_WARPS_MAX : warps);
-    const size_t smem = warps * warp_bytes;
-    const unsigned blocks = unsigned((B + 32 * warps - 1) / (32 * warps));
-#define ELFI_SIM_MG1(KPL)                                                                          \
-    ELFI_CUDA_OK(cudaFuncSetAttribute(sim_mg1_kernel<KPL>,                                         \
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));    \
-    sim_mg1_kernel<KPL><<<blocks, 32 * warps, smem, stream>>>(P, ldP, B, n, npad, int(nq), Q,      \
-                                                              seed, offset, Y, ldY, S, ldS)
-    switch (quantile_kpl(n)) {
-    case 1: ELFI_SIM_MG1(1); break;
-    case 2: ELFI_SIM_MG1(2); break;
-    case 4: ELFI_SIM_MG1(4); break;
-    case 8: ELFI_SIM_MG1(8); break;
-    default: ELFI_SIM_MG1(16); break;
-    }
-#undef ELFI_SIM_MG1
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    const int n = int(n_obs);
+    const WarpStrips st = warp_strips(B, n, MG1_STRIP_BUDGET, MG1_WARPS_MAX);
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        return with_pow2<1, 16>(kpl_for(n, 1), [&](auto K) {
+            ELFI_CUDA_OK(cudaFuncSetAttribute(sim_mg1_kernel<decltype(K)::value>,
+                                              cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              int(st.smem)));
+            sim_mg1_kernel<decltype(K)::value><<<st.blocks, 32 * st.warps, st.smem, stream>>>(
+                P, ldP, B, n, st.npad, int(nq), Q, seed, offset, Y, ldY, S, ldS);
+            return ELFI_B200_OK;
+        });
+    });
 }
 
 int elfi_b200_row_quantiles_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_b, int64_t ld_j,
@@ -160,23 +151,15 @@ int elfi_b200_row_quantiles_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_
     QuantileLevels Q;
     ELFI_REQUIRE(quantile_levels(q_host, nq, &Q), "row_quantiles: every q must lie in [0, 1]");
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     const int64_t want = (B + 7) / 8;
     const unsigned blocks = unsigned(want < 65535 * 16 ? want : 65535 * 16);
-#define ELFI_ROW_QUANTILES(KPL)                                                                    \
-    row_quantiles_kernel<KPL><<<blocks, 256, 0, stream>>>(X, ld_b, ld_j, B, int(n), int(nq), Q, S, \
-                                                          ldS)
-    switch (quantile_kpl(int(n))) {
-    case 1: ELFI_ROW_QUANTILES(1); break;
-    case 2: ELFI_ROW_QUANTILES(2); break;
-    case 4: ELFI_ROW_QUANTILES(4); break;
-    case 8: ELFI_ROW_QUANTILES(8); break;
-    default: ELFI_ROW_QUANTILES(16); break;
-    }
-#undef ELFI_ROW_QUANTILES
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        with_pow2<1, 16>(kpl_for(int(n), 1), [&](auto K) {
+            row_quantiles_kernel<decltype(K)::value><<<blocks, 256, 0, stream>>>(
+                X, ld_b, ld_j, B, int(n), int(nq), Q, S, ldS);
+        });
+        return ELFI_B200_OK;
+    });
 }
 
 }  // extern "C"

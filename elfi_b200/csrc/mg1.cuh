@@ -22,6 +22,7 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "hd.cuh"
 #include "gnkstats.cuh"
 #include "toad.cuh"
 

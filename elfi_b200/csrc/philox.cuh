@@ -6,15 +6,11 @@
 
 #include <stdint.h>
 
-#if defined(__CUDACC__)
-#define ELFI_PHILOX_HD __host__ __device__ __forceinline__
-#else
-#define ELFI_PHILOX_HD inline
-#endif
+#include "hd.cuh"
 
 namespace elfi {
 
-ELFI_PHILOX_HD uint32_t philox_mulhi(uint32_t a, uint32_t b) {
+ELFI_HD uint32_t philox_mulhi(uint32_t a, uint32_t b) {
 #if defined(__CUDA_ARCH__)
     return __umulhi(a, b);
 #else
@@ -31,8 +27,8 @@ struct PhiloxWords { uint32_t x, y, z, w; };
 // key (seed & 0xffffffff, seed >> 32), counter (c0, c1, c2, c3) -> four 32-bit words
 struct Philox {
     uint32_t key0, key1;
-    ELFI_PHILOX_HD Philox(uint64_t seed) : key0(uint32_t(seed)), key1(uint32_t(seed >> 32)) {}
-    ELFI_PHILOX_HD PhiloxWords operator()(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3) const {
+    ELFI_HD Philox(uint64_t seed) : key0(uint32_t(seed)), key1(uint32_t(seed >> 32)) {}
+    ELFI_HD PhiloxWords operator()(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3) const {
         uint32_t k0 = key0, k1 = key1;
 #pragma unroll
         for (int r = 0; r < 10; ++r) {
@@ -49,7 +45,7 @@ struct Philox {
 };
 
 // (0, 1] with 53 random bits: the 32 bits of a above the 21 high bits of b, plus one ulp
-ELFI_PHILOX_HD double u01(uint32_t a, uint32_t b) {
+ELFI_HD double u01(uint32_t a, uint32_t b) {
     const uint64_t v = (uint64_t(a) << 21) ^ uint64_t(b >> 11);
     return (double(v & ((uint64_t(1) << 53) - 1)) + 1.0) * (1.0 / 9007199254740992.0);
 }

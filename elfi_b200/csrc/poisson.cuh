@@ -35,11 +35,7 @@
 
 #include "philox.cuh"
 
-#if defined(__CUDACC__)
-#define ELFI_POIS_HD __host__ __device__ __forceinline__
-#else
-#define ELFI_POIS_HD inline
-#endif
+#include "hd.cuh"
 
 namespace elfi {
 
@@ -49,21 +45,21 @@ constexpr int POISSON_INV_MAX = 64;
 constexpr int POISSON_MAX_TRIALS = 32;
 constexpr double POISSON_HALF_LOG_2PI = 0.9189385332046728;   // log(2 pi) / 2
 
-ELFI_POIS_HD double pois_add(double a, double b) {
+ELFI_HD double pois_add(double a, double b) {
 #if defined(__CUDA_ARCH__)
     return __dadd_rn(a, b);
 #else
     return a + b;
 #endif
 }
-ELFI_POIS_HD double pois_sub(double a, double b) {
+ELFI_HD double pois_sub(double a, double b) {
 #if defined(__CUDA_ARCH__)
     return __dsub_rn(a, b);
 #else
     return a - b;
 #endif
 }
-ELFI_POIS_HD double pois_mul(double a, double b) {
+ELFI_HD double pois_mul(double a, double b) {
 #if defined(__CUDA_ARCH__)
     return __dmul_rn(a, b);
 #else
@@ -73,7 +69,7 @@ ELFI_POIS_HD double pois_mul(double a, double b) {
 
 // stirlerr(n) = log(n!) - log(sqrt(2 pi n) (n / e)^n) for an integer n >= 1: exact values (to
 // double precision) up to 15, the asymptotic series beyond
-ELFI_POIS_HD double poisson_stirlerr(double n) {
+ELFI_HD double poisson_stirlerr(double n) {
     if (n <= 15.0) {
         switch (int(n)) {
         case 1: return 0.08106146679532726;
@@ -99,7 +95,7 @@ ELFI_POIS_HD double poisson_stirlerr(double n) {
 }
 
 // bd0(x, m) = x log(x / m) + m - x >= 0 (Loader's deviance term)
-ELFI_POIS_HD double poisson_bd0(double x, double m) {
+ELFI_HD double poisson_bd0(double x, double m) {
     const double dx = pois_sub(x, m);
     if (fabs(dx) < pois_mul(0.1, pois_add(x, m))) {
         double v = dx / pois_add(x, m);
@@ -118,7 +114,7 @@ ELFI_POIS_HD double poisson_bd0(double x, double m) {
 }
 
 // log p(k; lam) for an integer-valued k >= 0 and lam > 0
-ELFI_POIS_HD double poisson_logpmf(double k, double lam) {
+ELFI_HD double poisson_logpmf(double k, double lam) {
     if (k == 0.0) return -lam;
     return pois_sub(-pois_add(poisson_stirlerr(k), poisson_bd0(k, lam)),
                     pois_add(POISSON_HALF_LOG_2PI, pois_mul(0.5, log(k))));
@@ -129,7 +125,7 @@ struct PtrsConst {
     double b, a, log_invalpha, vr;
 };
 
-ELFI_POIS_HD PtrsConst ptrs_const(double lam) {
+ELFI_HD PtrsConst ptrs_const(double lam) {
     PtrsConst c;
     c.b = pois_add(0.931, pois_mul(2.53, sqrt(lam)));
     c.a = pois_add(-0.059, pois_mul(0.02483, c.b));
@@ -141,8 +137,8 @@ ELFI_POIS_HD PtrsConst ptrs_const(double lam) {
 // One PTRS trial from U in (-1/2, 1/2] and V in (0, 1].  Returns 1 (accept *k), 0 (reject);
 // *margin = |lhs - log p| of the log-pmf test when it was taken, else +inf (the other tests
 // compare exactly rounded values, which the host build and the replay reproduce bit for bit).
-ELFI_POIS_HD int ptrs_trial(const PtrsConst& c, double lam, double U, double V, double* k,
-                            double* margin) {
+ELFI_HD int ptrs_trial(const PtrsConst& c, double lam, double U, double V, double* k,
+                       double* margin) {
     *margin = INFINITY;
     const double us = pois_sub(0.5, fabs(U));
     const double kf = floor(pois_add(pois_add(pois_mul(pois_add(pois_mul(2.0, c.a) / us, c.b), U), lam),
@@ -168,7 +164,7 @@ struct PoissonDraw {
 
 // Words: j -> PhiloxWords, the j-th block of this draw
 template <class Words>
-ELFI_POIS_HD PoissonDraw poisson_draw(double lam, const Words& words) {
+ELFI_HD PoissonDraw poisson_draw(double lam, const Words& words) {
     PoissonDraw d{0.0, 0, INFINITY};
     if (!(lam >= 0.0) || lam > POISSON_LAM_MAX) {
         d.k = NAN;

@@ -122,12 +122,11 @@ static int prior_rvs_launch(elfi_b200_ctx* ctx, const double* spec_host, int64_t
     ELFI_REQUIRE(prior_entry_from_words(spec_host, loc ? 0 : -1, scale ? 0 : -1, &e, why, sizeof(why)),
                  "prior_rvs: prior parameter 0: %s", why);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    prior_rvs_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(B, seed, offset, e, loc, scale,
-                                                                    out);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        prior_rvs_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(B, seed, offset, e, loc,
+                                                                        scale, out);
+        return ELFI_B200_OK;
+    });
 }
 
 static int prior_logpdf_launch(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int64_t B,
@@ -139,11 +138,11 @@ static int prior_logpdf_launch(elfi_b200_ctx* ctx, const double* x, int64_t ldx,
     const int rc = prior_table_from_host("prior_logpdf", spec_host, int(p), words, &tab);
     if (rc != ELFI_B200_OK) return rc;
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    prior_logpdf_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(x, ldx, B, int(p), tab, out);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        prior_logpdf_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(x, ldx, B, int(p), tab,
+                                                                           out);
+        return ELFI_B200_OK;
+    });
 }
 
 }  // namespace elfi

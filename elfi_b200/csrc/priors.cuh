@@ -35,11 +35,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
-#if defined(__CUDACC__)
-#define ELFI_PRIOR_HD __host__ __device__ __forceinline__
-#else
-#define ELFI_PRIOR_HD inline
-#endif
+#include "hd.cuh"
 
 namespace elfi {
 
@@ -68,16 +64,16 @@ struct PriorEntry {
 struct PriorTable { PriorEntry e[PRIOR_MAX_PARAMS]; };
 
 // scipy.special.xlogy / xlog1py: 0 when the factor is 0 (and y is not NaN)
-ELFI_PRIOR_HD double prior_xlogy(double f, double y) {
+ELFI_HD double prior_xlogy(double f, double y) {
     return (f == 0.0 && y == y) ? 0.0 : f * log(y);
 }
 
-ELFI_PRIOR_HD double prior_xlog1py(double f, double y) {
+ELFI_HD double prior_xlog1py(double f, double y) {
     return (f == 0.0 && y == y) ? 0.0 : f * log1p(y);
 }
 
 // closed support of the standardised variable y
-ELFI_PRIOR_HD bool prior_in_support(const PriorEntry& e, double y) {
+ELFI_HD bool prior_in_support(const PriorEntry& e, double y) {
     switch (e.kind) {
     case PRIOR_NORM: return y == y;
     case PRIOR_TRUNCNORM: return y >= e.a && y <= e.b;
@@ -88,7 +84,7 @@ ELFI_PRIOR_HD bool prior_in_support(const PriorEntry& e, double y) {
 }
 
 // standardised log density at y inside the support (scipy's _logpdf of the kind)
-ELFI_PRIOR_HD double prior_std_logpdf(const PriorEntry& e, double y) {
+ELFI_HD double prior_std_logpdf(const PriorEntry& e, double y) {
     switch (e.kind) {
     case PRIOR_UNIFORM: return 0.0;
     case PRIOR_NORM: return -y * y / 2.0 - PRIOR_NORM_LOGC;
@@ -103,7 +99,7 @@ ELFI_PRIOR_HD double prior_std_logpdf(const PriorEntry& e, double y) {
 // (read only for a sourced loc or scale).  COND = false compiles the sources out, for tables
 // known to have none.
 template <bool COND = true, class Col>
-ELFI_PRIOR_HD double prior_logpdf1(const PriorEntry& e, double x, const Col& col) {
+ELFI_HD double prior_logpdf1(const PriorEntry& e, double x, const Col& col) {
     const double loc = (COND && e.loc_src >= 0) ? col(e.loc_src) : e.loc;
     double scale = e.scale, log_scale = e.log_scale;
     if (COND && e.scale_src >= 0) {
@@ -120,7 +116,7 @@ ELFI_PRIOR_HD double prior_logpdf1(const PriorEntry& e, double x, const Col& col
 // x[src] of a row held in a local array: an unrolled select over PMAX, so that x[] can stay in
 // registers (an indexed load would put it on the stack)
 template <int PMAX>
-ELFI_PRIOR_HD double prior_pick(const double* x, int src) {
+ELFI_HD double prior_pick(const double* x, int src) {
     double v = 0.0;
 #pragma unroll
     for (int b = 0; b < PMAX; ++b)
@@ -131,7 +127,7 @@ ELFI_PRIOR_HD double prior_pick(const double* x, int src) {
 // joint log density of p <= PMAX parameters: the terms summed left to right (the loop is
 // unrolled over PMAX so that a caller's x[] can live in registers)
 template <int PMAX = PRIOR_MAX_PARAMS, bool COND = true>
-ELFI_PRIOR_HD double prior_joint_logpdf(const PriorEntry* e, const double* x, int p) {
+ELFI_HD double prior_joint_logpdf(const PriorEntry* e, const double* x, int p) {
     double s = 0.0;
     const auto col = [&](int j) { return prior_pick<PMAX>(x, j); };
 #pragma unroll
@@ -144,8 +140,8 @@ ELFI_PRIOR_HD double prior_joint_logpdf(const PriorEntry* e, const double* x, in
 // accepted iff 1 + c z > 0 and log u < z^2 / 2 + d - d v + d log v with v = (1 + c z)^3; the
 // draw is then d v.  *margin: the distance of log u from the bound (for replays that exclude
 // knife-edge decisions), or +inf when 1 + c z <= 0.
-ELFI_PRIOR_HD bool prior_mt_accept(double d, double c, double z, double u, double* v,
-                                   double* margin) {
+ELFI_HD bool prior_mt_accept(double d, double c, double z, double u, double* v,
+                             double* margin) {
     const double t = 1.0 + c * z;
     if (!(t > 0.0)) {
         *margin = INFINITY;

@@ -174,11 +174,10 @@ int elfi_b200_poisson_f64(elfi_b200_ctx* ctx, const double* lam, int64_t n, uint
     using namespace elfi;
     ELFI_REQUIRE(ctx && n >= 0 && (n == 0 || (lam && out)), "poisson: bad argument");
     if (n == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    poisson_kernel<<<unsigned((n + 255) / 256), 256, 0, stream>>>(lam, n, seed, offset, out);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        poisson_kernel<<<unsigned((n + 255) / 256), 256, 0, stream>>>(lam, n, seed, offset, out);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_sim_ricker_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t n_params,
@@ -199,19 +198,14 @@ int elfi_b200_sim_ricker_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, i
                  "sim_ricker: fused summaries need n_obs <= %d and ldS >= 3 (n_obs=%lld)",
                  RICKER_FUSED_MAX, (long long)n_obs);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     const int n = int(n_obs);
-    int rc;
-    if (n_params == 3)
-        rc = S ? launch_sim_ricker<true, true>(P, ldP, B, n, stock_init, seed, offset, Y, ldY, N, ldN, S, ldS, stream)
-               : launch_sim_ricker<true, false>(P, ldP, B, n, stock_init, seed, offset, Y, ldY, N, ldN, S, ldS, stream);
-    else
-        rc = S ? launch_sim_ricker<false, true>(P, ldP, B, n, stock_init, seed, offset, Y, ldY, N, ldN, S, ldS, stream)
-               : launch_sim_ricker<false, false>(P, ldP, B, n, stock_init, seed, offset, Y, ldY, N, ldN, S, ldS, stream);
-    if (rc) return rc;
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        if (n_params == 3)
+            return S ? launch_sim_ricker<true, true>(P, ldP, B, n, stock_init, seed, offset, Y, ldY, N, ldN, S, ldS, stream)
+                     : launch_sim_ricker<true, false>(P, ldP, B, n, stock_init, seed, offset, Y, ldY, N, ldN, S, ldS, stream);
+        return S ? launch_sim_ricker<false, true>(P, ldP, B, n, stock_init, seed, offset, Y, ldY, N, ldN, S, ldS, stream)
+                 : launch_sim_ricker<false, false>(P, ldP, B, n, stock_init, seed, offset, Y, ldY, N, ldN, S, ldS, stream);
+    });
 }
 
 int elfi_b200_count_zeros_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, int64_t B, int64_t n,
@@ -222,13 +216,11 @@ int elfi_b200_count_zeros_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, 
                  "count_zeros: bad shape (B=%lld n=%lld ldX=%lld)", (long long)B, (long long)n,
                  (long long)ldX);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    int64_t blocks = (B + 7) / 8;
-    if (blocks > int64_t(ctx->sm_count) * 16) blocks = int64_t(ctx->sm_count) * 16;
-    count_zeros_kernel<<<unsigned(blocks), 256, 0, stream>>>(X, ldX, B, n, out, ld_out);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        count_zeros_kernel<<<capped_grid(ctx, B, 8, 16), 256, 0, stream>>>(X, ldX, B, n, out,
+                                                                           ld_out);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_chi_squared_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B, int64_t K,
@@ -238,13 +230,11 @@ int elfi_b200_chi_squared_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, 
     ELFI_REQUIRE(B >= 0 && K >= 1 && K <= LEAF_MAX_TERMS && ldS >= K,
                  "chi_squared: bad shape (1 <= K <= %d; K=%lld)", LEAF_MAX_TERMS, (long long)K);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    int64_t blocks = (B + 255) / 256;
-    if (blocks > int64_t(ctx->sm_count) * 16) blocks = int64_t(ctx->sm_count) * 16;
-    chi_squared_kernel<<<unsigned(blocks), 256, 0, stream>>>(S, ldS, B, int(K), obs, out);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        chi_squared_kernel<<<capped_grid(ctx, B, 256, 16), 256, 0, stream>>>(S, ldS, B, int(K), obs,
+                                                                             out);
+        return ELFI_B200_OK;
+    });
 }
 
 }  // extern "C"

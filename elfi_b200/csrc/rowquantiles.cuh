@@ -3,7 +3,8 @@
 // volatility model's fused kurtosis and skewness (svm.cu).  The row's n <= MG1_NOBS_MAX keys
 // (bitonic.cuh's order-preserving u64, padding ~0) are sorted by bitonic_in_registers; lane k then
 // picks and interpolates level k (mg1.cuh's toad_quantile_pick and gnk_lerp).  A row containing NaN
-// has every quantile NaN (NaN sorts last, NumPy checks the last element).
+// has every quantile NaN (NaN sorts last, NumPy checks the last element).  kpl_for also sizes the
+// register rows of the g-and-k summaries (gnkstats.cu).
 #pragma once
 
 #include <string.h>
@@ -17,11 +18,33 @@ struct QuantileLevels {
     double q[MG1_NQ_MAX];
 };
 
-// keys per lane of a row of n <= MG1_NOBS_MAX values: the power of two with 32 * kpl >= n
-static inline int quantile_kpl(int n) {
-    int kpl = 1;
+// keys per lane of a row of n values that a warp holds in registers: the least power of two
+// kpl >= min_kpl with 32 * kpl >= n
+static inline int kpl_for(int n, int min_kpl) {
+    int kpl = min_kpl;
     while (32 * kpl < n) kpl <<= 1;
     return kpl;
+}
+
+// The per-warp strips of the one-thread-per-row simulators (mg1.cu, svm.cu): thread r of a warp
+// writes its row of n values to strip[r * npad + j], npad = n | 1 (an odd stride: no bank
+// conflicts), and a block of 32 * warps threads has as many warps (1 .. warps_max) as fit in
+// `budget` bytes of shared memory.
+struct WarpStrips {
+    int npad, warps;
+    size_t smem;        // dynamic shared memory of a block
+    unsigned blocks;    // blocks that cover B rows
+};
+
+static inline WarpStrips warp_strips(int64_t B, int n, size_t budget, int warps_max) {
+    WarpStrips s;
+    s.npad = n | 1;
+    const size_t warp_bytes = size_t(32) * s.npad * sizeof(double);
+    const int warps = int(budget / warp_bytes);
+    s.warps = warps < 1 ? 1 : (warps > warps_max ? warps_max : warps);
+    s.smem = s.warps * warp_bytes;
+    s.blocks = unsigned((B + 32 * s.warps - 1) / (32 * s.warps));
+    return s;
 }
 
 // the levels as the kernels take them; false if one lies outside [0, 1] (or is NaN)

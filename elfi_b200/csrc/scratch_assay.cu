@@ -195,8 +195,6 @@ int elfi_b200_sim_scratch_assay_f64(elfi_b200_ctx* ctx, const double* P, int64_t
                  (long long)B, (long long)nrows, (long long)ncols, (long long)num_iter,
                  (long long)obs_interval, (long long)ldS);
     if (B == 0 || (S == nullptr && X == nullptr)) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     SaSim a;
     a.P = P;
     a.ldP = ldP;
@@ -213,9 +211,10 @@ int elfi_b200_sim_scratch_assay_f64(elfi_b200_ctx* ctx, const double* P, int64_t
     a.X = X;
     const size_t smem = size_t(SA_WARPS) * sa_row_words(int(nrows * ncols)) * sizeof(uint32_t);
     const unsigned blocks = unsigned((B + SA_WARPS - 1) / SA_WARPS);
-    sim_scratch_assay_kernel<<<blocks, 32 * SA_WARPS, smem, stream>>>(a);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        sim_scratch_assay_kernel<<<blocks, 32 * SA_WARPS, smem, stream>>>(a);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_scratch_assay_summaries_f64(elfi_b200_ctx* ctx, const uint8_t* X, int64_t ld_b,
@@ -230,14 +229,12 @@ int elfi_b200_scratch_assay_summaries_f64(elfi_b200_ctx* ctx, const uint8_t* X, 
                  "n_frames; nrows=%lld ncols=%lld n_frames=%lld ldS=%lld)", (long long)nrows,
                  (long long)ncols, (long long)n_frames, (long long)ldS);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    int64_t blocks = (B * n_frames + SA_SUMM_THREADS - 1) / SA_SUMM_THREADS;
-    if (blocks > int64_t(ctx->sm_count) * 32) blocks = int64_t(ctx->sm_count) * 32;
-    scratch_assay_summaries_kernel<<<unsigned(blocks), SA_SUMM_THREADS, 0, stream>>>(
-        X, ld_b, ld_r, ld_c, ld_k, B, int(nrows), int(ncols), int(n_frames), S, ldS);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        const unsigned blocks = capped_grid(ctx, B * n_frames, SA_SUMM_THREADS, 32);
+        scratch_assay_summaries_kernel<<<blocks, SA_SUMM_THREADS, 0, stream>>>(
+            X, ld_b, ld_r, ld_c, ld_k, B, int(nrows), int(ncols), int(n_frames), S, ldS);
+        return ELFI_B200_OK;
+    });
 }
 
 }  // extern "C"

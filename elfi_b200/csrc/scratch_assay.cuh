@@ -38,6 +38,7 @@
 
 #include <stdint.h>
 
+#include "hd.cuh"
 #include "leafsum.cuh"
 #include "philox.cuh"
 

@@ -540,11 +540,11 @@ int elfi_b200_prior_ma2_f64(elfi_b200_ctx* ctx, int64_t B, uint64_t seed, uint64
     ELFI_REQUIRE(ctx && mode >= 0 && mode <= 2, "prior_ma2: bad argument");
     ELFI_REQUIRE(B == 0 || (t1 && (mode == 1 || t2)), "prior_ma2: NULL argument");
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    prior_ma2_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(B, seed, offset, mode, t1, t2);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        prior_ma2_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(B, seed, offset, mode, t1,
+                                                                        t2);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_logprior_ma2_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int64_t B,
@@ -552,11 +552,10 @@ int elfi_b200_logprior_ma2_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx,
     using namespace elfi;
     ELFI_REQUIRE(ctx && (B == 0 || (x && out)) && ldx >= 2, "logprior_ma2: bad argument");
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    logprior_ma2_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(x, ldx, B, out);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        logprior_ma2_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(x, ldx, B, out);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_sim_ma2_f64(elfi_b200_ctx* ctx, const double* t1, const double* t2, int64_t B,
@@ -569,29 +568,27 @@ int elfi_b200_sim_ma2_f64(elfi_b200_ctx* ctx, const double* t1, const double* t2
     ELFI_REQUIRE(X || S, "sim_ma2: nothing to produce (X and S are both NULL)");
     ELFI_REQUIRE((!X || ldX >= n_obs) && (!S || ldS >= 2), "sim_ma2: bad leading dimension");
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     const unsigned blocks = unsigned((B + 127) / 128);
     const bool leaf = n_obs - 1 <= LEAF_MAX_TERMS && getenv("ELFI_B200_SIM_MA2_TREE") == nullptr;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
 #define ELFI_SIM_MA2(WX, SM, LF) \
     sim_ma2_kernel<WX, SM, LF><<<blocks, 128, 0, stream>>>(t1, t2, B, int(n_obs), seed, offset, X, ldX, S, ldS)
-    if (X && S) { if (leaf) ELFI_SIM_MA2(true, true, true); else ELFI_SIM_MA2(true, true, false); }
-    else if (X) ELFI_SIM_MA2(true, false, false);
-    else { if (leaf) ELFI_SIM_MA2(false, true, true); else ELFI_SIM_MA2(false, true, false); }
+        if (X && S) { if (leaf) ELFI_SIM_MA2(true, true, true); else ELFI_SIM_MA2(true, true, false); }
+        else if (X) ELFI_SIM_MA2(true, false, false);
+        else { if (leaf) ELFI_SIM_MA2(false, true, true); else ELFI_SIM_MA2(false, true, false); }
 #undef ELFI_SIM_MA2
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_gm_cdf_f64(elfi_b200_ctx* ctx, const double* weights, int64_t N, double* cumw,
                          void* stream_) {
     using namespace elfi;
     ELFI_REQUIRE(ctx && cumw && N >= 1, "gm_cdf: bad argument");
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    cumsum_kernel<<<1, 1024, 0, stream>>>(weights, N, cumw);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        cumsum_kernel<<<1, 1024, 0, stream>>>(weights, N, cumw);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_gm_rvs_cdf_f64(elfi_b200_ctx* ctx, const double* means, int64_t ldm, const double* cumw,
@@ -629,38 +626,36 @@ int elfi_b200_gm_rvs_cdf_f64(elfi_b200_ctx* ctx, const double* means, int64_t ld
         if (support == 2)
             for (int a = 0; a < p; ++a) { box16.lo[a] = box_host[a]; box16.hi[a] = box_host[p + a]; }
         if (B == 0) return ELFI_B200_OK;
-        cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-        ELFI_CUDA_OK(cudaSetDevice(ctx->device));
         PackedLower16 Lp;
         memset(&Lp, 0, sizeof(Lp));
         for (int a = 0; a < p; ++a)
             for (int b = 0; b <= a; ++b) Lp.v[a * (a + 1) / 2 + b] = Lchol_host[a * p + b];
+        return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
 #define ELFI_GM_RVS_WIDE(PMAX, COND)                                                             \
-        gm_rvs_wide_kernel<PMAX, COND><<<unsigned((B + 127) / 128), 128, 0, stream>>>(            \
-            means, ldm, cumw, N, int(p), Lp, B, seed, offset, support, box16, prior, out, ldo)
-        if (p <= 4) { if (cond) ELFI_GM_RVS_WIDE(4, true); else ELFI_GM_RVS_WIDE(4, false); }
-        else if (p <= 8) { if (cond) ELFI_GM_RVS_WIDE(8, true); else ELFI_GM_RVS_WIDE(8, false); }
-        else if (cond) ELFI_GM_RVS_WIDE(16, true);
-        else ELFI_GM_RVS_WIDE(16, false);
+            gm_rvs_wide_kernel<PMAX, COND><<<unsigned((B + 127) / 128), 128, 0, stream>>>(        \
+                means, ldm, cumw, N, int(p), Lp, B, seed, offset, support, box16, prior, out, ldo)
+            if (p <= 4) { if (cond) ELFI_GM_RVS_WIDE(4, true); else ELFI_GM_RVS_WIDE(4, false); }
+            else if (p <= 8) { if (cond) ELFI_GM_RVS_WIDE(8, true); else ELFI_GM_RVS_WIDE(8, false); }
+            else if (cond) ELFI_GM_RVS_WIDE(16, true);
+            else ELFI_GM_RVS_WIDE(16, false);
 #undef ELFI_GM_RVS_WIDE
-        ELFI_CUDA_OK(cudaGetLastError());
-        return ELFI_B200_OK;
+            return ELFI_B200_OK;
+        });
     }
     BoxSupport box;
     memset(&box, 0, sizeof(box));
     if (support == 2)
         for (int a = 0; a < p; ++a) { box.lo[a] = box_host[a]; box.hi[a] = box_host[p + a]; }
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     LowerFactor4 Lc;
     memset(&Lc, 0, sizeof(Lc));
     for (int a = 0; a < p; ++a)
         for (int b = 0; b <= a; ++b) Lc.v[a * p + b] = Lchol_host[a * p + b];
-    gm_rvs_kernel<<<unsigned((B + 127) / 128), 128, 0, stream>>>(means, ldm, cumw, N, int(p), Lc, B,
-                                                                seed, offset, support, box, out, ldo);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        gm_rvs_kernel<<<unsigned((B + 127) / 128), 128, 0, stream>>>(
+            means, ldm, cumw, N, int(p), Lc, B, seed, offset, support, box, out, ldo);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_gm_rvs_f64(elfi_b200_ctx* ctx, const double* means, int64_t ldm, const double* weights,
@@ -670,13 +665,14 @@ int elfi_b200_gm_rvs_f64(elfi_b200_ctx* ctx, const double* means, int64_t ldm, c
     using namespace elfi;
     ELFI_REQUIRE(ctx && N >= 1, "gm_rvs: bad argument");
     if (B == 0) return ELFI_B200_OK;
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    double* cumw = static_cast<double*>(ctx_scratch(ctx, size_t(N) * 8 + 256));
-    if (!cumw) return ELFI_B200_ERR_NOMEM;
-    int rc = elfi_b200_gm_cdf_f64(ctx, weights, N, cumw, stream_);
-    if (rc != ELFI_B200_OK) return rc;
-    return elfi_b200_gm_rvs_cdf_f64(ctx, means, ldm, cumw, N, p, Lchol_host, B, seed, offset, support,
-                                    box_host, out, ldo, stream_);
+    return run_on_device(ctx, stream_, [&](cudaStream_t) {
+        double* cumw = static_cast<double*>(ctx_scratch(ctx, size_t(N) * 8 + 256));
+        if (!cumw) return ELFI_B200_ERR_NOMEM;
+        int rc = elfi_b200_gm_cdf_f64(ctx, weights, N, cumw, stream_);
+        if (rc != ELFI_B200_OK) return rc;
+        return elfi_b200_gm_rvs_cdf_f64(ctx, means, ldm, cumw, N, p, Lchol_host, B, seed, offset,
+                                        support, box_host, out, ldo, stream_);
+    });
 }
 
 static elfi::GaussPrior make_gauss_prior(const double* prm) {
@@ -698,12 +694,11 @@ int elfi_b200_prior_gauss_f64(elfi_b200_ctx* ctx, int64_t B, uint64_t seed, uint
     ELFI_REQUIRE(ctx && prm_host && (B == 0 || (mu && sigma)), "prior_gauss: NULL argument");
     ELFI_REQUIRE(prm_host[1] > 0 && prm_host[3] > prm_host[2], "prior_gauss: bad prior parameters");
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    prior_gauss_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(B, seed, offset,
-                                                                     make_gauss_prior(prm_host), mu, sigma);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        prior_gauss_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(
+            B, seed, offset, make_gauss_prior(prm_host), mu, sigma);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_logprior_gauss_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int64_t B,
@@ -711,12 +706,11 @@ int elfi_b200_logprior_gauss_f64(elfi_b200_ctx* ctx, const double* x, int64_t ld
     using namespace elfi;
     ELFI_REQUIRE(ctx && prm_host && (B == 0 || (x && out)) && ldx >= 2, "logprior_gauss: bad argument");
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    logprior_gauss_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(x, ldx, B,
-                                                                        make_gauss_prior(prm_host), out);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        logprior_gauss_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(
+            x, ldx, B, make_gauss_prior(prm_host), out);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_sim_gauss_f64(elfi_b200_ctx* ctx, const double* mu, const double* sigma, int64_t B,
@@ -729,17 +723,16 @@ int elfi_b200_sim_gauss_f64(elfi_b200_ctx* ctx, const double* mu, const double* 
     ELFI_REQUIRE(Y || S, "sim_gauss: nothing to produce (Y and S are both NULL)");
     ELFI_REQUIRE((!Y || ldY >= n_obs) && (!S || ldS >= 2), "sim_gauss: bad leading dimension");
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     const unsigned blocks = unsigned((B + 127) / 128);
     const bool leaf = n_obs <= LEAF_MAX_TERMS && getenv("ELFI_B200_SIM_GAUSS_TREE") == nullptr;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
 #define ELFI_SIM_GAUSS(WY, LF) \
     sim_gauss_kernel<WY, LF><<<blocks, 128, 0, stream>>>(mu, sigma, B, int(n_obs), seed, offset, Y, ldY, S, ldS)
-    if (Y) { if (leaf) ELFI_SIM_GAUSS(true, true); else ELFI_SIM_GAUSS(true, false); }
-    else { if (leaf) ELFI_SIM_GAUSS(false, true); else ELFI_SIM_GAUSS(false, false); }
+        if (Y) { if (leaf) ELFI_SIM_GAUSS(true, true); else ELFI_SIM_GAUSS(true, false); }
+        else { if (leaf) ELFI_SIM_GAUSS(false, true); else ELFI_SIM_GAUSS(false, false); }
 #undef ELFI_SIM_GAUSS
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_sim_gnk_f64(elfi_b200_ctx* ctx, const double* A, const double* Bs, const double* g,
@@ -751,15 +744,13 @@ int elfi_b200_sim_gnk_f64(elfi_b200_ctx* ctx, const double* A, const double* Bs,
                  (long long)B, (long long)n_obs);
     ELFI_REQUIRE(ldY >= n_obs, "sim_gnk: bad leading dimension");
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    const int64_t total = B * ((n_obs + 1) / 2);
-    int64_t blocks = (total + 255) / 256;
-    const int64_t cap = int64_t(ctx->sm_count) * 64;   // grid-stride beyond 8 waves of 8 CTAs/SM
-    if (blocks > cap) blocks = cap;
-    sim_gnk_kernel<<<unsigned(blocks), 256, 0, stream>>>(A, Bs, g, k, c, B, int(n_obs), seed, offset, Y, ldY);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        // grid-stride beyond 8 waves of 8 CTAs/SM
+        const unsigned blocks = capped_grid(ctx, B * ((n_obs + 1) / 2), 256, 64);
+        sim_gnk_kernel<<<blocks, 256, 0, stream>>>(A, Bs, g, k, c, B, int(n_obs), seed, offset, Y,
+                                                   ldY);
+        return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_logprior_box_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int64_t B, int64_t p,
@@ -777,11 +768,11 @@ int elfi_b200_logprior_box_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx,
         box.logdens -= log(box_host[p + a]);
     }
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    logprior_box_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(x, ldx, B, int(p), box, out);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        logprior_box_kernel<<<unsigned((B + 255) / 256), 256, 0, stream>>>(x, ldx, B, int(p), box,
+                                                                           out);
+        return ELFI_B200_OK;
+    });
 }
 
 }  // extern "C"

@@ -22,6 +22,7 @@
 
 #include <math.h>
 
+#include "hd.cuh"
 #include "gnkstats.cuh"
 
 namespace elfi {

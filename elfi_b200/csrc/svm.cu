@@ -12,12 +12,13 @@
 //
 // Layout: mg1.cu's.  x_t is sequential in t, so one thread simulates one row; the quantiles need
 // the whole row sorted, which one warp does in registers.  Thread r writes its row to a per-warp
-// shared-memory strip, strip[r * npad + j] (npad = n | 1: no bank conflicts); the warp then loads
-// each row in turn, lane L taking elements k * 32 + L, sorts it (rowquantiles.cuh), lanes 0..4 pick
-// the levels 0.05, 0.25, 0.5, 0.75, 0.95 and lane 0 writes S[b, 0:2] = (kurt, skew).  The data
-// reaches HBM only when asked for, copied out of the strip row by row (coalesced).  The fused
-// summaries are those of ops.svm_summaries (row_quantiles of the data, then the same IEEE
-// arithmetic) bit for bit, as a sorted row does not depend on the order its keys came in.
+// shared-memory strip, strip[r * npad + j] (npad = n | 1: no bank conflicts; rowquantiles.cuh's
+// warp_strips, here with at most SVM_WARPS_MAX warps in SVM_STRIP_BUDGET bytes per block); the
+// warp then loads each row in turn, lane L taking elements k * 32 + L, sorts it (rowquantiles.cuh),
+// lanes 0..4 pick the levels 0.05, 0.25, 0.5, 0.75, 0.95 and lane 0 writes S[b, 0:2] = (kurt,
+// skew).  The data reaches HBM only when asked for, copied out of the strip row by row (coalesced).
+// The fused summaries are those of ops.svm_summaries (row_quantiles of the data, then the same
+// IEEE arithmetic) bit for bit, as a sorted row does not depend on the order its keys came in.
 #include "boxmuller.cuh"
 #include "common.cuh"
 #include "philox.cuh"
@@ -114,29 +115,18 @@ int elfi_b200_sim_svm_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int6
                  "B=%lld n_obs=%lld ldP=%lld)", MG1_NOBS_MIN, MG1_NOBS_MAX, SVM_NPARAMS,
                  SVM_NSUMM, (long long)B, (long long)n_obs, (long long)ldP);
     if (B == 0 || (Y == nullptr && S == nullptr)) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    const int n = int(n_obs), npad = n | 1;
-    const size_t warp_bytes = size_t(32) * npad * sizeof(double);
-    int warps = int(SVM_STRIP_BUDGET / warp_bytes);
-    warps = warps < 1 ? 1 : (warps > SVM_WARPS_MAX ? SVM_WARPS_MAX : warps);
-    const size_t smem = warps * warp_bytes;
-    const unsigned blocks = unsigned((B + 32 * warps - 1) / (32 * warps));
-#define ELFI_SIM_SVM(KPL)                                                                          \
-    ELFI_CUDA_OK(cudaFuncSetAttribute(sim_svm_kernel<KPL>,                                         \
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));    \
-    sim_svm_kernel<KPL><<<blocks, 32 * warps, smem, stream>>>(P, ldP, B, n, npad, seed, offset, Y, \
-                                                              ldY, S, ldS)
-    switch (quantile_kpl(n)) {
-    case 1: ELFI_SIM_SVM(1); break;
-    case 2: ELFI_SIM_SVM(2); break;
-    case 4: ELFI_SIM_SVM(4); break;
-    case 8: ELFI_SIM_SVM(8); break;
-    default: ELFI_SIM_SVM(16); break;
-    }
-#undef ELFI_SIM_SVM
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    const int n = int(n_obs);
+    const WarpStrips st = warp_strips(B, n, SVM_STRIP_BUDGET, SVM_WARPS_MAX);
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        return with_pow2<1, 16>(kpl_for(n, 1), [&](auto K) {
+            ELFI_CUDA_OK(cudaFuncSetAttribute(sim_svm_kernel<decltype(K)::value>,
+                                              cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              int(st.smem)));
+            sim_svm_kernel<decltype(K)::value><<<st.blocks, 32 * st.warps, st.smem, stream>>>(
+                P, ldP, B, n, st.npad, seed, offset, Y, ldY, S, ldS);
+            return ELFI_B200_OK;
+        });
+    });
 }
 
 }  // extern "C"

@@ -17,6 +17,7 @@
 
 #include <math.h>
 
+#include "hd.cuh"
 #include "gnkstats.cuh"
 #include "stable.cuh"
 #include "toad.cuh"

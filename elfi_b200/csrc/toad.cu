@@ -200,11 +200,6 @@ sim_toad_fused_kernel(const ToadSim a, const ToadSumm s, double* __restrict__ S,
     }
 }
 
-static int64_t toad_grid(elfi_b200_ctx* ctx, int64_t B, int per_sm) {
-    int64_t g = int64_t(ctx->sm_count) * per_sm;
-    return B < g ? B : g;
-}
-
 static int toad_summ_args(ToadSumm& s, int64_t n_lags, const int64_t* lags, int64_t n_p,
                           const double* p, double thd) {
     s.n_lags = int(n_lags);
@@ -241,8 +236,6 @@ int elfi_b200_sim_toad_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int
                          (long long)lags[l]);
     }
     if (B == 0 || (X == nullptr && S == nullptr)) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     ToadSim a;
     a.P = P;
     a.ldP = ldP;
@@ -253,29 +246,30 @@ int elfi_b200_sim_toad_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int
     a.offset = offset;
     ToadSumm s;
     if (S) toad_summ_args(s, n_lags, lags, n_p, p, thd);
-    if (X) {
-        const int64_t blocks = (B * n_toads + TOAD_SIM_THREADS - 1) / TOAD_SIM_THREADS;
-        ELFI_REQUIRE(blocks < (int64_t(1) << 31), "sim_toad: B * n_toads too large");
-        sim_toad_kernel<<<unsigned(blocks), TOAD_SIM_THREADS, 0, stream>>>(a, X);
-        ELFI_CUDA_OK(cudaGetLastError());
-        if (S) {
-            const int64_t nt = n_days * n_toads;
-            for (int64_t l = 0; l < n_lags; ++l) {
-                toad_summaries_kernel<<<unsigned(toad_grid(ctx, B, 8)), TOAD_THREADS, 0, stream>>>(
-                    X, n_toads, 1, nt, int(n_days), int(n_toads), B, int(lags[l]), s,
-                    S + l * (n_p + 1), ldS);
-                ELFI_CUDA_OK(cudaGetLastError());
+    const unsigned grid = capped_grid(ctx, B, 1, 8);   // a CTA per row, at most 8 per SM
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        if (X) {
+            const int64_t blocks = (B * n_toads + TOAD_SIM_THREADS - 1) / TOAD_SIM_THREADS;
+            ELFI_REQUIRE(blocks < (int64_t(1) << 31), "sim_toad: B * n_toads too large");
+            sim_toad_kernel<<<unsigned(blocks), TOAD_SIM_THREADS, 0, stream>>>(a, X);
+            ELFI_CUDA_OK(cudaGetLastError());
+            if (S) {
+                const int64_t nt = n_days * n_toads;
+                for (int64_t l = 0; l < n_lags; ++l) {
+                    toad_summaries_kernel<<<grid, TOAD_THREADS, 0, stream>>>(
+                        X, n_toads, 1, nt, int(n_days), int(n_toads), B, int(lags[l]), s,
+                        S + l * (n_p + 1), ldS);
+                    ELFI_CUDA_OK(cudaGetLastError());
+                }
             }
+            return ELFI_B200_OK;
         }
+        const size_t smem = size_t(n_days * n_toads) * sizeof(double);
+        ELFI_CUDA_OK(cudaFuncSetAttribute(sim_toad_fused_kernel,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+        sim_toad_fused_kernel<<<grid, TOAD_THREADS, smem, stream>>>(a, s, S, ldS);
         return ELFI_B200_OK;
-    }
-    const size_t smem = size_t(n_days * n_toads) * sizeof(double);
-    ELFI_CUDA_OK(cudaFuncSetAttribute(sim_toad_fused_kernel,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-    sim_toad_fused_kernel<<<unsigned(toad_grid(ctx, B, 8)), TOAD_THREADS, smem, stream>>>(a, s, S,
-                                                                                         ldS);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    });
 }
 
 int elfi_b200_toad_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_day,
@@ -292,14 +286,13 @@ int elfi_b200_toad_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld
                  TOAD_NP_MAX, (long long)n_days, (long long)n_toads, (long long)lag,
                  (long long)n_p);
     if (B == 0) return ELFI_B200_OK;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
     ToadSumm s;
     toad_summ_args(s, 1, &lag, n_p, p, thd);
-    toad_summaries_kernel<<<unsigned(toad_grid(ctx, B, 8)), TOAD_THREADS, 0, stream>>>(
-        X, ld_day, ld_toad, ld_row, int(n_days), int(n_toads), B, int(lag), s, S, ldS);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
+    return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
+        toad_summaries_kernel<<<capped_grid(ctx, B, 1, 8), TOAD_THREADS, 0, stream>>>(
+            X, ld_day, ld_toad, ld_row, int(n_days), int(n_toads), B, int(lag), s, S, ldS);
+        return ELFI_B200_OK;
+    });
 }
 
 }  // extern "C"

@@ -15,6 +15,7 @@
 
 #include <stdint.h>
 
+#include "hd.cuh"
 #include "leafsum.cuh"
 
 namespace elfi {

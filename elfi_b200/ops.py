@@ -32,6 +32,42 @@ def _ld(t):
     return t.stride(0) if t.shape[0] > 1 else t.shape[1]
 
 
+def _params(params, model, names):
+    """The (batch, p) parameter matrix of a model whose p parameters are ``names``."""
+    P = _matrix(params)
+    if P.shape[1] != len(names):
+        raise ValueError('the {} model has {} parameters ({}), got a parameter width of {}'.format(
+            model, len(names), ', '.join(names), P.shape[1]))
+    return P
+
+
+def _axes(x, name, layout):
+    if x.dim() != len(layout) or any(isinstance(a, int) and a != n
+                                     for a, n in zip(layout, x.shape)):
+        raise ValueError('{} takes ({}) data, got shape {}'.format(
+            name, ', '.join(str(a) for a in layout), tuple(x.shape)))
+    return x
+
+
+def _data(x, name, layout):
+    """x as float64 device data with the axes ``layout`` (an int is a required size): device float64
+    data is read in place, whatever its strides; anything else is uploaded."""
+    if not (dev.is_device_array(x) and x.dtype == torch.float64):
+        x = dev.to_device(x)
+    return _axes(x, name, layout)
+
+
+def _mask(x, name, layout):
+    """x as bool or uint8 device data with the axes ``layout``, nonzero meaning set: such device
+    data is read in place, whatever its strides; other device data is compared with 0, host data
+    is uploaded first."""
+    if not dev.is_device_array(x):
+        x = dev.to_device(np.asarray(x, dtype=np.float64))
+    if x.dtype not in (torch.bool, torch.uint8):
+        x = x != 0
+    return _axes(x, name, layout)
+
+
 def _dist_prepare(S, obs, thresholds, K=1, want_indices=True, device_thresholds=False):
     """What the device distance wrappers share: the matrix, ``obs`` flattened and checked against
     its width, the K thresholds as a host float64 array (or None) -- or left as a device tensor
@@ -1051,14 +1087,6 @@ LORENZ_SUMM_MAX_TERMS = 30728                 # n_timestep * n_obs of the summar
 LORENZ_NSUMM = 6
 
 
-def _lorenz_params(params):
-    P = _matrix(params)
-    if P.shape[1] != 2:
-        raise ValueError('the Lorenz model has 2 parameters (theta1, theta2), got a parameter width '
-                         'of {}'.format(P.shape[1]))
-    return P
-
-
 def sim_lorenz(params, n_timestep=160, initial_state=None, f=10., phi=0.984, total_duration=4.,
                seed=0, offset=0, want_data=False, want_summaries=True):
     """Stochastic Lorenz 96 forecast model on the device (elfi/examples/lorenz.py:94-163).
@@ -1089,7 +1117,7 @@ def sim_lorenz(params, n_timestep=160, initial_state=None, f=10., phi=0.984, tot
     if want_summaries and n_timestep * m > LORENZ_SUMM_MAX_TERMS:
         raise ValueError('the device Lorenz summaries take n_timestep * n_obs <= {}, got {} * {}'
                          .format(LORENZ_SUMM_MAX_TERMS, n_timestep, m))
-    P = _lorenz_params(params)
+    P = _params(params, 'Lorenz', ('theta1', 'theta2'))
     B = P.shape[0]
     dt = total_duration / n_timestep
     with np.errstate(invalid='ignore'):
@@ -1107,10 +1135,7 @@ def lorenz_summaries(x):
     (elfi/examples/lorenz.py:231-320) of device data x (B, n_timestep, n_obs), any strides: a
     (B, 6) tensor, bit for bit NumPy's on the C-contiguous array.  2 <= n_timestep,
     2 <= n_obs <= 128, n_timestep * n_obs <= LORENZ_SUMM_MAX_TERMS."""
-    x = dev.to_device(x) if not (dev.is_device_array(x) and x.dtype == torch.float64) else x
-    if x.dim() != 3:
-        raise ValueError('lorenz_summaries takes (batch, n_timestep, n_obs) data, got shape {}'
-                         .format(tuple(x.shape)))
+    x = _data(x, 'lorenz_summaries', ('batch', 'n_timestep', 'n_obs'))
     B, T, m = x.shape
     if not LORENZ_SUMM_NOBS_MIN <= m <= LORENZ_NOBS_MAX or T < 2 or T * m > LORENZ_SUMM_MAX_TERMS:
         raise ValueError('lorenz_summaries takes {} <= n_obs <= {}, 2 <= n_timestep and n_timestep * '
@@ -1179,10 +1204,7 @@ def sim_toad(params, n_toads=66, n_days=63, seed=0, offset=0, want_data=False, l
         lag_arr = np.array([_toad_lag(lag, n_days) for lag in lags], dtype=np.int64)
         _toad_disp(n_toads, n_days - 1)
         pv = _toad_p(p)
-    P = _matrix(params)
-    if P.shape[1] != 3:
-        raise ValueError('the toad model has 3 parameters (alpha, gamma, p0), got a parameter '
-                         'width of {}'.format(P.shape[1]))
+    P = _params(params, 'toad', ('alpha', 'gamma', 'p0'))
     B = P.shape[0]
     X = dev.empty((B, n_days, n_toads)) if want_data else None
     w = len(lags) * (pv.size + 1) if lags else 0
@@ -1198,10 +1220,7 @@ def toad_summaries(x, lag, p=np.linspace(0, 1, 11), thd=10.):
     any strides: a (batch, len(p) + 1) tensor [number of returns, median, len(p) - 1 log gaps], bit
     for bit NumPy's except that the logs use the device's log.  1 <= lag < n_days, n_toads *
     (n_days - lag) <= TOAD_DISP_MAX, 1 <= len(p) <= TOAD_NP_MAX levels in [0, 1]."""
-    x = dev.to_device(x) if not (dev.is_device_array(x) and x.dtype == torch.float64) else x
-    if x.dim() != 3:
-        raise ValueError('toad_summaries takes (n_days, n_toads, batch) data, got shape {}'.format(
-            tuple(x.shape)))
+    x = _data(x, 'toad_summaries', ('n_days', 'n_toads', 'batch'))
     n_days, n_toads, B = x.shape
     lag = _toad_lag(lag, n_days)
     _toad_disp(n_toads, n_days - lag)
@@ -1244,10 +1263,7 @@ def sim_lotka_volterra(params, n_obs=16, time_end=30., seed=0, offset=0, max_eve
     if int(max_events) != max_events or not 1 <= max_events <= LV_MAX_EVENTS_LIMIT:
         raise ValueError('max_events must be an integer with 1 <= max_events <= {} (the event '
                          'index is one Philox word), got {}'.format(LV_MAX_EVENTS_LIMIT, max_events))
-    P = _matrix(params)
-    if P.shape[1] != 6:
-        raise ValueError('the Lotka-Volterra model has 6 parameters (r1, r2, r3, prey0, predator0, '
-                         'sigma), got a parameter width of {}'.format(P.shape[1]))
+    P = _params(params, 'Lotka-Volterra', ('r1', 'r2', 'r3', 'prey0', 'predator0', 'sigma'))
     B = P.shape[0]
     t_out = dev.to_device(np.linspace(0, time_end, n_obs))
     obs = dev.empty((B, n_obs, 2))
@@ -1264,10 +1280,7 @@ def lv_summaries(x):
     pred_log_var, prey_autocorr_1, pred_autocorr_1, prey_autocorr_2, pred_autocorr_2, crosscorr],
     bit for bit NumPy's except that log(var + 1) uses the device's log.
     LV_SUMM_NOBS_MIN <= n_obs <= LV_SUMM_NOBS_MAX."""
-    x = dev.to_device(x) if not (dev.is_device_array(x) and x.dtype == torch.float64) else x
-    if x.dim() != 3 or x.shape[2] != 2:
-        raise ValueError('lv_summaries takes (batch, n_obs, 2) data, got shape {}'.format(
-            tuple(x.shape)))
+    x = _data(x, 'lv_summaries', ('batch', 'n_obs', 2))
     B, n_obs = x.shape[0], x.shape[1]
     if not LV_SUMM_NOBS_MIN <= n_obs <= LV_SUMM_NOBS_MAX:
         raise ValueError('the device Lotka-Volterra summaries take {} <= n_obs <= {}, got {}'.format(
@@ -1325,10 +1338,7 @@ def sim_daycare(params, n_dcc=29, n_ind=53, n_strains=33, freq_strains_commun=No
             n_strains, f.size))
     if not (np.all(np.isfinite(f)) and np.all(f >= 0)):
         raise ValueError('freq_strains_commun must be finite and >= 0, got {}'.format(f))
-    P = _matrix(params)
-    if P.shape[1] != 3:
-        raise ValueError('the day care model has 3 parameters (t1, t2, t3), got a parameter width '
-                         'of {}'.format(P.shape[1]))
+    P = _params(params, 'day care', ('t1', 't2', 't3'))
     B = P.shape[0]
     if B > DC_BATCH_MAX:
         raise ValueError('the device day care simulator takes at most {} rows per call, got '
@@ -1348,13 +1358,7 @@ def daycare_summaries(data):
     n_strains), any strides, nonzero meaning a carrier: a (batch, 4 n_dcc) tensor in column blocks
     [Shannon | n_strains | prevalence | multi], bit for bit NumPy's except that Shannon uses the
     device's log.  n_strains <= DC_SUMM_STRAINS_MAX."""
-    if not dev.is_device_array(data):
-        data = dev.to_device(np.asarray(data, dtype=np.float64))
-    if data.dtype not in (torch.bool, torch.uint8):
-        data = data != 0
-    if data.dim() != 4:
-        raise ValueError('daycare_summaries takes (batch, n_dcc, n_obs, n_strains) data, got shape '
-                         '{}'.format(tuple(data.shape)))
+    data = _mask(data, 'daycare_summaries', ('batch', 'n_dcc', 'n_obs', 'n_strains'))
     B, n_dcc, n_obs, n_strains = (int(v) for v in data.shape)
     if n_dcc < 1 or n_obs < 1 or not 1 <= n_strains <= DC_SUMM_STRAINS_MAX:
         raise ValueError('the device day care summaries take n_dcc, n_obs >= 1 and 1 <= n_strains '
@@ -1432,10 +1436,7 @@ def sim_arch(params, n_obs=100, n_lags=5, seed=0, offset=0, want_data=False, wan
     arch_nsumm(n_lags)) its summaries [MU, VAR, AC_1 .. AC_L, PW in itertools.combinations order],
     computed in the simulator without writing Y, bit for bit :func:`arch_summaries` of Y."""
     n_obs, n_lags = _arch_shape(n_obs, n_lags, 'the device ARCH simulator and its summaries')
-    P = _matrix(params)
-    if P.shape[1] != 2:
-        raise ValueError('the ARCH model has 2 parameters (t1, t2), got a parameter width of {}'
-                         .format(P.shape[1]))
+    P = _params(params, 'ARCH', ('t1', 't2'))
     B = P.shape[0]
     K = arch_nsumm(n_lags)
     Y = dev.empty((B, n_obs)) if want_data else None
@@ -1449,10 +1450,7 @@ def arch_summaries(y, n_lags=5):
     """The ARCH summaries of elfi/examples/arch.py:135-208 for each row of device data y (batch, n),
     any strides (the reference's y[:, 1:] view included): a (batch, arch_nsumm(n_lags)) tensor
     [MU, VAR, AC_1 .. AC_L, PW_i_j in itertools.combinations order], bit for bit NumPy's."""
-    if not (dev.is_device_array(y) and y.dtype == torch.float64):
-        y = dev.to_device(y)
-    if y.dim() != 2:
-        raise ValueError('arch_summaries takes (batch, n) data, got shape {}'.format(tuple(y.shape)))
+    y = _data(y, 'arch_summaries', ('batch', 'n'))
     B = int(y.shape[0])
     n, n_lags = _arch_shape(int(y.shape[1]), n_lags, 'the device ARCH summaries')
     K = arch_nsumm(n_lags)
@@ -1496,10 +1494,7 @@ def sim_mg1(params, n_obs=50, q=np.linspace(0, 1, 10), seed=0, offset=0, want_da
     without writing Y, bit for bit :func:`row_quantiles` of Y."""
     n_obs = _mg1_n(n_obs, 'the device M/G/1 simulator and its quantiles')
     qv = _mg1_q(q)
-    P = _matrix(params)
-    if P.shape[1] != 3:
-        raise ValueError('the M/G/1 model has 3 parameters (t1, t2, t3), got a parameter width '
-                         'of {}'.format(P.shape[1]))
+    P = _params(params, 'M/G/1', ('t1', 't2', 't3'))
     B = P.shape[0]
     Y = dev.empty((B, n_obs)) if want_data else None
     S = dev.empty((B, qv.size)) if want_summaries else None
@@ -1513,10 +1508,7 @@ def row_quantiles(x, q):
     """np.quantile(x, q, axis=1).T (method 'linear') of device data x (batch, n), any strides:
     a (batch, len(q)) tensor, bit for bit NumPy's; a row containing NaN has every quantile NaN.
     Limits: 2 <= n <= MG1_NOBS_MAX, 1 <= len(q) <= MG1_NQ_MAX, q in [0, 1]."""
-    if not (dev.is_device_array(x) and x.dtype == torch.float64):
-        x = dev.to_device(x)
-    if x.dim() != 2:
-        raise ValueError('row_quantiles takes (batch, n) data, got shape {}'.format(tuple(x.shape)))
+    x = _data(x, 'row_quantiles', ('batch', 'n'))
     n = _mg1_n(int(x.shape[1]), 'the device row quantiles')
     qv = _mg1_q(q)
     B = int(x.shape[0])
@@ -1541,10 +1533,8 @@ def sim_svm(params, n_obs=50, seed=0, offset=0, want_data=False, want_summaries=
     their quantile kurtosis and skewness [kurt, skew], computed in the simulator without writing
     Y, bit for bit :func:`svm_summaries` of Y."""
     n_obs = _mg1_n(n_obs, 'the device stochastic volatility simulator and its summaries')
-    P = _matrix(params)
-    if P.shape[1] != SVM_NPARAMS:
-        raise ValueError('the stochastic volatility model has 7 parameters (alpha, beta, kappa, '
-                         'eta, mu, phi, sigma), got a parameter width of {}'.format(P.shape[1]))
+    P = _params(params, 'stochastic volatility',
+                ('alpha', 'beta', 'kappa', 'eta', 'mu', 'phi', 'sigma'))
     B = P.shape[0]
     Y = dev.empty((B, n_obs)) if want_data else None
     S = dev.empty((B, 2)) if want_summaries else None
@@ -1617,10 +1607,7 @@ def sim_scratch_assay(params, init_arr, obs_period=12, obs_interval=1 / 12, tau=
     num_iter, interval, num_obs = scratch_assay_steps(obs_period, obs_interval, tau)
     init = _scratch_init(init_arr)
     nrows, ncols = (int(v) for v in init.shape)
-    P = _matrix(params)
-    if P.shape[1] != 2:
-        raise ValueError('the scratch assay model has 2 parameters (pm, pp), got a parameter width '
-                         'of {}'.format(P.shape[1]))
+    P = _params(params, 'scratch assay', ('pm', 'pp'))
     B = P.shape[0]
     if B > SA_BATCH_MAX:
         raise ValueError('the device scratch assay simulator takes at most {} rows per call, got '
@@ -1638,13 +1625,7 @@ def scratch_assay_summaries(x):
     meaning a cell: a (batch, n_frames) float64 tensor of the n_frames - 1 mismatches between
     consecutive frames, then the cells of the last frame.  On 0 / 1 data these are NumPy's values
     exactly (they are integers)."""
-    if not dev.is_device_array(x):
-        x = dev.to_device(np.asarray(x, dtype=np.float64))
-    if x.dtype not in (torch.bool, torch.uint8):
-        x = x != 0
-    if x.dim() != 4:
-        raise ValueError('scratch_assay_summaries takes (batch, nrows, ncols, n_frames) data, got '
-                         'shape {}'.format(tuple(x.shape)))
+    x = _mask(x, 'scratch_assay_summaries', ('batch', 'nrows', 'ncols', 'n_frames'))
     B, nrows, ncols, frames = (int(v) for v in x.shape)
     if min(nrows, ncols, frames) < 1:
         raise ValueError('scratch_assay_summaries takes nrows, ncols, n_frames >= 1, got shape '
