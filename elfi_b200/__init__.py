@@ -16,5 +16,6 @@ from .samplers import (SMC, AdaptiveDistanceSMC, AdaptiveThresholdSMC,  # noqa: 
                        DensityRatioEstimation, GMDistribution, ModelPrior, Rejection)
 from .store import OutputPool  # noqa: F401
 from .priors import DeviceModelPrior  # noqa: F401
+from .bsl import BSL  # noqa: F401
 from .bo import (BOLFI, LCBSC, BayesianOptimization, BolfiPosterior, GPyRegression,  # noqa: F401
                  ExpIntVar, MaxVar, RandMaxVar, UniformAcquisition)

@@ -1,0 +1,530 @@
+"""Bayesian synthetic likelihood (Price et al. 2018) with the Gaussian likelihoods on the device.
+
+Host control flow follows the reference (paths relative to elfi-dev/elfi):
+  BSL, its Metropolis-Hastings step and logit transform   elfi/methods/inference/bsl.py
+  ModelBased (rounds of n_sim_round simulations)          elfi/methods/inference/parameter_inference.py
+  likelihoods                                             elfi/methods/bsl/pdf_methods.py
+  log_SL_stdev, select_penalty, estimate_whitening_matrix elfi/methods/bsl/pre_sample_methods.py
+What runs on the device: the simulations of a device model, the (n_sim_round, d) feature matrix
+of a round, and the whole likelihood (moments, shrinkage, whitening, Cholesky, log density:
+ops.synlik).  The host reads one value per round, for the Metropolis-Hastings step.  The
+pre-sample tools evaluate all M simulation sets, and all penalties, in one call.
+
+The standard (Warton-shrunk, whitened) and unbiased Gaussian likelihoods are provided.
+semiBSL, the R-BSL adjustments and graphical-lasso shrinkage raise NotImplementedError.  Any other
+callable likelihood is called on the host with NumPy (ssx, ssy).
+"""
+import logging
+
+import numpy as np
+import scipy.linalg
+import torch
+
+from . import device as dev
+from . import model as em
+from . import ops
+from .results import BslSample
+from .samplers import ModelPrior, ParameterInference
+
+logger = logging.getLogger(__name__)
+
+__all__ = ['BSL', 'standard_likelihood', 'unbiased_likelihood', 'semiparametric_likelihood',
+           'robust_likelihood', 'gaussian_syn_likelihood', 'gaussian_syn_likelihood_ghurye_olkin',
+           'log_SL_stdev', 'select_penalty', 'estimate_whitening_matrix']
+
+
+# ------------------------------------------------------------------------------- likelihoods
+class SyntheticLikelihood:
+    """A Gaussian synthetic likelihood evaluated by ops.synlik: estimator 'standard' (optional
+    Warton penalty and whitening matrix) or 'unbiased'.  Called with (ssx, ssy) it returns
+    np.array([ll]) like the reference's likelihoods; ``device`` keeps the result on the device."""
+
+    def __init__(self, estimator='standard', penalty=None, whitening=None):
+        if penalty is not None and not 0 <= penalty <= 1:
+            raise ValueError('The Warton penalty must lie in [0, 1], got {}'.format(penalty))
+        self.estimator = estimator
+        self.penalty = penalty
+        self.whitening = whitening
+        self._w_dev = None
+
+    def device(self, ssx, ssy, penalties=None):
+        """ll of each group of ssx ((n, d) or (G, n, d)) as a device tensor (G,), or (G, K) for
+        the K `penalties` given here in place of this likelihood's own."""
+        if self.whitening is not None and self._w_dev is None:
+            self._w_dev = dev.to_device(np.asarray(self.whitening, dtype=np.float64))
+        pen = penalties if penalties is not None else \
+            (None if self.penalty is None else [self.penalty])
+        ll = ops.synlik(ssx, ssy, estimator=self.estimator, penalties=pen, whitening=self._w_dev)
+        return ll if penalties is not None else ll.reshape(-1)
+
+    def __call__(self, ssx, ssy):
+        return np.array([float(self.device(ssx, ssy)[0].item())])
+
+    def __repr__(self):
+        return 'SyntheticLikelihood({!r}, penalty={}, whitening={})'.format(
+            self.estimator, self.penalty, None if self.whitening is None else 'W')
+
+
+def standard_likelihood(shrinkage=None, penalty=None, whitening=None, standardise=False):
+    """The standard Gaussian synthetic likelihood, with Warton shrinkage (shrinkage='warton' and a
+    penalty in [0, 1]) and whitening by a (d, d) matrix, both optional.  `standardise` belongs to
+    graphical-lasso shrinkage, which is not provided."""
+    if shrinkage == 'glasso':
+        raise NotImplementedError("shrinkage='glasso' (graphical lasso) is not provided; use "
+                                  "shrinkage='warton' or none")
+    if shrinkage not in (None, 'warton'):
+        raise ValueError("shrinkage must be None or 'warton', got {!r}".format(shrinkage))
+    if shrinkage == 'warton':
+        if penalty is None:
+            raise ValueError("shrinkage='warton' needs a penalty in [0, 1]")
+        return SyntheticLikelihood('standard', float(np.reshape(penalty, -1)[0]), whitening)
+    return SyntheticLikelihood('standard', None, whitening)
+
+
+def unbiased_likelihood():
+    """The unbiased Gaussian synthetic likelihood of Ghurye and Olkin (1969)."""
+    return SyntheticLikelihood('unbiased')
+
+
+def semiparametric_likelihood(shrinkage=None, penalty=None, whitening=None):
+    raise NotImplementedError('semiBSL (semiparametric_likelihood: the KDE marginals and the '
+                              'Gaussian copula) is not provided')
+
+
+def robust_likelihood(adjustment):
+    raise NotImplementedError('R-BSL (robust_likelihood, the {!r} adjustment and its slice '
+                              'sampler) is not provided'.format(adjustment))
+
+
+def semi_param_kernel_estimate(ssx, ssy, shrinkage=None, penalty=None, whitening=None):
+    semiparametric_likelihood()
+
+
+def syn_likelihood_misspec(ssx, ssy, gamma, adjustment):
+    robust_likelihood(adjustment)
+
+
+def gaussian_syn_likelihood(ssx, ssy, shrinkage=None, penalty=None, whitening=None,
+                            standardise=False):
+    """np.array([ll]): the standard synthetic log-likelihood of ssy under the simulated summaries
+    ssx (n, d), computed on the device (see standard_likelihood)."""
+    return standard_likelihood(shrinkage, penalty, whitening, standardise)(ssx, ssy)
+
+
+def gaussian_syn_likelihood_ghurye_olkin(ssx, ssy):
+    """np.array([ll]): the unbiased synthetic log-likelihood, computed on the device."""
+    return unbiased_likelihood()(ssx, ssy)
+
+
+def _device_likelihood(likelihood):
+    """The SyntheticLikelihood a likelihood argument stands for, or None for a host callable."""
+    if likelihood is None or likelihood is gaussian_syn_likelihood:
+        return SyntheticLikelihood('standard')
+    if likelihood is gaussian_syn_likelihood_ghurye_olkin:
+        return SyntheticLikelihood('unbiased')
+    if isinstance(likelihood, SyntheticLikelihood):
+        return likelihood
+    return None
+
+
+# ------------------------------------------------------------------------------- features
+def _feature_columns(batch, names, rows):
+    """The outputs `names` of a batch as 2-d float64 device blocks of `rows` rows, in order (the
+    columns of batch_to_arr2d): lazy simulations are materialised, host arrays uploaded."""
+    blocks = []
+    for name in names:
+        v = batch[name]
+        if hasattr(v, 'materialize'):
+            v = v.materialize()
+        t = v if dev.is_device_array(v) else dev.to_device(np.asarray(v, dtype=np.float64))
+        if t.dtype != torch.float64:
+            t = t.to(torch.float64)
+        if t.dim() == 1:
+            t = t[:, None]
+        if t.dim() != 2 or t.shape[0] != rows:
+            raise ValueError('Feature {} must be a ({}, k) array per batch, got shape {}'.format(
+                name, rows, tuple(t.shape)))
+        blocks.append(t)
+    return blocks
+
+
+def _simulate_features(model, n_sim, feature_names, params, seed):
+    """(n_sim, d) device matrix of the features simulated at params (model.generate)."""
+    out = model.generate(n_sim, outputs=list(feature_names), with_values=params, seed=seed)
+    blocks = _feature_columns(out, feature_names, n_sim)
+    return blocks[0] if len(blocks) == 1 else torch.cat(blocks, dim=1)
+
+
+def _observed_row(model, feature_names):
+    return np.column_stack([dev.to_host(model[node].observed) for node in feature_names])
+
+
+def _param_values(model, theta):
+    return theta if isinstance(theta, dict) else dict(zip(model.parameter_names, theta))
+
+
+def _names(feature_names):
+    return [feature_names] if isinstance(feature_names, str) else list(feature_names)
+
+
+# ------------------------------------------------------------------------------- sampler
+class BSL(ParameterInference):
+    """Bayesian synthetic likelihood with a random-walk Metropolis-Hastings sampler (Price et al.
+    2018).  Each round simulates n_sim_round times at one parameter; the round's features stay on
+    the device and go to one likelihood call.  Runs on this rank only."""
+
+    def __init__(self, model, n_sim_round, feature_names=None, likelihood=None, batch_size=None,
+                 seed=None, pool=None):
+        model = model.model if isinstance(model, em.NodeReference) else model
+        self.n_sim_round = int(n_sim_round)
+        batch_size = batch_size or self.n_sim_round
+        if self.n_sim_round % batch_size != 0:
+            raise ValueError('n_sim_round must be a multiple of batch_size.')
+        feature_names = _names(feature_names) if feature_names else [
+            node for node in model.nodes
+            if isinstance(model[node], em.Summary) and not node.startswith('_')]
+        if not feature_names:
+            raise ValueError('feature_names must include at least one item.')
+        for node in feature_names:
+            if node not in model.nodes:
+                raise ValueError('Node {} not found in the model'.format(node))
+        self.feature_names = feature_names
+        super().__init__(model, model.parameter_names + feature_names, batch_size=batch_size,
+                         seed=seed, pool=pool, distributed=False)
+        self.observed = _observed_row(self.model, feature_names)
+        d = self.observed.size
+        if not 1 <= d <= ops.SYNLIK_D_MAX:
+            raise ValueError('BSL takes 1 to {} features, got {}'.format(ops.SYNLIK_D_MAX, d))
+        self.random_state = np.random.RandomState(self.seed)
+        self.likelihood = likelihood
+        self._device_lik = _device_likelihood(likelihood)
+        self._obs_dev = None
+        self._sim = None                  # (n_sim_round, d) device features of the round
+        self.state['round'] = 0
+        self.state['n_sim_round'] = 0
+        self.param_names = None
+        self.prior = None
+        self.sigma_proposals = None
+        self.burn_in = 0
+        self.logit_transform_bound = None
+
+    @property
+    def parameter_names(self):
+        return self.param_names or self.model.parameter_names
+
+    def sample(self, n_samples, sigma_proposals, params0=None, param_names=None, burn_in=0,
+               logit_transform_bound=None):
+        """Run a chain of n_samples iterations (burn-in included) from params0 with Gaussian
+        random-walk proposals of covariance sigma_proposals, in the logit-transformed space when
+        logit_transform_bound ((p, 2) lower and upper bounds) is given.  Returns a BslSample."""
+        self.sigma_proposals = sigma_proposals
+        self.param_names = param_names
+        self.prior = ModelPrior(self.model, parameter_names=self.parameter_names)
+        self.burn_in = burn_in
+        self.logit_transform_bound = None if logit_transform_bound is None else \
+            np.array(logit_transform_bound)
+        self._init_state(n_samples, params0)
+        return self.infer(n_samples)
+
+    def _init_state(self, n_samples, params0=None):
+        self.state['n_batches'] = 0
+        self.state['n_sim'] = 0
+        self.state['round'] = 0
+        self.state['n_sim_round'] = 0
+        if params0 is None:
+            drawn = self.model.generate(1, self.parameter_names, seed=self.seed)
+            params0 = np.column_stack([dev.to_host(drawn[p]) for p in self.parameter_names])
+        else:
+            params0 = np.array(params0)
+            if not np.isfinite(self.prior.logpdf(params0)):
+                raise ValueError('Initial point {} is outside prior support.'.format(params0))
+        self.state['n_samples'] = 0
+        self.num_accepted = 0
+        self.state['params'] = np.zeros((n_samples, len(self.parameter_names)))
+        self.state['params'][0] = params0
+        self.state['logprior'] = np.zeros(n_samples)
+        self.state['logprior'][0] = np.reshape(self.prior.logpdf(params0), -1)[0]
+        self.state['logposterior'] = np.zeros(n_samples)
+
+    def set_objective(self, rounds):
+        self.objective['round'] = rounds
+        self.objective['n_batches'] = rounds * (self.n_sim_round // self.batch_size)
+
+    def infer(self, *args, **kwargs):
+        if self.state['round'] > 0:
+            self._init_round()
+        return super().infer(*args, **kwargs)
+
+    @property
+    def current_params(self):
+        return self.state['params'][self.state['n_samples']]
+
+    def prepare_new_batch(self, batch_index):
+        params = np.repeat(np.atleast_2d(self.current_params), self.batch_size, axis=0)
+        return {p: params[:, i] for i, p in enumerate(self.parameter_names)}
+
+    def update(self, batch, batch_index):
+        super().update(batch, batch_index)
+        self._merge_batch(batch)
+        if self.state['n_sim_round'] == self.n_sim_round:
+            self._process_simulated()
+            self.state['round'] += 1
+            if self.state['round'] < self.objective['round']:
+                self._init_round()
+
+    def _merge_batch(self, batch):
+        if self._sim is None:
+            self._sim = dev.empty((self.n_sim_round, self.observed.size))
+        row = self.state['n_sim_round']
+        col = 0
+        for block in _feature_columns(batch, self.feature_names, self.batch_size):
+            w = int(block.shape[1])
+            if col + w > self._sim.shape[1]:
+                raise ValueError('The features are wider than their observed values ({})'.format(
+                    self._sim.shape[1]))
+            self._sim[row:row + self.batch_size, col:col + w] = block
+            col += w
+        if col != self._sim.shape[1]:
+            raise ValueError('The features have {} columns, their observed values {}'.format(
+                col, self._sim.shape[1]))
+        self.state['n_sim_round'] += self.batch_size
+
+    def _loglikelihood(self):
+        if self._device_lik is not None:
+            if self._obs_dev is None:
+                self._obs_dev = dev.to_device(self.observed.reshape(-1))
+            # the one device-to-host read of the round
+            return float(self._device_lik.device(self._sim, self._obs_dev)[0].item())
+        sim = dev.to_host(self._sim)
+        if not np.all(np.isfinite(sim)):
+            return -np.inf
+        return float(np.reshape(self.likelihood(sim, self.observed), -1)[0])
+
+    def _process_simulated(self):
+        loglikelihood = self._loglikelihood()
+        n = self.state['n_samples']
+        if not np.isfinite(loglikelihood):
+            if n == 0:
+                raise RuntimeError('Estimated likelihood not finite on initialisation round.')
+            logger.warning('Estimated likelihood not finite.')
+        self.state['logposterior'][n] = loglikelihood + self.state['logprior'][n]
+        if n == 0:
+            accept = True
+        else:
+            prob = np.minimum(1.0, self._get_mh_ratio())
+            accept = self.random_state.uniform() < prob
+        if accept:
+            if n >= self.burn_in:
+                self.num_accepted += 1
+        else:
+            self._copy_previous(n)
+        self.state['n_samples'] += 1
+
+    def _copy_previous(self, n):
+        for key in ('logprior', 'params', 'logposterior'):
+            self.state[key][n] = self.state[key][n - 1]
+
+    def _init_round(self):
+        """Propose the next parameter; proposals outside the prior support are rejected without
+        simulating, and each one shortens the remaining objective by one round."""
+        while self.state['n_samples'] < len(self.state['params']):
+            n = self.state['n_samples']
+            prop = self._propagate_state()
+            logprior = np.reshape(self.prior.logpdf(prop), -1)[0]
+            if np.isfinite(logprior):
+                self.state['logprior'][n] = logprior
+                self.state['params'][n] = prop
+                self.state['n_sim_round'] = 0
+                break
+            self._copy_previous(n)
+            self.state['n_samples'] += 1
+            self.set_objective(self.objective['round'] - 1)
+
+    def _propagate_state(self):
+        mean = self.state['params'][self.state['n_samples'] - 1]
+        bound = self.logit_transform_bound
+        if bound is None:
+            prop = self.random_state.multivariate_normal(mean, self.sigma_proposals)
+        else:
+            prop = self._para_logit_back_transform(self.random_state.multivariate_normal(
+                self._para_logit_transform(mean, bound), self.sigma_proposals), bound)
+        return np.atleast_2d(prop)
+
+    def _get_mh_ratio(self):
+        n = self.state['n_samples']
+        log_ratio = self.state['logposterior'][n] - self.state['logposterior'][n - 1]
+        jac = 0
+        if self.logit_transform_bound is not None:
+            # the Jacobian terms are evaluated at the parameters themselves, as in the reference
+            jac = self._jacobian_logit_transform(self.state['params'][n], self.logit_transform_bound) \
+                - self._jacobian_logit_transform(self.state['params'][n - 1],
+                                                 self.logit_transform_bound)
+        res = jac + log_ratio
+        return np.exp(min(700, max(-700, res)))
+
+    # bound kinds: 0 both bounds finite, 1 lower infinite, 2 upper infinite, 3 both infinite
+    @staticmethod
+    def _bound_kinds(bound):
+        inf = np.isinf(np.asarray(bound, dtype=float))
+        return inf[:, 0] * 1 + inf[:, 1] * 2
+
+    @staticmethod
+    def _para_logit_transform(theta, bound):
+        """theta -> the unbounded proposal space: log((x - a) / (b - x)), log(1 / (b - x)),
+        log(x - a) or x, by which of the bounds (a, b) are finite."""
+        theta = np.asarray(theta, dtype=float).flatten()
+        kinds = BSL._bound_kinds(bound)
+        out = np.zeros(len(theta))
+        for i, (x, kind) in enumerate(zip(theta, kinds)):
+            a, b = bound[i, 0], bound[i, 1]
+            if kind == 0:
+                out[i] = np.log((x - a) / (b - x))
+            elif kind == 1:
+                out[i] = np.log(1 / (b - x))
+            elif kind == 2:
+                out[i] = np.log(x - a)
+            else:
+                out[i] = x
+        return out
+
+    @staticmethod
+    def _para_logit_back_transform(theta_tilde, bound):
+        """The inverse of _para_logit_transform."""
+        theta_tilde = np.asarray(theta_tilde, dtype=float).flatten()
+        kinds = BSL._bound_kinds(bound)
+        out = np.zeros(len(theta_tilde))
+        for i, (y, kind) in enumerate(zip(theta_tilde, kinds)):
+            a, b = bound[i, 0], bound[i, 1]
+            ey = np.exp(y)
+            if kind == 0:
+                out[i] = a / (1 + ey) + b / (1 + (1 / ey))
+            elif kind == 1:
+                out[i] = b - (1 / ey)
+            elif kind == 2:
+                out[i] = a + ey
+            else:
+                out[i] = y
+        return out
+
+    @staticmethod
+    def _jacobian_logit_transform(theta_tilde, bound):
+        """log |d theta / d theta_tilde| of the back transform, summed over the parameters."""
+        theta_tilde = np.asarray(theta_tilde, dtype=float).flatten()
+        kinds = BSL._bound_kinds(bound)
+        logj = np.zeros(len(theta_tilde))
+        for i, (y, kind) in enumerate(zip(theta_tilde, kinds)):
+            if kind == 0:
+                a, b = bound[i, 0], bound[i, 1]
+                ey = np.exp(y)
+                logj[i] = np.log(b - a) - np.log((1 / ey) + 2 + ey)
+            elif kind in (1, 2):
+                logj[i] = y
+        return np.sum(logj)
+
+    def extract_result(self):
+        samples_all = {p: np.array(self.state['params'][:, i])
+                       for i, p in enumerate(self.parameter_names)}
+        acc_rate = self.num_accepted / (self.state['n_samples'] - self.burn_in)
+        logger.info('MCMC acceptance rate: {}'.format(acc_rate))
+        return BslSample(method_name='BSL', samples_all=samples_all, acc_rate=acc_rate,
+                         burn_in=self.burn_in, n_sim=self.state['n_sim'],
+                         parameter_names=self.parameter_names)
+
+
+# ------------------------------------------------------------------------------- pre-sample tools
+def _simulation_sets(model, n_sim, feature_names, params, seed, M):
+    """(M, n_sim, d) device features of M simulation sets, set i from the i-th child seed of
+    SeedSequence(seed)."""
+    child_seeds = np.random.SeedSequence(seed).generate_state(M)
+    return torch.stack([_simulate_features(model, n_sim, feature_names, params, s)
+                        for s in child_seeds])
+
+
+def log_SL_stdev(model, theta, n_sim, feature_names, likelihood=None, M=20, seed=None):
+    """Standard deviation of the log synthetic likelihood at theta over M simulation sets, for
+    each simulation count in n_sim.  A device likelihood evaluates the M sets in one call per
+    count."""
+    params = _param_values(model, theta)
+    feature_names = _names(feature_names)
+    observed = _observed_row(model, feature_names)
+    n_sim = np.atleast_1d(n_sim)
+    sets = _simulation_sets(model, int(max(n_sim)), feature_names, params, seed, M)
+    lik = _device_likelihood(likelihood)
+    ll = np.zeros((len(n_sim), M))
+    for n_i, n in enumerate(n_sim):
+        if lik is not None:
+            ll[n_i] = dev.to_host(lik.device(sets[:, :int(n)], observed.reshape(-1)))
+        else:
+            host = dev.to_host(sets)
+            for i in range(M):
+                ll[n_i, i] = np.reshape(likelihood(host[i, :int(n)], observed), -1)[0]
+    return np.std(ll, axis=1)
+
+
+def select_penalty(model, n_sim, theta, feature_names, likelihood=None, lmdas=None, M=20,
+                   sigma=1.5, shrinkage='glasso', whitening=None, seed=None, verbose=False):
+    """The Warton penalty, per simulation count in n_sim, whose log synthetic likelihood standard
+    deviation over M simulation sets is closest to sigma.  Returns (penalties, standard
+    deviations).  With the default likelihood all M sets and all penalties of one simulation
+    count are one device call.  shrinkage='glasso' (the reference's default) is not provided."""
+    if shrinkage == 'glasso':
+        raise NotImplementedError("select_penalty: shrinkage='glasso' (graphical lasso) is not "
+                                  "provided; pass shrinkage='warton'")
+    if shrinkage != 'warton':
+        raise ValueError("shrinkage must be 'warton', got {!r}".format(shrinkage))
+    params = _param_values(model, theta)
+    feature_names = _names(feature_names)
+    ssy = _observed_row(model, feature_names)
+    if lmdas is None:
+        lmdas = list(np.arange(0.2, 0.8, 0.02))
+    lmdas = list(lmdas)
+    batch_size = np.array([n_sim]).flatten()
+    ns, n_lambda = len(batch_size), len(lmdas)
+    sets = _simulation_sets(model, int(max(batch_size)), feature_names, params, seed, M)
+    logliks = np.zeros((M, ns, n_lambda))
+    on_device = likelihood is None or likelihood is gaussian_syn_likelihood
+    if on_device:
+        lik = SyntheticLikelihood('standard', None, whitening)
+    for n_i, n in enumerate(batch_size):
+        if on_device:
+            logliks[:, n_i, :] = dev.to_host(lik.device(sets[:, :int(n)], ssy.reshape(-1),
+                                                        penalties=lmdas))
+        else:
+            host = dev.to_host(sets)
+            for m in range(M):
+                for k, lmda in enumerate(lmdas):
+                    logliks[m, n_i, k] = np.reshape(likelihood(
+                        host[m, :int(n)], ssy, shrinkage=shrinkage, penalty=lmda,
+                        whitening=whitening), -1)[0]
+    closest_lmdas = np.zeros(ns)
+    closest_std_devs = np.zeros(ns)
+    for i in range(ns):
+        std_devs = np.array([np.std(logliks[:, i, j]) for j in range(n_lambda)])
+        best = np.argmin(np.abs(std_devs - sigma))
+        closest_lmdas[i] = lmdas[best]
+        closest_std_devs[i] = std_devs[best]
+        if verbose:
+            print('n_sim {}: logliks {}, std_devs {}'.format(batch_size[i], logliks[:, i],
+                                                            std_devs))
+    return closest_lmdas, closest_std_devs
+
+
+def estimate_whitening_matrix(model, n_sim, theta, feature_names, likelihood_type='standard',
+                              seed=None):
+    """Whitening matrix W (d, d) of Priddle et al. (2021) from n_sim simulations at theta: the
+    eigen-decomposition of the correlation of the standardised features, W = diag(w^-1/2) V^T,
+    both factors rounded to 8 decimals.  Host arithmetic (one d x d set-up), so W is the same
+    bits for the same simulations."""
+    if likelihood_type not in ('standard', 'semiparametric'):
+        raise ValueError("Unsupported likelihood type '{}'.".format(likelihood_type))
+    if likelihood_type == 'semiparametric':
+        raise NotImplementedError("estimate_whitening_matrix: likelihood_type='semiparametric' "
+                                  "(semiBSL) is not provided")
+    params = _param_values(model, theta)
+    feature_names = _names(feature_names)
+    ssx = dev.to_host(_simulate_features(model, n_sim, feature_names, params, seed))
+    centred = ssx - np.mean(ssx, axis=0)
+    standardised = centred / np.std(ssx, axis=0)
+    eigval, eigvec = scipy.linalg.eig(np.cov(np.transpose(standardised)))
+    scale = np.diag(np.power(eigval, -0.5)).real.round(8)
+    return np.dot(scale, eigvec.T).real.round(8)

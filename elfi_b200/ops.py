@@ -1635,3 +1635,59 @@ def scratch_assay_summaries(x):
               x.stride(1), x.stride(2), x.stride(3), B, nrows, ncols, frames, dev.ptr(S), frames,
               dev.stream_ptr())
     return S
+
+
+# ---- Bayesian synthetic likelihood (elfi/methods/bsl/pdf_methods.py) ------------------------------
+SYNLIK_D_MAX = 160             # Sigma, its factor and the right-hand side in one CTA's shared memory
+SYNLIK_ESTIMATORS = {'standard': 0, 'unbiased': 1}
+
+
+def synlik(S, y, estimator='standard', penalties=None, whitening=None):
+    """Gaussian synthetic log-likelihood of the observed summaries y (d,) under each group of
+    simulated summaries S, (n, d) or (G, n, d), host or device, any row and group strides.
+
+    estimator 'standard' is gaussian_syn_likelihood (Warton shrinkage at each of the penalties, and
+    whitening by the (d, d) matrix W, both optional); 'unbiased' is
+    gaussian_syn_likelihood_ghurye_olkin.  Returns a device tensor (G,), or (G, K) for K penalties.
+    A group whose inputs are not all finite, or whose covariance fails its Cholesky test, gives
+    -inf (include/elfi_b200.h states the test).  Limits: 1 <= d <= SYNLIK_D_MAX, n >= 2."""
+    if estimator not in SYNLIK_ESTIMATORS:
+        raise ValueError("estimator must be 'standard' or 'unbiased', got {!r}".format(estimator))
+    if estimator == 'unbiased' and (penalties is not None or whitening is not None):
+        raise ValueError('the unbiased estimator takes no penalties and no whitening')
+    X = S if dev.is_device_array(S) and S.dtype == torch.float64 else dev.to_device(S)
+    if X.dim() == 2:
+        X = X[None]
+    if X.dim() != 3:
+        raise ValueError('synlik takes S of shape (n, d) or (G, n, d), got {}'.format(
+            tuple(X.shape)))
+    G, n, d = (int(v) for v in X.shape)
+    if not 1 <= d <= SYNLIK_D_MAX:
+        raise ValueError('synlik takes 1 <= d <= {} summaries, got d = {}'.format(SYNLIK_D_MAX, d))
+    if n < 2:
+        raise ValueError('synlik takes n >= 2 simulations per group, got n = {}'.format(n))
+    if X.stride(2) != 1 or X.stride(1) < d or X.stride(0) < 0:
+        X = X.contiguous()
+    yv = dev.to_device(y).reshape(-1).contiguous()
+    if yv.numel() != d:
+        raise ValueError('y has {} values, S has d = {} summaries'.format(yv.numel(), d))
+    W = None
+    if whitening is not None:
+        W = dev.to_device(whitening).contiguous()
+        if tuple(W.shape) != (d, d):
+            raise ValueError('whitening must be a ({0}, {0}) matrix, got shape {1}'.format(
+                d, tuple(W.shape)))
+    pen, K = None, 0
+    if penalties is not None:
+        pen = np.ascontiguousarray(np.asarray(penalties, dtype=np.float64).reshape(-1))
+        K = pen.size
+        if K == 0:
+            raise ValueError('penalties is empty')
+        if not np.all((pen >= 0) & (pen <= 1)):
+            raise ValueError('Warton penalties must lie in [0, 1], got {}'.format(pen))
+    out = dev.empty((G, K) if K else (G,))
+    _lib.call('elfi_b200_synlik_f64', dev.context(), dev.ptr(X), X.stride(1), X.stride(0), G, n,
+              d, dev.ptr(yv), dev.ptr(W), SYNLIK_ESTIMATORS[estimator],
+              None if pen is None else ctypes.c_void_p(pen.ctypes.data), K, dev.ptr(out),
+              dev.stream_ptr())
+    return out

@@ -741,6 +741,35 @@ int elfi_b200_scratch_assay_summaries_f64(elfi_b200_ctx* ctx, const uint8_t* X, 
                                           int64_t nrows, int64_t ncols, int64_t n_frames,
                                           double* S, int64_t ldS, void* stream);
 
+/* ---- Bayesian synthetic likelihood (elfi/methods/bsl/pdf_methods.py) ---------------------------
+ * elfi_b200_synlik_f64: the Gaussian synthetic log-likelihood of the observed summaries y (d) under
+ * each of G groups of n simulated summary rows, S[g * ld_group + i * ld_row + j], i < n, j < d
+ * (ld_row >= d; groups may be gapped or interleaved).  Per group: mu the column means, Sigma the
+ * covariance with divisor n - 1.
+ *   W (d x d row-major, device) or NULL: whitening; W mu, W Sigma W^T and W y replace mu, Sigma, y.
+ *   estimator 0, standard: ll = -(d log 2 pi + log det Sigma_l + m) / 2, m = (y - mu)^T Sigma_l^-1
+ *     (y - mu), with Warton shrinkage Sigma_l = (1 - l) Sigma + l diag(Sigma_jj + 1e-5) for each
+ *     of the K penalties l in [0, 1] (penalties_host, HOST), or Sigma itself when K = 0.
+ *   estimator 1, unbiased (Ghurye and Olkin 1969): ll = -d log(2 pi) / 2 + A + B + C with
+ *     A = log c(d, n - 2) - log c(d, n - 1) - d log(1 - 1/n) / 2,
+ *     B = -(n - d - 2)(log(n - 1) + log det Sigma) / 2,
+ *     C = (n - d - 3) log|det Psi| / 2, Psi = (n - 1) Sigma - (y - mu)(y - mu)^T / (1 - 1/n),
+ *     log|det Psi| = d log(n - 1) + log det Sigma + log|1 - n m / (n - 1)^2| (determinant lemma).
+ *     W must be NULL and K = 0.
+ * loglik[g * max(K, 1) + k] (device) gets group g's value at penalty k.  A group gives -inf when
+ * any of its n x d values is not finite (or its column sum overflows), or when a Cholesky pivot of
+ * Sigma_l is not finite or L_jj^2 <= 1e6 * DBL_EPSILON * max_i Sigma_l,ii.  SciPy instead tests the
+ * eigenvalues against 1e6 eps lambda_max and gives up near cond(Sigma) ~ 4.5e9; near that boundary
+ * the two tests can disagree (by a factor that depends on d), and one may return a finite value
+ * where the other returns -inf.  Limits: 1 <= d <= 160, n >= 2, G <= 2^22, K <= 65535.  Results
+ * are bit-identical across calls, and a group's value does not depend on G, K or the other
+ * groups.  Asynchronous on `stream`; uses the context's scratch (about G d^2 doubles, more with
+ * whitening or when few groups split their rows over several CTAs). */
+int elfi_b200_synlik_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_row, int64_t ld_group,
+                         int64_t G, int64_t n, int64_t d, const double* y, const double* W,
+                         int32_t estimator, const double* penalties_host, int64_t K,
+                         double* loglik, void* stream);
+
 /* ---- KLIEP density-ratio estimation (AdaptiveThresholdSMC) -------------------------------------
  * DensityRatioEstimation.fit + max_ratio (elfi/methods/density_ratio_estimation.py:71-207):
  * basis centres = first n_basis rows of x, A = RBF(x, centres), b = weighted RBF mean over y,
