@@ -1,8 +1,8 @@
 """elfi_b200 -- H100-native (sm_90a) implementation of ELFI's data-parallel hot path.
 
 The package mirrors the operator / sampler API of elfi-dev/elfi for the batched
-summary -> distance -> threshold/top-n selection -> SMC weight path and the BOLFI GP
-surrogate, with the arithmetic in hand-written CUDA reached through a C ABI
+summary -> distance -> threshold/top-n selection -> SMC weight path, the BOLFI GP
+surrogate, BSL's synthetic likelihood and BOLFIRE's ratio-estimation classifier, with the arithmetic in hand-written CUDA reached through a C ABI
 (include/elfi_b200.h).  See DESIGN.md and INTEGRATION.md.
 """
 __version__ = '0.1.0'
@@ -17,5 +17,6 @@ from .samplers import (SMC, AdaptiveDistanceSMC, AdaptiveThresholdSMC,  # noqa: 
 from .store import OutputPool  # noqa: F401
 from .priors import DeviceModelPrior  # noqa: F401
 from .bsl import BSL  # noqa: F401
+from .bolfire import BOLFIRE, BOLFIREPosterior  # noqa: F401
 from .bo import (BOLFI, LCBSC, BayesianOptimization, BolfiPosterior, GPyRegression,  # noqa: F401
                  ExpIntVar, MaxVar, RandMaxVar, UniformAcquisition)

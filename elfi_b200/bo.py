@@ -6,7 +6,7 @@ Mirrors (file:line in elfi-dev/elfi):
                          n_evidence, is_sampling, predict, predict_mean, predictive_gradients,
                          predictive_gradient_mean, update, optimize, copy)
   AcquisitionBase, LCBSC elfi/methods/bo/acquisition.py:16-301
-  minimize               elfi/methods/bo/utils.py:40-111
+  minimize, CostFunction elfi/methods/bo/utils.py:40-164
   BayesianOptimization, BOLFI.fit/extract_posterior   elfi/methods/inference/bolfi.py:26-462
   BolfiPosterior (logpdf / pdf core)                  elfi/methods/posteriors.py:21-189
 
@@ -381,6 +381,28 @@ def minimize(fun, bounds, method='L-BFGS-B', constraints=None, grad=None, prior=
                                     constraints=constraints, options=dict(maxiter=maxiter))
             for x0 in starts]
     return _best_of(runs, bounds)
+
+
+class CostFunction:
+    """An acquisition cost: scale * function(x) with its gradient (elfi/methods/bo/utils.py:
+    CostFunction).  BOLFIRE adds minus the log prior to LCBSC with it."""
+
+    def __init__(self, function, gradient, scale=1):
+        self.function = function
+        self.gradient = gradient
+        self.scale = scale
+
+    def evaluate(self, x):
+        """(n, 1) values at x, (input_dim,) or (n, input_dim)."""
+        x = np.atleast_2d(x)
+        n, input_dim = x.shape
+        return self.scale * np.asarray(self.function(x)).reshape(n, 1)
+
+    def evaluate_gradient(self, x):
+        """(n, input_dim) gradients at x."""
+        x = np.atleast_2d(x)
+        n, input_dim = x.shape
+        return self.scale * np.asarray(self.gradient(x)).reshape(n, input_dim)
 
 
 class _Rendezvous:

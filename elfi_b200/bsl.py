@@ -3,6 +3,7 @@
 Host control flow follows the reference (paths relative to elfi-dev/elfi):
   BSL, its Metropolis-Hastings step and logit transform   elfi/methods/inference/bsl.py
   ModelBased (rounds of n_sim_round simulations)          elfi/methods/inference/parameter_inference.py
+                                                          (model_based.py, shared with BOLFIRE)
   likelihoods                                             elfi/methods/bsl/pdf_methods.py
   log_SL_stdev, select_penalty, estimate_whitening_matrix elfi/methods/bsl/pre_sample_methods.py
 What runs on the device: the simulations of a device model, the (n_sim_round, d) feature matrix
@@ -21,10 +22,10 @@ import scipy.linalg
 import torch
 
 from . import device as dev
-from . import model as em
 from . import ops
 from .results import BslSample
-from .samplers import ModelPrior, ParameterInference
+from .model_based import ModelBased, feature_columns, feature_list, observed_row
+from .samplers import ModelPrior
 
 logger = logging.getLogger(__name__)
 
@@ -128,80 +129,33 @@ def _device_likelihood(likelihood):
 
 
 # ------------------------------------------------------------------------------- features
-def _feature_columns(batch, names, rows):
-    """The outputs `names` of a batch as 2-d float64 device blocks of `rows` rows, in order (the
-    columns of batch_to_arr2d): lazy simulations are materialised, host arrays uploaded."""
-    blocks = []
-    for name in names:
-        v = batch[name]
-        if hasattr(v, 'materialize'):
-            v = v.materialize()
-        t = v if dev.is_device_array(v) else dev.to_device(np.asarray(v, dtype=np.float64))
-        if t.dtype != torch.float64:
-            t = t.to(torch.float64)
-        if t.dim() == 1:
-            t = t[:, None]
-        if t.dim() != 2 or t.shape[0] != rows:
-            raise ValueError('Feature {} must be a ({}, k) array per batch, got shape {}'.format(
-                name, rows, tuple(t.shape)))
-        blocks.append(t)
-    return blocks
-
-
 def _simulate_features(model, n_sim, feature_names, params, seed):
     """(n_sim, d) device matrix of the features simulated at params (model.generate)."""
     out = model.generate(n_sim, outputs=list(feature_names), with_values=params, seed=seed)
-    blocks = _feature_columns(out, feature_names, n_sim)
+    blocks = feature_columns(out, feature_names, n_sim)
     return blocks[0] if len(blocks) == 1 else torch.cat(blocks, dim=1)
-
-
-def _observed_row(model, feature_names):
-    return np.column_stack([dev.to_host(model[node].observed) for node in feature_names])
 
 
 def _param_values(model, theta):
     return theta if isinstance(theta, dict) else dict(zip(model.parameter_names, theta))
 
 
-def _names(feature_names):
-    return [feature_names] if isinstance(feature_names, str) else list(feature_names)
-
-
 # ------------------------------------------------------------------------------- sampler
-class BSL(ParameterInference):
+class BSL(ModelBased):
     """Bayesian synthetic likelihood with a random-walk Metropolis-Hastings sampler (Price et al.
     2018).  Each round simulates n_sim_round times at one parameter; the round's features stay on
     the device and go to one likelihood call.  Runs on this rank only."""
 
+    D_MAX = ops.SYNLIK_D_MAX
+
     def __init__(self, model, n_sim_round, feature_names=None, likelihood=None, batch_size=None,
                  seed=None, pool=None):
-        model = model.model if isinstance(model, em.NodeReference) else model
-        self.n_sim_round = int(n_sim_round)
-        batch_size = batch_size or self.n_sim_round
-        if self.n_sim_round % batch_size != 0:
-            raise ValueError('n_sim_round must be a multiple of batch_size.')
-        feature_names = _names(feature_names) if feature_names else [
-            node for node in model.nodes
-            if isinstance(model[node], em.Summary) and not node.startswith('_')]
-        if not feature_names:
-            raise ValueError('feature_names must include at least one item.')
-        for node in feature_names:
-            if node not in model.nodes:
-                raise ValueError('Node {} not found in the model'.format(node))
-        self.feature_names = feature_names
-        super().__init__(model, model.parameter_names + feature_names, batch_size=batch_size,
-                         seed=seed, pool=pool, distributed=False)
-        self.observed = _observed_row(self.model, feature_names)
-        d = self.observed.size
-        if not 1 <= d <= ops.SYNLIK_D_MAX:
-            raise ValueError('BSL takes 1 to {} features, got {}'.format(ops.SYNLIK_D_MAX, d))
+        super().__init__(model, n_sim_round, feature_names=feature_names, batch_size=batch_size,
+                         seed=seed, pool=pool)
         self.random_state = np.random.RandomState(self.seed)
         self.likelihood = likelihood
         self._device_lik = _device_likelihood(likelihood)
         self._obs_dev = None
-        self._sim = None                  # (n_sim_round, d) device features of the round
-        self.state['round'] = 0
-        self.state['n_sim_round'] = 0
         self.param_names = None
         self.prior = None
         self.sigma_proposals = None
@@ -246,48 +200,9 @@ class BSL(ParameterInference):
         self.state['logprior'][0] = np.reshape(self.prior.logpdf(params0), -1)[0]
         self.state['logposterior'] = np.zeros(n_samples)
 
-    def set_objective(self, rounds):
-        self.objective['round'] = rounds
-        self.objective['n_batches'] = rounds * (self.n_sim_round // self.batch_size)
-
-    def infer(self, *args, **kwargs):
-        if self.state['round'] > 0:
-            self._init_round()
-        return super().infer(*args, **kwargs)
-
     @property
     def current_params(self):
         return self.state['params'][self.state['n_samples']]
-
-    def prepare_new_batch(self, batch_index):
-        params = np.repeat(np.atleast_2d(self.current_params), self.batch_size, axis=0)
-        return {p: params[:, i] for i, p in enumerate(self.parameter_names)}
-
-    def update(self, batch, batch_index):
-        super().update(batch, batch_index)
-        self._merge_batch(batch)
-        if self.state['n_sim_round'] == self.n_sim_round:
-            self._process_simulated()
-            self.state['round'] += 1
-            if self.state['round'] < self.objective['round']:
-                self._init_round()
-
-    def _merge_batch(self, batch):
-        if self._sim is None:
-            self._sim = dev.empty((self.n_sim_round, self.observed.size))
-        row = self.state['n_sim_round']
-        col = 0
-        for block in _feature_columns(batch, self.feature_names, self.batch_size):
-            w = int(block.shape[1])
-            if col + w > self._sim.shape[1]:
-                raise ValueError('The features are wider than their observed values ({})'.format(
-                    self._sim.shape[1]))
-            self._sim[row:row + self.batch_size, col:col + w] = block
-            col += w
-        if col != self._sim.shape[1]:
-            raise ValueError('The features have {} columns, their observed values {}'.format(
-                col, self._sim.shape[1]))
-        self.state['n_sim_round'] += self.batch_size
 
     def _loglikelihood(self):
         if self._device_lik is not None:
@@ -445,8 +360,8 @@ def log_SL_stdev(model, theta, n_sim, feature_names, likelihood=None, M=20, seed
     each simulation count in n_sim.  A device likelihood evaluates the M sets in one call per
     count."""
     params = _param_values(model, theta)
-    feature_names = _names(feature_names)
-    observed = _observed_row(model, feature_names)
+    feature_names = feature_list(feature_names)
+    observed = observed_row(model, feature_names)
     n_sim = np.atleast_1d(n_sim)
     sets = _simulation_sets(model, int(max(n_sim)), feature_names, params, seed, M)
     lik = _device_likelihood(likelihood)
@@ -473,8 +388,8 @@ def select_penalty(model, n_sim, theta, feature_names, likelihood=None, lmdas=No
     if shrinkage != 'warton':
         raise ValueError("shrinkage must be 'warton', got {!r}".format(shrinkage))
     params = _param_values(model, theta)
-    feature_names = _names(feature_names)
-    ssy = _observed_row(model, feature_names)
+    feature_names = feature_list(feature_names)
+    ssy = observed_row(model, feature_names)
     if lmdas is None:
         lmdas = list(np.arange(0.2, 0.8, 0.02))
     lmdas = list(lmdas)
@@ -521,7 +436,7 @@ def estimate_whitening_matrix(model, n_sim, theta, feature_names, likelihood_typ
         raise NotImplementedError("estimate_whitening_matrix: likelihood_type='semiparametric' "
                                   "(semiBSL) is not provided")
     params = _param_values(model, theta)
-    feature_names = _names(feature_names)
+    feature_names = feature_list(feature_names)
     ssx = dev.to_host(_simulate_features(model, n_sim, feature_names, params, seed))
     centred = ssx - np.mean(ssx, axis=0)
     standardised = centred / np.std(ssx, axis=0)

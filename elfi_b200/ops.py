@@ -1691,3 +1691,152 @@ def synlik(S, y, estimator='standard', penalties=None, whitening=None):
               None if pen is None else ctypes.c_void_p(pen.ctypes.data), K, dev.ptr(out),
               dev.stream_ptr())
     return out
+
+
+# ---- BOLFIRE ratio-estimation classifier (elfi/methods/classifier.py) ------------------------------
+LOGREG_D_MAX = 160             # H = X~^T D X~ (packed) and the row tiles in one CTA's shared memory
+LOGREG_PENALTIES = {'l1': 0, 'l2': 1}
+LOGREG_HEAD = 8                # header doubles of a fit block (include/elfi_b200.h)
+LOGREG_STATUS = {1: 'converged', 0: 'not converged', -1: 'bad labels', -2: 'non-finite input'}
+
+
+def logreg_block_size(d):
+    """Doubles of the device fit block of a d-feature logistic regression."""
+    return LOGREG_HEAD + 3 * int(d)
+
+
+class LogRegFit:
+    """A logistic-regression fit on the device: `block` is the (LOGREG_HEAD + 3 d,) result block of
+    elfi_b200_logreg_fit_f64 (intercept, n_iter, status, objective, subgradient norm, then mean_,
+    scale_ and coef_).  `host()` reads it once and keeps the host copy."""
+
+    def __init__(self, block, d, penalty, C):
+        self.block, self.d, self.penalty, self.C = block, int(d), penalty, float(C)
+        self._host = None
+
+    def set_host(self, values):
+        """Record the block's host values, read together with something else."""
+        self._host = np.asarray(values, dtype=np.float64)[:logreg_block_size(self.d)]
+
+    def host(self):
+        if self._host is None:
+            self._host = dev.to_host(self.block).astype(np.float64)
+        return self._host
+
+    def _part(self, k):
+        h = self.host()
+        return h[LOGREG_HEAD + k * self.d:LOGREG_HEAD + (k + 1) * self.d]
+
+    @property
+    def intercept_(self):
+        return float(self.host()[0])
+
+    @property
+    def n_iter(self):
+        return int(self.host()[1])
+
+    @property
+    def status(self):
+        return int(self.host()[2])
+
+    @property
+    def converged(self):
+        return self.status == 1
+
+    @property
+    def objective(self):
+        return float(self.host()[3])
+
+    @property
+    def subgradient_norm(self):
+        return float(self.host()[4])
+
+    @property
+    def mean_(self):
+        return self._part(0)
+
+    @property
+    def scale_(self):
+        return self._part(1)
+
+    @property
+    def coef_(self):
+        return self._part(2)
+
+    def check(self):
+        """ValueError for a fit the device rejected (labels, or non-finite values in X)."""
+        s = self.status
+        if s == -1:
+            raise ValueError('logreg_fit: the labels must be +1 or -1 with both classes present')
+        if s == -2:
+            raise ValueError('logreg_fit: X contains NaN or infinity, or a value too large for '
+                             'float64')
+        return self
+
+
+def _logreg_rows(X, name):
+    X = _matrix(X)
+    if X.shape[0] > 1 and X.stride(0) < X.shape[1]:
+        X = X.contiguous()
+    return X
+
+
+def logreg_fit(X, y, penalty='l1', C=1.0, max_iter=100, out=None):
+    """Fit the reference's ratio-estimation classifier (StandardScaler, then liblinear's L1- or
+    L2-penalised logistic regression with a penalised intercept) to the optimum on the device.
+    X is (n, d) with any row stride, y holds n labels +1 / -1; host or device.  Returns a LogRegFit
+    whose block stays on the device (`out`, of logreg_block_size(d) doubles, if given).  Host
+    labels are checked here; device labels are checked by the kernel and reported when the block
+    is read (LogRegFit.check)."""
+    if penalty not in LOGREG_PENALTIES:
+        raise ValueError("penalty must be 'l1' or 'l2', got {!r}".format(penalty))
+    C = float(C)
+    if not (C > 0 and np.isfinite(C)):
+        raise ValueError('C must be positive and finite, got {}'.format(C))
+    if int(max_iter) != max_iter or max_iter < 0:
+        raise ValueError('max_iter must be a non-negative integer, got {}'.format(max_iter))
+    if not dev.is_device_array(y):
+        yh = np.asarray(y, dtype=np.float64).reshape(-1)
+        if not np.all((yh == 1) | (yh == -1)):
+            raise ValueError('logreg_fit takes labels +1 and -1')
+        if np.all(yh == 1) or np.all(yh == -1):
+            raise ValueError('logreg_fit needs samples of both classes, got only {}'.format(
+                yh[0] if yh.size else 'none'))
+    Xd = _logreg_rows(X, 'X')
+    n, d = int(Xd.shape[0]), int(Xd.shape[1])
+    if not 1 <= d <= LOGREG_D_MAX:
+        raise ValueError('logreg_fit takes 1 <= d <= {} features, got d = {}'.format(
+            LOGREG_D_MAX, d))
+    if n < 2:
+        raise ValueError('logreg_fit takes n >= 2 rows, got n = {}'.format(n))
+    yd = y if dev.is_device_array(y) else dev.to_device(yh)
+    yd = yd.reshape(-1)
+    if yd.dtype != torch.float64 or not yd.is_contiguous():
+        yd = yd.to(torch.float64).contiguous()
+    if yd.numel() != n:
+        raise ValueError('y has {} labels, X has {} rows'.format(yd.numel(), n))
+    block = dev.empty((logreg_block_size(d),)) if out is None else out
+    if block.numel() != logreg_block_size(d) or not block.is_contiguous():
+        raise ValueError('out must be a contiguous device buffer of {} doubles'.format(
+            logreg_block_size(d)))
+    _lib.call('elfi_b200_logreg_fit_f64', dev.context(), dev.ptr(Xd), _ld(Xd), n, d, dev.ptr(yd),
+              LOGREG_PENALTIES[penalty], C, int(max_iter), dev.ptr(block), dev.stream_ptr())
+    return LogRegFit(block, d, penalty, C)
+
+
+def logreg_predict(fit, X, class_min=0.0, out=None):
+    """log(p / (1 - p)) per row of X (m, d), p = max(expit(decision value), class_min): the
+    reference's predict_log_likelihood_ratio, as a device tensor (m,) (`out` if given).  A row
+    with a non-finite value, or a fit the device rejected, gives NaN."""
+    if not isinstance(fit, LogRegFit):
+        raise ValueError('logreg_predict takes the LogRegFit of logreg_fit')
+    Xd = _logreg_rows(X, 'X')
+    m, d = int(Xd.shape[0]), int(Xd.shape[1])
+    if d != fit.d:
+        raise ValueError('X has {} features per row, the fit {}'.format(d, fit.d))
+    res = dev.empty((m,)) if out is None else out
+    if res.numel() != m or not res.is_contiguous():
+        raise ValueError('out must be a contiguous device buffer of {} doubles'.format(m))
+    _lib.call('elfi_b200_logreg_predict_f64', dev.context(), dev.ptr(fit.block), d, dev.ptr(Xd),
+              _ld(Xd), m, float(class_min), dev.ptr(res), dev.stream_ptr())
+    return res

@@ -178,6 +178,12 @@ class BolfiSample(Sample):
                          chains=chains, n_chains=chains.shape[0], warmup=warmup, **meta)
 
 
+class BOLFIRESample(BolfiSample):
+    """Posterior draws of BOLFIRE.sample (elfi/methods/results.py BOLFIRESample): `chains` is
+    (n_chains, n_samples, n_parameters) with the warm-up included, `samples` the post-warm-up draws
+    of all chains.  Like BolfiSample without a threshold."""
+
+
 class BslSample(Sample):
     """Metropolis-Hastings chain of BSL.sample (elfi/methods/results.py BslSample): `samples_all`
     holds every iteration per parameter, burn-in included; `samples` those after `burn_in`."""

@@ -770,6 +770,40 @@ int elfi_b200_synlik_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_row, in
                          int32_t estimator, const double* penalties_host, int64_t K,
                          double* loglik, void* stream);
 
+/* ---- BOLFIRE ratio-estimation classifier (elfi/methods/classifier.py: LogisticRegression) ------
+ * elfi_b200_logreg_fit_f64: sklearn's StandardScaler then penalised logistic regression with
+ * liblinear's primal and intercept_scaling = 1, on the n rows X[i * ld_row + j], j < d (device,
+ * ld_row >= d) with labels y[i] (device, each +1 or -1).
+ *   Standardisation: mean_j and var_j over all n rows (ddof 0; var_j = (S2 - S1^2 / n) / n with
+ *     S1, S2 the sums of x - mean_j and (x - mean_j)^2), scale_j = sqrt(var_j), or 1 when the column
+ *     is constant by sklearn's rule var_j <= n eps var_j + (n mean_j eps)^2.  x~_ij =
+ *     (x_ij - mean_j) / scale_j, and every row gets a trailing 1 (the intercept, penalised too).
+ *   Objective, penalty 0 (L1): F(w) = sum_j |w_j| + C sum_i log(1 + exp(-y_i w . x~_i));
+ *              penalty 1 (L2): F(w) = |w|^2 / 2 + C sum_i log(1 + exp(-y_i w . x~_i)).
+ *   Solved to convergence (proximal Newton, liblinear's newGLMNET without its tolerance): stops
+ *     when the infinity norm of the minimum-norm subgradient is <= 1e-10 C n (for L1, g_j +
+ *     sign(w_j) where w_j != 0 and max(|g_j| - 1, 0) where w_j = 0), or after max_iter Newton steps,
+ *     or when a step gives no decrease; the last two return the last iterate with status 0.
+ *   fit (device, ELFI_B200_LOGREG_BLOCK(d) doubles): [0] intercept_, [1] Newton steps taken
+ *     (n_iter_), [2] status (1 converged, 0 not converged, -1 labels not all +-1 or one class only,
+ *     -2 a non-finite value in X or a variance that overflows), [3] F at the returned weights,
+ *     [4] the subgradient norm there, [5..7] 0, then mean_ (d), scale_ (d), coef_ (d).  A negative
+ *     status leaves NaN in every other value.
+ * elfi_b200_logreg_predict_f64: out[i] (device, i < m) = log(p / (1 - p)) of row Xq[i * ld_row + j]
+ *   with v = sum_j coef_j (x_j - mean_j) / scale_j + intercept_, p = 1 / (1 + exp(-v)), then
+ *   p = max(p, class_min): the reference's log-likelihood ratio (p = 1 gives +inf).  A row with a
+ *   non-finite value, or a fit with a negative status, gives NaN.
+ * Limits: 1 <= d <= 160, 2 <= n < 2^31, C > 0.  One CTA per fit; reductions in a fixed order, no
+ * atomics: repeated calls are bit-identical.  Asynchronous on `stream`; the fit uses 4 n doubles of
+ * the context's scratch. */
+#define ELFI_B200_LOGREG_BLOCK(d) (8 + 3 * (d))
+int elfi_b200_logreg_fit_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_row, int64_t n,
+                             int64_t d, const double* y, int32_t penalty, double C,
+                             int64_t max_iter, double* fit, void* stream);
+int elfi_b200_logreg_predict_f64(elfi_b200_ctx* ctx, const double* fit, int64_t d,
+                                 const double* Xq, int64_t ld_row, int64_t m, double class_min,
+                                 double* out, void* stream);
+
 /* ---- KLIEP density-ratio estimation (AdaptiveThresholdSMC) -------------------------------------
  * DensityRatioEstimation.fit + max_ratio (elfi/methods/density_ratio_estimation.py:71-207):
  * basis centres = first n_basis rows of x, A = RBF(x, centres), b = weighted RBF mean over y,
