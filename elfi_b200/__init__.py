@@ -2,7 +2,9 @@
 
 The package mirrors the operator / sampler API of elfi-dev/elfi for the batched
 summary -> distance -> threshold/top-n selection -> SMC weight path, the BOLFI GP
-surrogate, BSL's synthetic likelihood and BOLFIRE's ratio-estimation classifier, with the arithmetic in hand-written CUDA reached through a C ABI
+surrogate, BSL's synthetic likelihood, BOLFIRE's ratio-estimation classifier and the two-stage
+summary-statistic selection of Nunes and Balding (TwoStageSelection), with the arithmetic in
+hand-written CUDA reached through a C ABI
 (include/elfi_b200.h).  See DESIGN.md and INTEGRATION.md.
 """
 __version__ = '0.1.0'
@@ -18,5 +20,6 @@ from .store import OutputPool  # noqa: F401
 from .priors import DeviceModelPrior  # noqa: F401
 from .bsl import BSL  # noqa: F401
 from .bolfire import BOLFIRE, BOLFIREPosterior  # noqa: F401
+from .diagnostics import TwoStageSelection  # noqa: F401
 from .bo import (BOLFI, LCBSC, BayesianOptimization, BolfiPosterior, GPyRegression,  # noqa: F401
                  ExpIntVar, MaxVar, RandMaxVar, UniformAcquisition)

@@ -133,6 +133,12 @@ SIGNATURES = {
                                  c_i64, c_ptr, c_ptr],
     'elfi_b200_logreg_predict_f64': [c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_i64, c_dbl, c_ptr,
                                      c_ptr],
+    'elfi_b200_subset_distance_f64': [c_ptr, ctypes.c_int32, c_ptr, c_i64, c_i64, c_i64, c_ptr,
+                                      c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_ptr],
+    'elfi_b200_knn_entropy_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr, c_ptr,
+                                  c_ptr],
+    'elfi_b200_mrsse_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_i64, c_i64, c_ptr,
+                            c_ptr],
     'elfi_b200_gp_padded_size': [c_i64],
     'elfi_b200_gp_fit_f64': [c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_i64, c_dbl, c_dbl, c_dbl, c_dbl,
                              c_ptr, c_ptr, c_ptr, c_i64, c_ptr, c_ptr, c_ptr],

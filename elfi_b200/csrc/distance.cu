@@ -19,6 +19,7 @@
 // a consumer, a thread-per-row kernel and a case in launch_dist() or launch_metric().
 #include <cstdlib>
 
+#include "metric.cuh"
 #include "rowstream.cuh"
 
 namespace elfi {
@@ -505,10 +506,9 @@ int launch_dist(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B, int
 
 // ---- other cdist metrics (elfi/model/elfi_model.py:1037: Distance passes any metric string to
 // scipy.spatial.distance.cdist) ------------------------------------------------------------------
-// SciPy 1.18 accumulates 'sqeuclidean', 'cityblock', 'chebyshev' and 'minkowski' left to right in
-// fp64 like 'euclidean' (probed: bit-identical to a sequential loop at 2000 x 128), so they are
-// variants of EuclidConsumer with another per-term operation and another finish.  Unweighted,
-// one column (K = 1).  Zero padding (TMA fill, obs pad) adds |0|, 0^2, 0^p or max(acc, 0): no-ops.
+// 'sqeuclidean', 'cityblock', 'chebyshev' and 'minkowski' are variants of EuclidConsumer with
+// another per-term operation and another finish (metric.cuh).  Unweighted, one column (K = 1).
+// Zero padding (TMA fill, obs pad) adds |0|, 0^2, 0^p or max(acc, 0): no-ops.
 struct MetricParams : DistParams {
     double pexp;       // Minkowski exponent
     const double* V;   // (D) component variances of 'seuclidean', else nullptr
@@ -518,19 +518,6 @@ struct MetricParams : DistParams {
 // (elfi_b200_dist_seuclidean_thr_f64, because of V), and elfi_b200_dist_metric_thr_f64 keeps
 // rejecting every code beyond ELFI_B200_METRIC_MINKOWSKI.
 constexpr int METRIC_SEUCLIDEAN = ELFI_B200_METRIC_MINKOWSKI + 1;
-
-template <int METRIC>
-__device__ __forceinline__ double metric_term(double acc, double d, double pexp) {
-    if (METRIC == ELFI_B200_METRIC_SQEUCLIDEAN) return __dadd_rn(acc, __dmul_rn(d, d));
-    if (METRIC == ELFI_B200_METRIC_CITYBLOCK) return __dadd_rn(acc, fabs(d));
-    if (METRIC == ELFI_B200_METRIC_CHEBYSHEV) return fabs(d) > acc ? fabs(d) : acc;
-    return __dadd_rn(acc, pow(fabs(d), pexp));                       // Minkowski
-}
-
-template <int METRIC>
-__device__ __forceinline__ double metric_value(double acc, double pexp) {
-    return METRIC == ELFI_B200_METRIC_MINKOWSKI ? pow(acc, 1.0 / pexp) : acc;
-}
 
 template <int METRIC>
 struct MetricConsumer {

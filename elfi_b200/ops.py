@@ -1840,3 +1840,127 @@ def logreg_predict(fit, X, class_min=0.0, out=None):
     _lib.call('elfi_b200_logreg_predict_f64', dev.context(), dev.ptr(fit.block), d, dev.ptr(Xd),
               _ld(Xd), m, float(class_min), dev.ptr(res), dev.stream_ptr())
     return res
+
+
+# ---- summary-statistic selection (TwoStageSelection, elfi/methods/diagnostics.py) ---------------
+SUBSET_METRIC_CODES = {'euclidean': 0, 'sqeuclidean': 1, 'cityblock': 2, 'chebyshev': 3}
+SUBSET_MAX_WIDTH = 512
+SUBSET_MAX_COMBINATIONS = 2 ** 24 - 1
+KNN_MAX_Q = 16
+KNN_MAX_K = 32
+KNN_MAX_N = 2 ** 20
+KNN_MAX_SETS = 2 ** 16 - 1
+
+
+class SubsetLayout:
+    """The candidate combinations of :func:`subset_distance`, checked and uploaded once: each
+    combination is an ordered list of column ranges (col, width) of a (B, width) summary matrix."""
+
+    def __init__(self, combinations, width):
+        width = int(width)
+        if not 1 <= width <= SUBSET_MAX_WIDTH:
+            raise ValueError('subset_distance takes 1 <= {} summary columns, got {}'.format(
+                SUBSET_MAX_WIDTH, width))
+        combinations = [list(c) for c in combinations]
+        if not 1 <= len(combinations) <= SUBSET_MAX_COMBINATIONS:
+            raise ValueError('subset_distance takes 1 to {} combinations, got {}'.format(
+                SUBSET_MAX_COMBINATIONS, len(combinations)))
+        ranges, offsets = [], [0]
+        for comb in combinations:
+            if not comb:
+                raise ValueError('a combination needs at least one column range')
+            for col, w in comb:
+                if not (w >= 1 and col >= 0 and col + w <= width):
+                    raise ValueError('column range ({}, {}) outside the {} summary columns'.format(
+                        col, w, width))
+                ranges.append((int(col), int(w)))
+            offsets.append(len(ranges))
+        self.width = width
+        self.n_combinations = len(combinations)
+        self.ranges = dev.to_device(np.asarray(ranges, dtype=np.int32).reshape(-1, 2),
+                                    dtype=torch.int32)
+        self.offsets = dev.to_device(np.asarray(offsets, dtype=np.int32), dtype=torch.int32)
+
+
+def subset_distance(S, obs, layout, metric='euclidean', out=None):
+    """cdist of every combination of ``layout`` (a :class:`SubsetLayout`) at once: row c of the
+    (C, B) result is cdist(X_c, obs_c, metric), X_c and obs_c the concatenated column ranges of
+    combination c, bit for bit ('euclidean', 'sqeuclidean', 'cityblock' or 'chebyshev').  `out` may
+    be a (C, >= B) device matrix with unit column stride."""
+    if metric not in SUBSET_METRIC_CODES:
+        raise ValueError('subset_distance takes the metrics {}, got {!r}'.format(
+            ', '.join(SUBSET_METRIC_CODES), metric))
+    S = _matrix(S)
+    B, W = int(S.shape[0]), int(S.shape[1])
+    if W != layout.width:
+        raise ValueError('S has {} columns, the layout {}'.format(W, layout.width))
+    obs_t = dev.to_device(obs).reshape(-1)
+    if obs_t.numel() != W:
+        raise ValueError('obs has {} values, S has {} columns'.format(obs_t.numel(), W))
+    C = layout.n_combinations
+    if out is None:
+        out = dev.empty((C, B))
+    if tuple(out.shape[:1]) != (C,) or out.dim() != 2 or out.shape[1] < B or \
+            (B and out.stride(1) != 1):
+        raise ValueError('out must be a ({}, >= {}) device matrix'.format(C, B))
+    _lib.call('elfi_b200_subset_distance_f64', dev.context(), SUBSET_METRIC_CODES[metric],
+              dev.ptr(S), _ld(S), B, W, dev.ptr(obs_t), dev.ptr(layout.ranges),
+              dev.ptr(layout.offsets), C, dev.ptr(out), max(out.stride(0), B), dev.stream_ptr())
+    return out
+
+
+def _point_sets(X, name):
+    """X (C, n, q) or (n, q) as a contiguous (C, n, q) float64 device array."""
+    if not (dev.is_device_array(X) and X.dtype == torch.float64):
+        X = dev.to_device(X)
+    if X.dim() == 2:
+        X = X[None]
+    if X.dim() != 3:
+        raise ValueError('{} takes (sets, points, dim) or (points, dim) data, got shape {}'.format(
+            name, tuple(X.shape)))
+    return X.contiguous()
+
+
+def knn_entropy(X, k):
+    """The k-th nearest-neighbour radii of C point sets and their log sums (the device part of
+    diagnostics.py:214-253).  X (C, n, q) or (n, q).  Returns (R (C, n), logsum (C,)): R[c, i] is
+    cKDTree(X[c]).query(X[c, i], k)[0][-1] and logsum[c] = sum_i log R[c, i] in a fixed order."""
+    X = _point_sets(X, 'knn_entropy')
+    C, n, q = (int(s) for s in X.shape)
+    k = int(k)
+    if not 1 <= q <= KNN_MAX_Q:
+        raise ValueError('knn_entropy takes 1 <= q <= {} dimensions, got {}'.format(KNN_MAX_Q, q))
+    if not 1 <= k <= KNN_MAX_K:
+        raise ValueError('knn_entropy takes 1 <= k <= {}, got {}'.format(KNN_MAX_K, k))
+    if not 1 <= n <= KNN_MAX_N:
+        raise ValueError('knn_entropy takes 1 <= n <= {} points per set, got {}'.format(
+            KNN_MAX_N, n))
+    if not 1 <= C <= KNN_MAX_SETS:
+        raise ValueError('knn_entropy takes 1 to {} sets, got {}'.format(KNN_MAX_SETS, C))
+    R = dev.empty((C, n))
+    logsum = dev.empty((C,))
+    _lib.call('elfi_b200_knn_entropy_f64', dev.context(), dev.ptr(X), q, C, n, q, k, dev.ptr(R),
+              dev.ptr(logsum), dev.stream_ptr())
+    return R, logsum
+
+
+def mrsse(T, P, out=None):
+    """Mean root sum of squared errors of C parameter sets against m 'closest' parameter vectors
+    (diagnostics.py:255-289): out[c] = mean_j ||T[c] - P[j]||_F.  T (C, n, q) or (n, q), P (m, q).
+    Returns a (C,) device array (`out` if given)."""
+    T = _point_sets(T, 'mrsse')
+    C, n, q = (int(s) for s in T.shape)
+    Pd = _matrix(P)
+    m = int(Pd.shape[0])
+    if not 1 <= q <= KNN_MAX_Q:
+        raise ValueError('mrsse takes 1 <= q <= {} dimensions, got {}'.format(KNN_MAX_Q, q))
+    if int(Pd.shape[1]) != q:
+        raise ValueError('P has {} columns, the sets {}'.format(int(Pd.shape[1]), q))
+    if n < 1 or m < 1 or C < 1:
+        raise ValueError('mrsse needs at least one set, one point and one closest vector')
+    res = dev.empty((C,)) if out is None else out
+    if res.numel() != C or not res.is_contiguous():
+        raise ValueError('out must be a contiguous device buffer of {} doubles'.format(C))
+    _lib.call('elfi_b200_mrsse_f64', dev.context(), dev.ptr(T), q, C, n, q, dev.ptr(Pd), _ld(Pd),
+              m, dev.ptr(res), dev.stream_ptr())
+    return res

@@ -823,6 +823,66 @@ int elfi_b200_kliep_fit_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx, in
 int elfi_b200_rowsort_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, int64_t B, int64_t n,
                           double* out, int64_t ld_out, void* stream);
 
+/* ---- summary-statistic selection (TwoStageSelection, elfi/methods/diagnostics.py) -------------
+ * elfi_b200_subset_distance_f64: the distance of every candidate combination of summaries, from
+ * one read of each row (diagnostics.py:172-212 runs one rejection sampler per combination).
+ *   S       (B, W) row-major resident summary columns, leading dimension ldS >= W; a candidate
+ *           summary is a column range [col, col + width) of it.
+ *   obs     (W) the observed summaries in the same columns.
+ *   ranges  device int32 (n_ranges, 2) rows (col, width), width >= 1, col + width <= W;
+ *   comb    device int32 (C + 1) offsets: combination c is the ordered list of ranges
+ *           comb[c] .. comb[c + 1] - 1 (at least one).
+ *   d_out   (C, ld_out) row-major, ld_out >= B: d_out[c, i] = cdist(X_c[i], obs_c, metric), where
+ *           X_c and obs_c are the concatenations of combination c's ranges in list order.
+ * metric is ELFI_B200_METRIC_EUCLIDEAN, _SQEUCLIDEAN, _CITYBLOCK or _CHEBYSHEV; the terms are
+ * accumulated left to right over the concatenated columns with one rounding per multiply and add,
+ * the arithmetic of elfi_b200_dist_metric_thr_f64, so every value is bit-identical to SciPy's cdist
+ * on the concatenation, NaN and +-inf included (a NaN term makes the sums NaN; 'chebyshev' skips
+ * it, as SciPy does).  Limits: 1 <= W <= 512, 1 <= C < 2^24, 0 <= B < 2^31.  One CTA stages 32
+ * rows in shared memory (32 (W + 1) doubles) and its warps take the combinations in turn, so each
+ * row is read from HBM once for all C.  No scratch, no atomics: repeated calls give the same bits.
+ * Asynchronous on `stream`. */
+#define ELFI_B200_METRIC_EUCLIDEAN 0
+int elfi_b200_subset_distance_f64(elfi_b200_ctx* ctx, int32_t metric, const double* S, int64_t ldS,
+                                  int64_t B, int64_t W, const double* obs, const int32_t* ranges,
+                                  const int32_t* comb, int64_t C, double* d_out, int64_t ld_out,
+                                  void* stream);
+
+/* elfi_b200_knn_entropy_f64: the nearest-neighbour part of the minimum-entropy criterion
+ * (diagnostics.py:214-253) for C point sets of n points in q dimensions at once.
+ *   X       (C * n, q) row-major, leading dimension ldX >= q: set c is rows c n .. c n + n - 1.
+ *   R       (C, n): R[c, i] = the k-th smallest Euclidean distance from point i of set c to the
+ *           points of set c, the point itself included -- cKDTree(X_c).query(X_c[i], k)[0][-1]: the
+ *           self-distance is 0, so k = 1 gives 0; a duplicate gives 0; k > n gives +inf.  Squared
+ *           distances are summed over the q coordinates in order with one rounding per multiply
+ *           and add, then the root is taken (cKDTree agrees to a few ulps).  Coordinates must be
+ *           finite.
+ *   logsum  (C): logsum[c] = sum_i log(R[c, i]) added in a fixed order (each of 256 threads sums
+ *           i = t, t + 256, ... in turn, then a fixed pairwise tree), so identical sets give
+ *           identical bits; a zero R gives -inf, an infinite one +inf.
+ * The host forms the entropy log(pi^(q/2) / Gamma(q/2 + 1)) - digamma(k) + log(n) + q / n logsum.
+ * Limits: 1 <= q <= 16, 1 <= k <= 32, 1 <= n <= 2^20, 1 <= C < 2^16.  Brute force: a CTA of 128
+ * query points streams the set through shared memory in tiles of 256 points, and each thread keeps
+ * its k smallest squared distances in registers (a sorted insertion).  Two launches, no scratch,
+ * no atomics.  Asynchronous on `stream`. */
+int elfi_b200_knn_entropy_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, int64_t C,
+                              int64_t n, int64_t q, int64_t k, double* R, double* logsum,
+                              void* stream);
+
+/* elfi_b200_mrsse_f64: the mean root sum of squared errors of diagnostics.py:255-289 for C sets.
+ *   T       (C * n, q) row-major, leading dimension ldT >= q: set c is rows c n .. c n + n - 1.
+ *   P       (m, q) row-major, leading dimension ldP >= q: the m 'closest' parameter vectors.
+ *   out     (C): out[c] = sum_j sqrt(sum_{i,l} (T_c[i, l] - P[j, l])^2) / m, j = 0 .. m - 1 -- the
+ *           Frobenius norm of the (n, q) difference per closest vector.  Each sum of squares is
+ *           taken in a fixed order (256 threads over the n q entries, then a fixed tree) and the
+ *           roots are added in order of j, so repeated calls give the same bits; NumPy's norm sums
+ *           in another order, so the two agree to rounding.  NaN and inf propagate.
+ * Limits: 1 <= q <= 16, 1 <= n q < 2^31, 1 <= m < 2^31, 1 <= C < 2^31.  One CTA per set, one
+ * launch, no scratch, no atomics.  Asynchronous on `stream`. */
+int elfi_b200_mrsse_f64(elfi_b200_ctx* ctx, const double* T, int64_t ldT, int64_t C, int64_t n,
+                        int64_t q, const double* P, int64_t ldP, int64_t m, double* out,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif
