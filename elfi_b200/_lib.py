@@ -139,6 +139,19 @@ SIGNATURES = {
                                   c_ptr],
     'elfi_b200_mrsse_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_i64, c_i64, c_ptr,
                             c_ptr],
+    'elfi_b200_romc_nm_init_f64': [c_ptr, c_i64, c_i64, c_ptr, c_i64, c_ptr, c_ptr, c_ptr, c_i64,
+                                   c_ptr],
+    'elfi_b200_romc_nm_step_f64': [c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64,
+                                   c_i64, c_dbl, c_dbl, c_ptr],
+    'elfi_b200_romc_line_search_f64': [c_ptr, ctypes.c_int32, c_i64, c_i64, c_ptr, c_ptr, c_ptr,
+                                       c_ptr, c_ptr, c_ptr, c_ptr, c_dbl, c_i64, c_dbl, c_i64,
+                                       c_ptr, c_ptr],
+    'elfi_b200_romc_box_sample_f64': [c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
+                                      c_u64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
+    'elfi_b200_romc_weights_f64': [c_ptr, c_i64, c_ptr, c_ptr, c_ptr, c_dbl, c_ptr, c_ptr],
+    'elfi_b200_romc_posterior_unnorm_f64': [c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr, c_ptr,
+                                            c_ptr, c_ptr, c_ptr, c_i64, c_dbl, c_ptr, c_ptr,
+                                            c_ptr],
     'elfi_b200_gp_padded_size': [c_i64],
     'elfi_b200_gp_fit_f64': [c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_i64, c_dbl, c_dbl, c_dbl, c_dbl,
                              c_ptr, c_ptr, c_ptr, c_i64, c_ptr, c_ptr, c_ptr],

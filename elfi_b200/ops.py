@@ -1964,3 +1964,179 @@ def mrsse(T, P, out=None):
     _lib.call('elfi_b200_mrsse_f64', dev.context(), dev.ptr(T), q, C, n, q, dev.ptr(Pd), _ld(Pd),
               m, dev.ptr(res), dev.stream_ptr())
     return res
+
+
+# ---- robust optimisation Monte Carlo (ROMC, elfi/methods/inference/romc.py) ---------------------
+ROMC_MAX_P = 16
+ROMC_NM_INTS = 8
+ROMC_NM_DONE = 6
+
+
+def romc_nm_doubles(p):
+    """Doubles of device Nelder-Mead state per problem (include/elfi_b200.h)."""
+    return (p + 1) * (p + 1) + 3 * p + 2
+
+
+def _romc_p(p):
+    p = int(p)
+    if not 1 <= p <= ROMC_MAX_P:
+        raise ValueError('ROMC takes 1 <= p <= {} parameters, got {}'.format(ROMC_MAX_P, p))
+    return p
+
+
+def _dev_f64(x):
+    t = x if dev.is_device_array(x) and x.dtype == torch.float64 else dev.to_device(x)
+    return t.contiguous()
+
+
+class RomcNelderMead:
+    """P Nelder-Mead problems advanced in lock-step on the device (scipy's _minimize_neldermead
+    with adaptive=False and no bounds).  ``theta`` (P, p) holds the point every problem needs
+    next; pass f at those points to :meth:`step` until :meth:`running` is 0."""
+
+    def __init__(self, x0, maxiter=None, maxfev=None, xatol=1e-4, fatol=1e-4):
+        x0 = _dev_f64(x0)
+        if x0.dim() != 2:
+            raise ValueError('x0 must be (P, p), got shape {}'.format(tuple(x0.shape)))
+        self.P, self.p = int(x0.shape[0]), _romc_p(x0.shape[1])
+        self.maxiter = 200 * self.p if maxiter is None else int(maxiter)
+        self.maxfev = 200 * self.p if maxfev is None else int(maxfev)
+        if self.maxiter < 1 or self.maxfev < 1:
+            raise ValueError('maxiter and maxfev must be positive')
+        self.xatol, self.fatol = float(xatol), float(fatol)
+        self.state = dev.empty((self.P, romc_nm_doubles(self.p)))
+        self.istate = dev.empty((self.P, ROMC_NM_INTS), dtype=torch.int32)
+        self.theta = dev.empty((self.P, self.p))
+        _lib.call('elfi_b200_romc_nm_init_f64', dev.context(), self.P, self.p, dev.ptr(x0), self.p,
+                  dev.ptr(self.state), dev.ptr(self.istate), dev.ptr(self.theta), self.p,
+                  dev.stream_ptr())
+
+    def step(self, fvals):
+        f = _dev_f64(fvals).reshape(-1)
+        if f.numel() != self.P:
+            raise ValueError('step takes {} values, got {}'.format(self.P, f.numel()))
+        _lib.call('elfi_b200_romc_nm_step_f64', dev.context(), self.P, self.p, dev.ptr(self.state),
+                  dev.ptr(self.istate), dev.ptr(f), dev.ptr(self.theta), self.p, self.maxiter,
+                  self.maxfev, self.xatol, self.fatol, dev.stream_ptr())
+
+    def running(self):
+        """Problems not finished (one device-to-host read)."""
+        return int((self.istate[:, 0] != ROMC_NM_DONE).sum())
+
+    def result(self):
+        """Host (x_min (P, p), f_min (P,), nit (P,), nfev (P,), success (P,))."""
+        s, i = dev.to_host(self.state), dev.to_host(self.istate)
+        return (s[:, :self.p].copy(), s[:, -1].copy(), i[:, 1].astype(np.int64),
+                i[:, 2].astype(np.int64), i[:, 4] == 0)
+
+
+class RomcLineSearch:
+    """romc.py line_search for the 2p (direction, side) pairs of every active problem in
+    lock-step.  ``theta`` (2p, P, p) holds the next points; pass f at them, (2p, P), to
+    :meth:`step` until :meth:`running` is 0.  ``limits()`` is the (P, p, 2) box of each problem."""
+
+    def __init__(self, x_min, rot, active, eps, K=10, eta=1.0, rep_lim=300):
+        self.x_min = _dev_f64(x_min)
+        self.P, self.p = int(self.x_min.shape[0]), _romc_p(self.x_min.shape[1])
+        self.rot = _dev_f64(rot)
+        if tuple(self.rot.shape) != (self.P, self.p, self.p):
+            raise ValueError('rot must be ({0}, {1}, {1})'.format(self.P, self.p))
+        act = np.asarray(dev.to_host(active) if dev.is_device_array(active) else active).reshape(-1)
+        if act.size != self.P:
+            raise ValueError('active has {} entries, x_min {} rows'.format(act.size, self.P))
+        self.active = dev.to_device(act.astype(np.int32), dtype=torch.int32)
+        self.eps, self.K, self.eta, self.rep_lim = float(eps), int(K), float(eta), int(rep_lim)
+        if self.K < 1 or self.rep_lim < 0 or not (self.eta > 0 and np.isfinite(self.eta)):
+            raise ValueError('line search needs K >= 1, rep_lim >= 0 and a finite eta > 0')
+        n = 2 * self.p * self.P
+        self.state = dev.empty((n, self.p + 2))
+        self.istate = dev.empty((n, 4), dtype=torch.int32)
+        self.theta = dev.empty((2 * self.p, self.P, self.p))
+        self._limits = dev.zeros((self.P, self.p, 2))
+        self._call(1, None)
+
+    def _call(self, init, f):
+        _lib.call('elfi_b200_romc_line_search_f64', dev.context(), init, self.P, self.p,
+                  dev.ptr(self.x_min), dev.ptr(self.rot), dev.ptr(self.active), dev.ptr(self.state),
+                  dev.ptr(self.istate), dev.ptr(f), dev.ptr(self.theta), self.eps, self.K,
+                  self.eta, self.rep_lim, dev.ptr(self._limits), dev.stream_ptr())
+
+    def step(self, fvals):
+        f = _dev_f64(fvals)
+        if f.numel() != 2 * self.p * self.P:
+            raise ValueError('step takes (2p, P) = ({}, {}) values'.format(2 * self.p, self.P))
+        self._call(0, f)
+
+    def running(self):
+        return int((self.istate[:, 2] == 0).sum())
+
+    def limits(self):
+        return dev.to_host(self._limits)
+
+
+def romc_box_sample(center, rot, rot_inv, limits, volume, n2, seed, coef=None):
+    """n2 uniform draws from each of R rotated boxes (include/elfi_b200.h).  Returns device
+    (pts (R, n2, p), q (R, n2), surr (R, n2) or None): q = contains / volume, surr the region's
+    local quadratic (coef (R, 1 + p + p (p + 1) / 2)) at each point."""
+    center = _dev_f64(center)
+    R, p = int(center.shape[0]), _romc_p(center.shape[1])
+    rot, rot_inv, limits, volume = (_dev_f64(a) for a in (rot, rot_inv, limits, volume))
+    if tuple(rot.shape) != (R, p, p) or tuple(rot_inv.shape) != (R, p, p) or \
+            tuple(limits.shape) != (R, p, 2) or volume.numel() != R:
+        raise ValueError('box_sample takes center (R, p), rot and rot_inv (R, p, p), limits '
+                         '(R, p, 2) and volume (R,)')
+    n2 = int(n2)
+    if n2 < 0:
+        raise ValueError('n2 must be non-negative, got {}'.format(n2))
+    if coef is not None:
+        coef = _dev_f64(coef)
+        if tuple(coef.shape) != (R, 1 + p + p * (p + 1) // 2):
+            raise ValueError('coef must be (R, 1 + p + p (p + 1) / 2)')
+    pts, q = dev.empty((R, n2, p)), dev.empty((R, n2))
+    surr = None if coef is None else dev.empty((R, n2))
+    _lib.call('elfi_b200_romc_box_sample_f64', dev.context(), R, p, n2, dev.ptr(center),
+              dev.ptr(rot), dev.ptr(rot_inv), dev.ptr(limits), dev.ptr(volume),
+              int(seed) & 0xffffffffffffffff, dev.ptr(coef), dev.ptr(pts), dev.ptr(q),
+              dev.ptr(surr), dev.stream_ptr())
+    return pts, q, surr
+
+
+def romc_weights(dist, prior, q, eps):
+    """(dist < eps) prior / q, 0 where q <= 0, elementwise; a device array of dist's shape."""
+    dist, prior, q = (_dev_f64(a) for a in (dist, prior, q))
+    n = dist.numel()
+    if prior.numel() != n or q.numel() != n:
+        raise ValueError('dist, prior and q must have the same number of entries')
+    w = dev.empty(tuple(dist.shape))
+    _lib.call('elfi_b200_romc_weights_f64', dev.context(), n, dev.ptr(dist), dev.ptr(prior),
+              dev.ptr(q), float(eps), dev.ptr(w), dev.stream_ptr())
+    return w
+
+
+def romc_posterior_unnorm(theta, prior, eps, center=None, rot_inv=None, limits=None, coef=None,
+                          fvals=None):
+    """prior (M,) times the number of regions that count theta (M, p): with local models those
+    containing it whose quadratic is <= eps, else those whose objective value fvals (M, R) is
+    <= eps.  A device array (M,)."""
+    theta = _dev_f64(theta)
+    M, p = int(theta.shape[0]), _romc_p(theta.shape[1])
+    prior = _dev_f64(prior)
+    if prior.numel() != M:
+        raise ValueError('prior has {} values, theta {} rows'.format(prior.numel(), M))
+    if fvals is not None:
+        fvals = _dev_f64(fvals)
+        if fvals.dim() != 2 or int(fvals.shape[0]) != M:
+            raise ValueError('fvals must be (M, R)')
+        R = int(fvals.shape[1])
+    else:
+        center, rot_inv, limits, coef = (_dev_f64(a) for a in (center, rot_inv, limits, coef))
+        R = int(center.shape[0])
+        if tuple(center.shape) != (R, p) or tuple(rot_inv.shape) != (R, p, p) or \
+                tuple(limits.shape) != (R, p, 2) or tuple(coef.shape) != (R, 1 + p + p * (p + 1) // 2):
+            raise ValueError('posterior_unnorm takes center (R, p), rot_inv (R, p, p), limits '
+                             '(R, p, 2) and coef (R, 1 + p + p (p + 1) / 2)')
+    out = dev.empty((M,))
+    _lib.call('elfi_b200_romc_posterior_unnorm_f64', dev.context(), M, R, p, dev.ptr(theta), p,
+              dev.ptr(center), dev.ptr(rot_inv), dev.ptr(limits), dev.ptr(coef), dev.ptr(fvals),
+              R, float(eps), dev.ptr(prior), dev.ptr(out), dev.stream_ptr())
+    return out

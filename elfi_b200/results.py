@@ -198,3 +198,11 @@ class BslSample(Sample):
         """Effective sample size of the chain after burn-in, per parameter."""
         from .mcmc import eff_sample_size
         return {p: eff_sample_size(self.samples[p]) for p in self.parameter_names}
+
+
+class RomcSample(Sample):
+    """Weighted draws of ROMC (elfi/methods/results.py RomcSample)."""
+
+    def samples_cov(self):
+        """The weighted covariance matrix of the draws."""
+        return np.cov(self.samples_array, rowvar=False, aweights=self.weights)

@@ -883,6 +883,98 @@ int elfi_b200_mrsse_f64(elfi_b200_ctx* ctx, const double* T, int64_t ldT, int64_
                         int64_t q, const double* P, int64_t ldP, int64_t m, double* out,
                         void* stream);
 
+/* ---- robust optimisation Monte Carlo (ROMC, elfi/methods/inference/romc.py) ----------------
+ * P optimisation problems with 1 <= p <= 16 parameters advance in lock-step: every call consumes
+ * the objective value of the point each problem proposed last call and writes the next point.
+ * The host evaluates all P points of a call as one batch, so the stream row of problem i stays i.
+ * Products, sums and quotients that must match NumPy use round-to-nearest intrinsics (no FMA).
+ * One thread per problem (or per point), no scratch, no atomics.  Asynchronous on `stream`. */
+#define ELFI_B200_ROMC_MAX_P 16
+#define ELFI_B200_ROMC_NM_INTS 8   /* ints of Nelder-Mead state per problem */
+/* doubles of Nelder-Mead state per problem: the simplex (p + 1, p), fsim (p + 1), xbar, the
+ * reflected point and the trial point (p each), f at the reflection and f_min */
+#define ELFI_B200_ROMC_NM_DOUBLES(p) (((p) + 1) * ((p) + 1) + 3 * (p) + 2)
+
+/* elfi_b200_romc_nm_init_f64: scipy's initial simplex around each x0 row (x0, then x0 with
+ * coordinate k scaled by 1 + 0.05, or set to 0.00025 when it is 0) and fsim = +inf.
+ *   x0       (P, p), leading dimension ld_x0 >= p.
+ *   state    (P, ELFI_B200_ROMC_NM_DOUBLES(p)) and istate (P, ELFI_B200_ROMC_NM_INTS), written.
+ *   theta    (P, p), leading dimension ld_theta: the first point of every problem (x0). */
+int elfi_b200_romc_nm_init_f64(elfi_b200_ctx* ctx, int64_t P, int64_t p, const double* x0,
+                               int64_t ld_x0, double* state, int32_t* istate, double* theta,
+                               int64_t ld_theta, void* stream);
+
+/* elfi_b200_romc_nm_step_f64: one step of scipy 1.18's _minimize_neldermead (adaptive=False,
+ * bounds=None) per problem.  fvals (P) holds f at the points of the previous call; each running
+ * problem advances to the next point it needs and writes it to row i of theta.  The reflection,
+ * expansion, outside and inside contractions and the shrink use scipy's expressions in scipy's
+ * order (xbar = the first p vertices added row after row, divided by p); a shrink proposes its p
+ * vertices in p calls.  The convergence test (xatol, fatol), the maxiter / maxfev stops and an
+ * evaluation refused at maxfev (the iteration is not counted) are scipy's.  Vertices are ordered
+ * by a stable sort, NaN last: np.argsort's order whenever fsim has no ties, and for p <= 2; with
+ * ties at p >= 3 NumPy's order depends on the CPU's SIMD sort (DESIGN.md section 7, "ROMC").
+ * A finished problem keeps x_min in its theta row and ignores its value from then on:
+ *   istate[i, 0] = 6 (done), istate[i, 1] = nit, istate[i, 2] = nfev, istate[i, 4] = scipy's
+ *   warnflag (0 success, 1 maxfev, 2 maxiter); the first p doubles of state row i are x_min and
+ *   double ELFI_B200_ROMC_NM_DOUBLES(p) - 1 is f_min = np.min(fsim) (NaN when any vertex is NaN).
+ * Limits: 0 <= P < 2^31, 1 <= maxiter, maxfev < 2^30. */
+int elfi_b200_romc_nm_step_f64(elfi_b200_ctx* ctx, int64_t P, int64_t p, double* state,
+                               int32_t* istate, const double* fvals, double* theta,
+                               int64_t ld_theta, int64_t maxiter, int64_t maxfev, double xatol,
+                               double fatol, void* stream);
+
+/* elfi_b200_romc_line_search_f64: romc.py line_search for the 2p (direction, side) pairs of every
+ * problem with active[i] != 0.  Pair dp = 2 d + s searches from x_min[i] along -v (s = 0) or +v
+ * (s = 1), v = column d of rot[i] (P, p, p row-major): while f(th) < eps and rep <= rep_lim,
+ * th += eta v and offset += eta; then one step back, and eta halves, K times or until rep_lim is
+ * exceeded; an offset <= 0 becomes the last eta.
+ *   init != 0: th = x_min for every pair; fvals is not read.
+ *   fvals    (2p, P): f at the points of the previous call; theta (2p, P, p): the next points.
+ *   state    (2p P, p + 2) doubles and istate (2p P, 4) ints.
+ *   limits   (P, p, 2): limits[i, d, 0] = -offset of side 0, limits[i, d, 1] = offset of side 1,
+ *            written when the pair finishes; istate[t, 2] != 0 marks a finished pair t = dp P + i.
+ * Limits: 2 p P < 2^31, 1 <= K < 2^30, 0 <= rep_lim < 2^30, finite eta > 0. */
+int elfi_b200_romc_line_search_f64(elfi_b200_ctx* ctx, int32_t init, int64_t P, int64_t p,
+                                   const double* x_min, const double* rot, const int32_t* active,
+                                   double* state, int32_t* istate, const double* fvals,
+                                   double* theta, double eps, int64_t K, double eta,
+                                   int64_t rep_lim, double* limits, void* stream);
+
+/* elfi_b200_romc_box_sample_f64: n2 uniform points in each of R rotated boxes.
+ *   center (R, p), rot and rot_inv (R, p, p), limits (R, p, 2) [lo, hi], volume (R).
+ *   pts (R, n2, p): point j of box r is center + rot (lo + (hi - lo) u), u_d the 53-bit (0, 1]
+ *            uniform of Philox4x32-10 keyed by seed at counter (j, r, d / 2, 0x524f4d43), words
+ *            (x, y) for even d and (z, w) for odd d; the product is summed over d in order.
+ *   q (R, n2): 1 / volume[r] when rot_inv (x - center) lies within [lo, hi] (NDimBoundingBox.
+ *            contains), else 0.
+ *   surr (R, n2), optional (then coef (R, 1 + p + p (p + 1) / 2) is read): the region's local
+ *            quadratic at the point, coefficients in PolynomialFeatures(degree=2) order (1, x_i,
+ *            then x_i x_j for i <= j), summed in that order. */
+int elfi_b200_romc_box_sample_f64(elfi_b200_ctx* ctx, int64_t R, int64_t p, int64_t n2,
+                                  const double* center, const double* rot, const double* rot_inv,
+                                  const double* limits, const double* volume, uint64_t seed,
+                                  const double* coef, double* pts, double* q, double* surr,
+                                  void* stream);
+
+/* elfi_b200_romc_weights_f64: RomcPosterior.sample's weights, w = (dist < eps) prior / q, or 0
+ * when q <= 0; all arrays (n). */
+int elfi_b200_romc_weights_f64(elfi_b200_ctx* ctx, int64_t n, const double* dist,
+                               const double* prior, const double* q, double eps, double* w,
+                               void* stream);
+
+/* elfi_b200_romc_posterior_unnorm_f64: RomcPosterior's unnormalised density at M points theta
+ * (M, p; leading dimension ld_theta): out[m] = prior[m] * count[m], where with fitted local
+ * models (fvals NULL) count[m] = #{k : region k contains theta_m and its quadratic <= eps}, and
+ * without them (fvals (M, R), leading dimension ld_f) count[m] = #{k : fvals[m, k] <= eps}, as the
+ * reference counts objectives without a surrogate.  center, rot_inv, limits and coef as above.
+ * Limits: M < 2^40, R < 2^31. */
+int elfi_b200_romc_posterior_unnorm_f64(elfi_b200_ctx* ctx, int64_t M, int64_t R, int64_t p,
+                                        const double* theta, int64_t ld_theta,
+                                        const double* center, const double* rot_inv,
+                                        const double* limits, const double* coef,
+                                        const double* fvals, int64_t ld_f, double eps,
+                                        const double* prior, double* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
