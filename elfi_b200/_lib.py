@@ -129,6 +129,13 @@ SIGNATURES = {
                                               c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr],
     'elfi_b200_synlik_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr, c_ptr,
                              ctypes.c_int32, c_ptr, c_i64, c_ptr, c_ptr],
+    'elfi_b200_regadj_mask_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_i64, c_i64,
+                                  c_ptr, c_ptr, c_ptr],
+    'elfi_b200_regadj_moments_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_i64, c_i64,
+                                     c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr],
+    'elfi_b200_regadj_adjust_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_i64, c_i64,
+                                    c_ptr, c_ptr, c_i64, c_i64, ctypes.c_int32, c_ptr, c_ptr, c_i64,
+                                    c_ptr],
     'elfi_b200_logreg_fit_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, ctypes.c_int32, c_dbl,
                                  c_i64, c_ptr, c_ptr],
     'elfi_b200_logreg_predict_f64': [c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_i64, c_dbl, c_ptr,

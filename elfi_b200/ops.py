@@ -2140,3 +2140,125 @@ def romc_posterior_unnorm(theta, prior, eps, center=None, rot_inv=None, limits=N
               dev.ptr(center), dev.ptr(rot_inv), dev.ptr(limits), dev.ptr(coef), dev.ptr(fvals),
               R, float(eps), dev.ptr(prior), dev.ptr(out), dev.stream_ptr())
     return out
+
+
+# ---- regression adjustment (elfi/methods/post_processing.py: LinearAdjustment) ----------------------
+REGADJ_D_MAX = 256             # q + p: the mean and the tile rows of one group in shared memory
+REGADJ_N_MAX = 2 ** 31 - 1     # rows: int32 row ranks in the kernels' compaction
+
+
+def _regadj_shape(x):
+    return tuple(x.shape) if hasattr(x, 'shape') else np.shape(x)
+
+
+def _regadj_block(X, name):
+    """X as an (N, w) float64 device matrix with unit column stride: an (N, w) array, or a list of w
+    (N,) columns (stacked here).  Shapes are checked before anything is uploaded."""
+    if isinstance(X, (list, tuple)):
+        if not X:
+            raise ValueError('{} has no columns'.format(name))
+        lengths = set()
+        for j, c in enumerate(X):
+            shape = _regadj_shape(c)
+            if len(shape) != 1:
+                raise ValueError('{} column {} must be 1-d (one scalar per row), got shape {}'.format(
+                    name, j, shape))
+            lengths.add(shape[0])
+        if len(lengths) != 1:
+            raise ValueError('the columns of {} differ in length: {}'.format(name, sorted(lengths)))
+        N = lengths.pop()
+        if N > REGADJ_N_MAX:
+            raise ValueError('{} has N = {} rows; linear_adjust takes N < 2^31'.format(name, N))
+        cols = [c if dev.is_device_array(c) and c.dtype == torch.float64 else dev.to_device(c)
+                for c in X]
+        return torch.stack(cols, dim=1)
+    shape = _regadj_shape(X)
+    if len(shape) != 2:
+        raise ValueError('{} must be an (N, width) array or a list of (N,) columns, got shape '
+                         '{}'.format(name, shape))
+    if shape[0] > REGADJ_N_MAX:
+        raise ValueError('{} has N = {} rows; linear_adjust takes N < 2^31'.format(name, shape[0]))
+    M = X if dev.is_device_array(X) and X.dtype == torch.float64 else dev.to_device(X)
+    if M.shape[0] > 0 and (M.stride(1) != 1 or M.stride(0) < M.shape[1]):
+        M = M.contiguous()
+    return M
+
+
+def _regadj_solve(M, q, n, tol):
+    """The minimum-norm least-squares coefficients of the centred normal equations: the q x q block
+    A = X_c^T X_c and the q x pg block B = X_c^T Y_c of M.  Eigenvalues lambda <= tol^2 lambda_max
+    count as zero (scikit-learn's singular-value cut sigma <= tol sigma_max on X_c).  Returns coef
+    (q, pg), the rank and the singular values of X_c (descending, min(n, q) of them)."""
+    A, B = M[:q, :q], M[:q, q:]
+    w, V = np.linalg.eigh(A)
+    keep = w > tol * tol * w[-1] if w[-1] > 0 else np.zeros(q, dtype=bool)
+    Vr = V[:, keep]
+    coef = Vr @ ((Vr.T @ B) / w[keep][:, None])
+    singular = np.sqrt(np.clip(w[::-1], 0.0, None))[:min(n, q)]
+    return coef, int(keep.sum()), singular
+
+
+def linear_adjust(S, theta, observed, tol=1e-6):
+    """The local-linear regression adjustment of Beaumont et al. (2002), one least-squares fit with
+    an intercept per parameter, regressors x_i = S_i - observed.
+
+    S is (N, q) and theta (N, p), host or device, each as an array (any row stride) or a list of
+    (N,) columns.  Parameter k is fitted on the rows whose summaries and theta_k are finite; every
+    parameter without a non-finite theta_k on such rows shares one fit.  Each fit reads back its
+    count, means and centred (q + p_g)^2 moments and solves them on the host (_regadj_solve).
+
+    Returns (adjusted, fits): adjusted[k] is a device column (n_k,) of theta_k - x @ coef_k over
+    parameter k's rows in row order; fits[k] is a dict with 'coef' (q,), 'intercept', 'rank',
+    'singular' and 'n_rows'.  ValueError for q + p > REGADJ_D_MAX, N >= 2^31, a column that is not
+    1-d, or a parameter without any finite row."""
+    tol = float(tol)
+    if not tol >= 0:
+        raise ValueError('tol must be non-negative, got {}'.format(tol))
+    Sd = _regadj_block(S, 'S')
+    Td = _regadj_block(theta, 'theta')
+    N, q = int(Sd.shape[0]), int(Sd.shape[1])
+    p = int(Td.shape[1])
+    if int(Td.shape[0]) != N:
+        raise ValueError('S has {} rows, theta {}'.format(N, int(Td.shape[0])))
+    if q < 1 or p < 1 or q + p > REGADJ_D_MAX:
+        raise ValueError('linear_adjust takes q >= 1 summaries and p >= 1 parameters with q + p <= '
+                         '{}, got q = {}, p = {}'.format(REGADJ_D_MAX, q, p))
+    if N == 0:
+        raise ValueError('linear_adjust needs at least one row, got N = 0')
+    o = dev.to_device(observed).reshape(-1).contiguous()
+    if o.numel() != q:
+        raise ValueError('observed has {} values, S has q = {} summaries'.format(o.numel(), q))
+    ctx, stream = dev.context(), dev.stream_ptr()
+    shape = (dev.ptr(Sd), _ld(Sd), N, q, dev.ptr(o), dev.ptr(Td), _ld(Td), p)
+    flags = dev.empty((N,), dtype=torch.uint8)
+    counts = dev.empty((p + 1,), dtype=torch.int64)
+    _lib.call('elfi_b200_regadj_mask_f64', ctx, *shape, dev.ptr(flags), dev.ptr(counts), stream)
+    bad = dev.to_host(counts)[1:]
+    shared = [k for k in range(p) if bad[k] == 0]
+    groups = ([(shared, -1)] if shared else []) + [([k], k) for k in range(p) if bad[k] != 0]
+    adjusted, fits = [None] * p, [None] * p
+    for cols, sel in groups:
+        pg = len(cols)
+        d = q + pg
+        cols_h = np.ascontiguousarray(cols, dtype=np.int32)
+        mom = dev.empty((1 + d + d * d,))
+        _lib.call('elfi_b200_regadj_moments_f64', ctx, *shape, dev.ptr(flags),
+                  ctypes.c_void_p(cols_h.ctypes.data), pg, sel, dev.ptr(mom), stream)
+        h = dev.to_host(mom)
+        n = int(h[0])
+        if n == 0:
+            raise ValueError('no row has finite summaries and a finite value of parameter {}: '
+                             'nothing to fit (n_samples = 0)'.format(cols[0]))
+        mean, M = h[1:1 + d], h[1 + d:].reshape(d, d)
+        coef, rank, singular = _regadj_solve(M, q, n, tol)
+        intercept = mean[q:] - mean[:q] @ coef
+        coef_d = dev.to_device(np.ascontiguousarray(coef))
+        out = dev.empty((pg, n))
+        _lib.call('elfi_b200_regadj_adjust_f64', ctx, *shape, dev.ptr(flags),
+                  ctypes.c_void_p(cols_h.ctypes.data), pg, sel, int(sel < 0 and n == N),
+                  dev.ptr(coef_d), dev.ptr(out), n, stream)
+        for kk, k in enumerate(cols):
+            adjusted[k] = out[kk]
+            fits[k] = dict(coef=coef[:, kk].copy(), intercept=float(intercept[kk]), rank=rank,
+                           singular=singular.copy(), n_rows=n)
+    return adjusted, fits

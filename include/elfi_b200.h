@@ -770,6 +770,42 @@ int elfi_b200_synlik_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_row, in
                          int32_t estimator, const double* penalties_host, int64_t K,
                          double* loglik, void* stream);
 
+/* ---- regression adjustment (elfi/methods/post_processing.py: LinearAdjustment) ------------------
+ * The local-linear adjustment of Beaumont et al. (2002) on N rows of q summaries
+ * S[i * ldS + j] (ldS >= q), the observed summaries obs (q) and p parameters T[i * ldT + k]
+ * (ldT >= p); all device.  The regressors are x_i = S_i - obs.
+ * elfi_b200_regadj_mask_f64: flags[i] (device, N bytes) = 1 when every S[i, j] - obs[j] is finite,
+ *   else 0 (a non-finite obs drops every row); counts (device, p + 1 int64) = [the flagged rows,
+ *   then per parameter k the flagged rows whose T[i, k] is not finite].
+ * A group is the parameter columns cols_host[0 .. pg - 1] (HOST int32, each in [0, p)) and the rows
+ *   with flags[i] != 0 and, when sel >= 0, T[i, sel] finite.  d = q + pg.
+ * elfi_b200_regadj_moments_f64: mom (device, 1 + d + d * d doubles) = [n_g, the means m of
+ *   [x | T_g] over the group's rows, the full symmetric d x d sum over those rows of
+ *   ([x | T_g] - m)([x | T_g] - m)^T, row-major].  Two passes, means first.  Rows are split into
+ *   chunks whose length depends on N and d only; each chunk sum starts from zero and the chunk sums
+ *   are added left to right, so the result is bit-identical across calls and GPUs.  n_g = 0
+ *   leaves NaN means and zero moments.
+ * elfi_b200_regadj_adjust_f64: for each group row i in row order and each k < pg,
+ *   out[k * ld_out + pos] = T[i, cols_host[k]] - sum_j (S[i, j] - obs[j]) coef[j * pg + k]
+ *   (coef device, q x pg row-major).  dense = 1 states that every row is in the group (n_g = N):
+ *   pos = i, with no compaction; dense = 0 gives pos = the rank of i among the group's rows.
+ *   ld_out >= N when dense.
+ * Limits: q, p >= 1, q + p <= 256, 1 <= N < 2^31, 1 <= pg <= p, -1 <= sel < p.  Asynchronous on
+ * `stream`; moments use about min(N / 256, 2048) * 64^2 doubles of the context's scratch, adjust
+ * N / 2048 int64. */
+int elfi_b200_regadj_mask_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t N,
+                              int64_t q, const double* obs, const double* T, int64_t ldT, int64_t p,
+                              uint8_t* flags, int64_t* counts, void* stream);
+int elfi_b200_regadj_moments_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t N,
+                                 int64_t q, const double* obs, const double* T, int64_t ldT,
+                                 int64_t p, const uint8_t* flags, const int32_t* cols_host,
+                                 int64_t pg, int64_t sel, double* mom, void* stream);
+int elfi_b200_regadj_adjust_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t N,
+                                int64_t q, const double* obs, const double* T, int64_t ldT,
+                                int64_t p, const uint8_t* flags, const int32_t* cols_host,
+                                int64_t pg, int64_t sel, int32_t dense, const double* coef,
+                                double* out, int64_t ld_out, void* stream);
+
 /* ---- BOLFIRE ratio-estimation classifier (elfi/methods/classifier.py: LogisticRegression) ------
  * elfi_b200_logreg_fit_f64: sklearn's StandardScaler then penalised logistic regression with
  * liblinear's primal and intercept_scaling = 1, on the n rows X[i * ld_row + j], j < d (device,
