@@ -8,8 +8,10 @@ Host control flow follows the reference (paths relative to elfi-dev/elfi):
   log_SL_stdev, select_penalty, estimate_whitening_matrix elfi/methods/bsl/pre_sample_methods.py
 What runs on the device: the simulations of a device model, the (n_sim_round, d) feature matrix
 of a round, and the whole likelihood (moments, shrinkage, whitening, Cholesky, log density:
-ops.synlik).  The host reads one value per round, for the Metropolis-Hastings step.  The
-pre-sample tools evaluate all M simulation sets, and all penalties, in one call.
+ops.synlik).  The host reads one value per chain and iteration, for the Metropolis-Hastings
+step; in throughput mode (device_proposal) the step runs on the device too (ops.bsl_mh_step) and
+hands the simulator device columns.  The pre-sample tools evaluate all M simulation sets, and all
+penalties, in one call.
 
 The standard (Warton-shrunk, whitened) and unbiased Gaussian likelihoods are provided.
 semiBSL, the R-BSL adjustments and graphical-lasso shrinkage raise NotImplementedError.  Any other
@@ -22,6 +24,8 @@ import scipy.linalg
 import torch
 
 from . import device as dev
+from . import mcmc
+from . import model as em
 from . import ops
 from .results import BslSample
 from .model_based import ModelBased, feature_columns, feature_list, observed_row
@@ -144,17 +148,29 @@ def _param_values(model, theta):
 class BSL(ModelBased):
     """Bayesian synthetic likelihood with a random-walk Metropolis-Hastings sampler (Price et al.
     2018).  Each round simulates n_sim_round times at one parameter; the round's features stay on
-    the device and go to one likelihood call.  Runs on this rank only."""
+    the device and go to one likelihood call.  Runs on this rank only.
+
+    Several chains (``sample(..., n_chains=C)``) run in lock-step: each batch holds batch_size rows
+    of every chain, and one likelihood call evaluates the C rounds of an iteration.
+    ``device_proposal`` (throughput mode, e.g. ``DeviceModelPrior(m)``: an object with the (p, 5)
+    prior table ``specs``, its ``sources`` and ``logpdf``) moves the proposals, the prior
+    densities, the Metropolis-Hastings decisions and the chains to the device
+    (ops.bsl_mh_step), so that the host only launches work; its chains follow the same sampler
+    from a Philox stream rather than the host RandomState."""
 
     D_MAX = ops.SYNLIK_D_MAX
 
     def __init__(self, model, n_sim_round, feature_names=None, likelihood=None, batch_size=None,
-                 seed=None, pool=None):
+                 seed=None, pool=None, device_proposal=None):
         super().__init__(model, n_sim_round, feature_names=feature_names, batch_size=batch_size,
                          seed=seed, pool=pool)
         self.random_state = np.random.RandomState(self.seed)
         self.likelihood = likelihood
         self._device_lik = _device_likelihood(likelihood)
+        if device_proposal is not None and self._device_lik is None:
+            raise ValueError('device_proposal keeps the chains on the device and needs a device '
+                             'likelihood (standard or unbiased), not a host callable')
+        self.device_proposal = device_proposal
         self._obs_dev = None
         self.param_names = None
         self.prior = None
@@ -167,113 +183,216 @@ class BSL(ModelBased):
         return self.param_names or self.model.parameter_names
 
     def sample(self, n_samples, sigma_proposals, params0=None, param_names=None, burn_in=0,
-               logit_transform_bound=None):
-        """Run a chain of n_samples iterations (burn-in included) from params0 with Gaussian
-        random-walk proposals of covariance sigma_proposals, in the logit-transformed space when
-        logit_transform_bound ((p, 2) lower and upper bounds) is given.  Returns a BslSample."""
+               logit_transform_bound=None, n_chains=1):
+        """Run n_chains chains of n_samples iterations (burn-in included) from params0 ((p,) for
+        every chain, or (n_chains, p); a prior draw per chain by default) with Gaussian random-walk
+        proposals of covariance sigma_proposals, in the logit-transformed space when
+        logit_transform_bound ((p, 2) lower and upper bounds) is given.  Chain 0 draws its
+        proposals and uniforms from RandomState(seed), chain c >= 1 from
+        RandomState(get_sub_seed(seed, c)).  Returns a BslSample; with n_chains > 1 it also holds
+        `chains` (n_chains, n_samples, p) and the per-chain `acc_rates`."""
+        n_chains = int(n_chains)
+        if n_chains < 1:
+            raise ValueError('n_chains must be at least 1, got {}'.format(n_chains))
+        if n_chains > 1 and self.pool is not None:
+            raise ValueError('BSL with n_chains > 1 does not store its batches in a pool')
         self.sigma_proposals = sigma_proposals
         self.param_names = param_names
         self.prior = ModelPrior(self.model, parameter_names=self.parameter_names)
         self.burn_in = burn_in
         self.logit_transform_bound = None if logit_transform_bound is None else \
             np.array(logit_transform_bound)
+        self._set_chains(n_chains)
         self._init_state(n_samples, params0)
         return self.infer(n_samples)
+
+    def _set_chains(self, C):
+        if C != self.n_chains:
+            self._sim = None
+        self.n_chains = C
+        self.computation_context.batch_size = C * self._rows_per_chain
+        self._random_states = [self.random_state] + [
+            np.random.RandomState(em.get_sub_seed(self.seed, c)) for c in range(1, C)]
+
+    def _initial_points(self, params0):
+        """(C, p) host starting points, each inside the prior support."""
+        C, p = self.n_chains, len(self.parameter_names)
+        if params0 is None:
+            drawn = self.model.generate(C, self.parameter_names, seed=self.seed)
+            return np.column_stack([dev.to_host(drawn[q]) for q in self.parameter_names])
+        params0 = np.array(params0, dtype=float)
+        if params0.size == p:
+            params0 = np.broadcast_to(params0.reshape(1, p), (C, p)).copy()
+        if params0.shape != (C, p):
+            raise ValueError('params0 must be ({0},) or ({1}, {0}), got shape {2}'.format(
+                p, C, params0.shape))
+        outside = ~np.isfinite(np.reshape(self.prior.logpdf(params0), -1))
+        if outside.any():
+            where = '' if C == 1 else ' (chain {})'.format(
+                ', '.join(str(c) for c in np.flatnonzero(outside)))
+            raise ValueError('Initial point {} is outside prior support{}.'.format(
+                params0[outside][0] if C > 1 else params0[0], where))
+        return params0
 
     def _init_state(self, n_samples, params0=None):
         self.state['n_batches'] = 0
         self.state['n_sim'] = 0
         self.state['round'] = 0
         self.state['n_sim_round'] = 0
-        if params0 is None:
-            drawn = self.model.generate(1, self.parameter_names, seed=self.seed)
-            params0 = np.column_stack([dev.to_host(drawn[p]) for p in self.parameter_names])
-        else:
-            params0 = np.array(params0)
-            if not np.isfinite(self.prior.logpdf(params0)):
-                raise ValueError('Initial point {} is outside prior support.'.format(params0))
         self.state['n_samples'] = 0
-        self.num_accepted = 0
-        self.state['params'] = np.zeros((n_samples, len(self.parameter_names)))
-        self.state['params'][0] = params0
-        self.state['logprior'] = np.zeros(n_samples)
-        self.state['logprior'][0] = np.reshape(self.prior.logpdf(params0), -1)[0]
-        self.state['logposterior'] = np.zeros(n_samples)
+        C, p = self.n_chains, len(self.parameter_names)
+        params0 = self._initial_points(params0)
+        # (C, n_samples, ...) host state; state[...] shows chain 0 alone when C = 1
+        self._params = np.zeros((C, n_samples, p))
+        self._logprior = np.zeros((C, n_samples))
+        self._logpost = np.zeros((C, n_samples))
+        self._n_acc = np.zeros(C, dtype=np.int64)
+        self._live = np.ones(C, dtype=bool)
+        self._params[:, 0] = params0
+        self._logprior[:, 0] = np.reshape(self.prior.logpdf(params0), -1)
+        self._share_state()
+        if self.device_proposal is not None:
+            self._init_device_chains(n_samples, params0)
+
+    def _share_state(self):
+        one = (lambda a: a[0]) if self.n_chains == 1 else (lambda a: a)
+        self.state['params'] = one(self._params)
+        self.state['logprior'] = one(self._logprior)
+        self.state['logposterior'] = one(self._logpost)
+
+    def _init_device_chains(self, n_samples, params0):
+        """Device state of throughput mode: the chains, their log posteriors and acceptance
+        counters, the pending proposals (params0 at iteration 0) and the (p, C b) parameters of
+        the next batch."""
+        dp = self.device_proposal
+        names = list(self.parameter_names)
+        if list(dp.parameter_names) != names:
+            raise ValueError('device_proposal has the parameters {}, the sampler {}'.format(
+                list(dp.parameter_names), names))
+        C, p, b = self.n_chains, len(names), self._rows_per_chain
+        sources = dp.sources if getattr(dp, '_cond', False) else None
+        self._tables = ops.bsl_mh_tables(dp.specs, self.sigma_proposals, sources,
+                                         self.logit_transform_bound)
+        self._prop = dev.to_device(params0).contiguous()
+        self._prop_lp = dp.logpdf(self._prop)
+        self._chains_dev = dev.zeros((C, n_samples, p))
+        self._logpost_dev = dev.zeros((C, n_samples))
+        self._n_acc_dev = dev.zeros((C,), dtype=torch.int64)
+        self._rows = dev.empty((p, C * b))
+        self._rows.view(p, C, b).copy_(self._prop.t()[:, :, None].expand(p, C, b))
+
+    def prepare_new_batch(self, batch_index):
+        if self.device_proposal is None:
+            return super().prepare_new_batch(batch_index)
+        return {q: self._rows[i] for i, q in enumerate(self.parameter_names)}
 
     @property
     def current_params(self):
-        return self.state['params'][self.state['n_samples']]
+        return self._params[:, self.state['n_samples']]
 
-    def _loglikelihood(self):
+    def _rounds(self):
+        return self._sim if self._sim.dim() == 3 else self._sim[None]
+
+    def _loglikelihoods(self):
+        """(C,) log-likelihoods of the rounds of the chains that simulated their proposal: a device
+        tensor for a device likelihood (one call with G = C), else a host array (NaN for the
+        other chains)."""
         if self._device_lik is not None:
             if self._obs_dev is None:
                 self._obs_dev = dev.to_device(self.observed.reshape(-1))
-            # the one device-to-host read of the round
-            return float(self._device_lik.device(self._sim, self._obs_dev)[0].item())
-        sim = dev.to_host(self._sim)
-        if not np.all(np.isfinite(sim)):
-            return -np.inf
-        return float(np.reshape(self.likelihood(sim, self.observed), -1)[0])
+            return self._device_lik.device(self._rounds(), self._obs_dev)
+        sims = dev.to_host(self._rounds())
+        ll = np.full(self.n_chains, np.nan)
+        for c in np.flatnonzero(self._live):
+            sim = sims[c]
+            ll[c] = -np.inf if not np.all(np.isfinite(sim)) else \
+                float(np.reshape(self.likelihood(sim, self.observed), -1)[0])
+        return ll
+
+    def _check_first_round(self, ll):
+        bad = np.flatnonzero(~np.isfinite(ll))
+        if len(bad):
+            where = '' if self.n_chains == 1 else ' (chain {})'.format(
+                ', '.join(str(c) for c in bad))
+            raise RuntimeError('Estimated likelihood not finite on initialisation round{}.'.format(
+                where))
 
     def _process_simulated(self):
-        loglikelihood = self._loglikelihood()
         n = self.state['n_samples']
-        if not np.isfinite(loglikelihood):
+        ll = self._loglikelihoods()
+        if self.device_proposal is not None:
             if n == 0:
-                raise RuntimeError('Estimated likelihood not finite on initialisation round.')
-            logger.warning('Estimated likelihood not finite.')
-        self.state['logposterior'][n] = loglikelihood + self.state['logprior'][n]
+                self._check_first_round(dev.to_host(ll))   # the one read of throughput mode
+            ops.bsl_mh_step(self._tables, n, ll, self._prop, self._prop_lp, self._chains_dev,
+                            self._logpost_dev, self._n_acc_dev, self._rows, int(self.seed),
+                            self.burn_in)
+            self.state['n_samples'] += 1
+            return
+        if dev.is_device_array(ll):
+            ll = dev.to_host(ll)          # the one device-to-host read of the iteration
         if n == 0:
-            accept = True
-        else:
-            prob = np.minimum(1.0, self._get_mh_ratio())
-            accept = self.random_state.uniform() < prob
-        if accept:
-            if n >= self.burn_in:
-                self.num_accepted += 1
-        else:
-            self._copy_previous(n)
+            self._check_first_round(ll)
+        if not np.all(np.isfinite(ll[self._live])):
+            logger.warning('Estimated likelihood not finite.')
+        for c in np.flatnonzero(self._live):
+            self._logpost[c, n] = ll[c] + self._logprior[c, n]
+            if n == 0:
+                accept = True
+            else:
+                prob = np.minimum(1.0, self._get_mh_ratio(c))
+                accept = self._random_states[c].uniform() < prob
+            if accept:
+                if n >= self.burn_in:
+                    self._n_acc[c] += 1
+            else:
+                self._copy_previous(n, c)
         self.state['n_samples'] += 1
 
-    def _copy_previous(self, n):
-        for key in ('logprior', 'params', 'logposterior'):
-            self.state[key][n] = self.state[key][n - 1]
+    def _copy_previous(self, n, chains):
+        for arr in (self._logprior, self._params, self._logpost):
+            arr[chains, n] = arr[chains, n - 1]
 
     def _init_round(self):
-        """Propose the next parameter; proposals outside the prior support are rejected without
-        simulating, and each one shortens the remaining objective by one round."""
-        while self.state['n_samples'] < len(self.state['params']):
+        """Propose the next parameter of every chain.  A chain whose proposal is outside the prior
+        support keeps its state for this iteration and simulates its rows at it; when every
+        chain's proposal is outside, nothing is simulated and the remaining objective shortens by
+        one round."""
+        if self.device_proposal is not None:
+            self.state['n_sim_round'] = 0          # ops.bsl_mh_step wrote the next parameters
+            return
+        while self.state['n_samples'] < self._params.shape[1]:
             n = self.state['n_samples']
-            prop = self._propagate_state()
-            logprior = np.reshape(self.prior.logpdf(prop), -1)[0]
-            if np.isfinite(logprior):
-                self.state['logprior'][n] = logprior
-                self.state['params'][n] = prop
+            props = np.vstack([self._propagate_state(c) for c in range(self.n_chains)])
+            logprior = np.reshape(self.prior.logpdf(props), -1)
+            live = np.isfinite(logprior)
+            self._live = live
+            self._copy_previous(n, ~live)
+            self._params[live, n] = props[live]
+            self._logprior[live, n] = logprior[live]
+            if live.any():
                 self.state['n_sim_round'] = 0
                 break
-            self._copy_previous(n)
             self.state['n_samples'] += 1
             self.set_objective(self.objective['round'] - 1)
 
-    def _propagate_state(self):
-        mean = self.state['params'][self.state['n_samples'] - 1]
+    def _propagate_state(self, c):
+        mean = self._params[c, self.state['n_samples'] - 1]
+        random_state = self._random_states[c]
         bound = self.logit_transform_bound
         if bound is None:
-            prop = self.random_state.multivariate_normal(mean, self.sigma_proposals)
-        else:
-            prop = self._para_logit_back_transform(self.random_state.multivariate_normal(
-                self._para_logit_transform(mean, bound), self.sigma_proposals), bound)
-        return np.atleast_2d(prop)
+            return random_state.multivariate_normal(mean, self.sigma_proposals)
+        return self._para_logit_back_transform(random_state.multivariate_normal(
+            self._para_logit_transform(mean, bound), self.sigma_proposals), bound)
 
-    def _get_mh_ratio(self):
+    def _get_mh_ratio(self, c):
         n = self.state['n_samples']
-        log_ratio = self.state['logposterior'][n] - self.state['logposterior'][n - 1]
+        params, logpost = self._params[c], self._logpost[c]
+        log_ratio = logpost[n] - logpost[n - 1]
         jac = 0
         if self.logit_transform_bound is not None:
             # the Jacobian terms are evaluated at the parameters themselves, as in the reference
-            jac = self._jacobian_logit_transform(self.state['params'][n], self.logit_transform_bound) \
-                - self._jacobian_logit_transform(self.state['params'][n - 1],
-                                                 self.logit_transform_bound)
+            jac = self._jacobian_logit_transform(params[n], self.logit_transform_bound) \
+                - self._jacobian_logit_transform(params[n - 1], self.logit_transform_bound)
         res = jac + log_ratio
         return np.exp(min(700, max(-700, res)))
 
@@ -337,13 +456,37 @@ class BSL(ModelBased):
         return np.sum(logj)
 
     def extract_result(self):
-        samples_all = {p: np.array(self.state['params'][:, i])
-                       for i, p in enumerate(self.parameter_names)}
-        acc_rate = self.num_accepted / (self.state['n_samples'] - self.burn_in)
-        logger.info('MCMC acceptance rate: {}'.format(acc_rate))
-        return BslSample(method_name='BSL', samples_all=samples_all, acc_rate=acc_rate,
-                         burn_in=self.burn_in, n_sim=self.state['n_sim'],
-                         parameter_names=self.parameter_names)
+        if self.device_proposal is not None:
+            # the one read of the device chains, at the end of the run
+            self._params[:] = dev.to_host(self._chains_dev)
+            self._logpost[:] = dev.to_host(self._logpost_dev)
+            self._n_acc[:] = dev.to_host(self._n_acc_dev)
+            self.state.pop('logprior', None)
+        n_kept = self.state['n_samples'] - self.burn_in
+        if self.n_chains == 1:
+            self.num_accepted = int(self._n_acc[0])
+            samples_all = {p: np.array(self._params[0, :, i])
+                           for i, p in enumerate(self.parameter_names)}
+            acc_rate = self.num_accepted / n_kept
+            logger.info('MCMC acceptance rate: {}'.format(acc_rate))
+            return BslSample(method_name='BSL', samples_all=samples_all, acc_rate=acc_rate,
+                             burn_in=self.burn_in, n_sim=self.state['n_sim'],
+                             parameter_names=self.parameter_names)
+        chains = np.array(self._params)
+        self.num_accepted = int(self._n_acc.sum())
+        acc_rate = self.num_accepted / (self.n_chains * n_kept)
+        logger.info('MCMC acceptance rate: {} ({} chains)'.format(acc_rate, self.n_chains))
+        logger.info('{} chains of {} iterations acquired. Effective sample size and Rhat for each '
+                    'parameter:'.format(self.n_chains, chains.shape[1]))
+        for i, name in enumerate(self.parameter_names):
+            kept = chains[:, self.burn_in:, i]
+            logger.info('{} {} {}'.format(name, mcmc.eff_sample_size(kept),
+                                          mcmc.gelman_rubin_statistic(kept)))
+        return BslSample(method_name='BSL',
+                         samples_all={p: chains[:, :, i] for i, p in enumerate(self.parameter_names)},
+                         acc_rate=acc_rate, burn_in=self.burn_in, n_sim=self.state['n_sim'],
+                         parameter_names=self.parameter_names, chains=chains,
+                         acc_rates=self._n_acc / n_kept, n_chains=self.n_chains)
 
 
 # ------------------------------------------------------------------------------- pre-sample tools

@@ -150,3 +150,21 @@ def get_device_model(n_obs=100, true_params=None, seed_obs=None):
     names as get_model).  Pass ``device_proposal=DeviceProposal`` to SMC for device proposals."""
     return _graph(em.ElfiModel(), DevicePrior1, DevicePrior2, partial(MA2_device, n_obs=n_obs),
                   _observed(n_obs, true_params, seed_obs))
+
+
+def get_uniform_device_model(n_obs=100, true_params=None, seed_obs=None):
+    """MA2 in throughput mode with stock uniform priors, t1 ~ U(-2, 2) and t2 ~ U(-1, 1) (the box
+    around the reference's triangular prior, which the device prior table does not cover), drawn
+    on the device, and the device simulator and summaries.  Returns (model, DeviceModelPrior);
+    pass the latter as ``device_proposal=`` to SMC or BSL."""
+    from ..priors import DeviceModelPrior
+    m = em.ElfiModel()
+    em.Prior('uniform', -2, 4, model=m, name='t1')
+    em.Prior('uniform', -1, 2, model=m, name='t2')
+    em.Simulator(partial(MA2_device, n_obs=n_obs), m['t1'], m['t2'],
+                 observed=_observed(n_obs, true_params, seed_obs), name='MA2')
+    em.Summary(autocov, m['MA2'], name='S1')
+    em.Summary(autocov, m['MA2'], 2, name='S2')
+    em.Distance('euclidean', m['S1'], m['S2'], name='d')
+    dp = DeviceModelPrior(m)
+    return dp.model, dp

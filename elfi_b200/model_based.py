@@ -6,6 +6,10 @@ for it.  The round's features go into one (n_sim_round, d) float64 device buffer
 the model: lazy device simulations are materialised in place, host outputs uploaded once per batch.
 When the round is full the method's `_process_simulated` runs, then `_init_round` prepares the
 next round.  Runs on this rank only.
+
+A method may run the rounds of `n_chains` chains side by side: each batch then holds batch_size
+rows of every chain, chain c in rows [c batch_size, (c + 1) batch_size), at that chain's
+parameter, and `_sim` is (n_chains, n_sim_round, d) (one chain keeps the (n_sim_round, d) view).
 """
 import numpy as np
 import torch
@@ -67,6 +71,8 @@ class ModelBased(ParameterInference):
             if node not in model.nodes:
                 raise ValueError('Node {} not found in the model'.format(node))
         self.feature_names = feature_names
+        self.n_chains = 1
+        self._rows_per_chain = batch_size      # the context's batch size is n_chains times this
         super().__init__(model, model.parameter_names + feature_names, batch_size=batch_size,
                          seed=seed, pool=pool, distributed=False)
         self.observed = observed_row(self.model, feature_names)
@@ -74,7 +80,7 @@ class ModelBased(ParameterInference):
         if not 1 <= d <= self.D_MAX:
             raise ValueError('{} takes 1 to {} features, got {}'.format(
                 type(self).__name__, self.D_MAX, d))
-        self._sim = None                  # (n_sim_round, d) device features of the round
+        self._sim = None                  # (n_sim_round, d) or (n_chains, n_sim_round, d) features
         self.state['round'] = 0
         self.state['n_sim_round'] = 0
 
@@ -86,7 +92,7 @@ class ModelBased(ParameterInference):
 
     def set_objective(self, rounds):
         self.objective['round'] = rounds
-        self.objective['n_batches'] = rounds * (self.n_sim_round // self.batch_size)
+        self.objective['n_batches'] = rounds * (self.n_sim_round // self._rows_per_chain)
 
     def infer(self, *args, **kwargs):
         if self.state['round'] > 0:
@@ -98,7 +104,7 @@ class ModelBased(ParameterInference):
         raise NotImplementedError
 
     def prepare_new_batch(self, batch_index):
-        params = np.repeat(np.atleast_2d(self.current_params), self.batch_size, axis=0)
+        params = np.repeat(np.atleast_2d(self.current_params), self._rows_per_chain, axis=0)
         return {p: params[:, i] for i, p in enumerate(self.parameter_names)}
 
     def update(self, batch, batch_index):
@@ -117,18 +123,21 @@ class ModelBased(ParameterInference):
         raise NotImplementedError
 
     def _merge_batch(self, batch):
+        C, b, d = self.n_chains, self._rows_per_chain, self.observed.size
         if self._sim is None:
-            self._sim = dev.empty((self.n_sim_round, self.observed.size))
+            sim = dev.empty((C, self.n_sim_round, d))
+            self._sim = sim[0] if C == 1 else sim
+        rounds = self._sim if self._sim.dim() == 3 else self._sim[None]
         row = self.state['n_sim_round']
         col = 0
         for block in feature_columns(batch, self.feature_names, self.batch_size):
             w = int(block.shape[1])
-            if col + w > self._sim.shape[1]:
-                raise ValueError('The features are wider than their observed values ({})'.format(
-                    self._sim.shape[1]))
-            self._sim[row:row + self.batch_size, col:col + w] = block
+            if col + w > d:
+                raise ValueError('The features are wider than their observed values ({})'.format(d))
+            # chain c's rows of the batch go to its own round
+            rounds[:, row:row + b, col:col + w] = block.reshape(C, b, w)
             col += w
-        if col != self._sim.shape[1]:
+        if col != d:
             raise ValueError('The features have {} columns, their observed values {}'.format(
-                col, self._sim.shape[1]))
-        self.state['n_sim_round'] += self.batch_size
+                col, d))
+        self.state['n_sim_round'] += b

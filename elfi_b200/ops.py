@@ -1693,6 +1693,65 @@ def synlik(S, y, estimator='standard', penalties=None, whitening=None):
     return out
 
 
+BSL_MAX_CHAINS = 1 << 22
+
+
+def bsl_mh_tables(specs, sigma_proposals, sources=None, bounds=None):
+    """The host constants of :func:`bsl_mh_step`, checked once per run: the (p, 7) prior table
+    (``specs`` (p, 5) and ``sources`` (p, 2) as in :func:`prior_logpdf`), the lower Cholesky
+    factor of the (p, p) proposal covariance, and the (p, 2) logit bounds or None."""
+    specs = np.atleast_2d(np.asarray(specs, dtype=np.float64))
+    p = specs.shape[0]
+    table = _prior_table(specs, -np.ones((p, 2)) if sources is None else sources)
+    cov = np.atleast_2d(np.asarray(sigma_proposals, dtype=np.float64))
+    if cov.shape != (p, p):
+        raise ValueError('sigma_proposals must be a ({0}, {0}) covariance, got shape {1}'.format(
+            p, cov.shape))
+    try:
+        L = np.ascontiguousarray(np.linalg.cholesky(cov))
+    except np.linalg.LinAlgError:
+        raise ValueError('sigma_proposals is not positive definite') from None
+    bnd = None
+    if bounds is not None:
+        bnd = np.ascontiguousarray(np.asarray(bounds, dtype=np.float64))
+        if bnd.shape != (p, 2) or np.isnan(bnd).any():
+            raise ValueError('logit_transform_bound must be ({}, 2) lower and upper bounds, got '
+                             '{}'.format(p, bounds))
+    return table, L, bnd
+
+
+def bsl_mh_step(tables, t, loglik, prop, prop_lp, chains, logpost, n_acc, rows, seed, burn_in=0):
+    """Iteration t of C lock-step BSL chains on the device (include/elfi_b200.h states the step
+    and its Philox stream): the decision of every chain from the round's log-likelihoods
+    ``loglik`` (C,) and the pending proposals ``prop`` (C, p) with their log priors ``prop_lp``
+    (C,), written to row t of ``chains`` (C, n_samples, p) and ``logpost`` (C, n_samples) and
+    counted in ``n_acc`` (C,) int64 from ``burn_in``; then, unless t is the last iteration, the
+    proposals of iteration t + 1 into ``prop`` / ``prop_lp`` and the next batch's parameters into
+    ``rows`` (p, C b), chain c's block in columns [c b, (c + 1) b).  ``tables`` is
+    :func:`bsl_mh_tables`.  Asynchronous; nothing is read back."""
+    table, L, bnd = tables
+    C, n_samples, p = (int(v) for v in chains.shape)
+    if not 1 <= C <= BSL_MAX_CHAINS:
+        raise ValueError('1 <= C <= 2^22 chains, got {}'.format(C))
+    if p != L.shape[0] or rows.dim() != 2 or rows.shape[0] != p or rows.shape[1] % C \
+            or rows.stride(1) != 1:
+        raise ValueError('rows must be a ({}, C b) array with contiguous columns'.format(p))
+    for name, x, shape, dtype in (('loglik', loglik, (C,), torch.float64),
+                                  ('prop', prop, (C, p), torch.float64),
+                                  ('prop_lp', prop_lp, (C,), torch.float64),
+                                  ('chains', chains, (C, n_samples, p), torch.float64),
+                                  ('logpost', logpost, (C, n_samples), torch.float64),
+                                  ('n_acc', n_acc, (C,), torch.int64)):
+        if not dev.is_device_array(x) or tuple(x.shape) != shape or x.dtype != dtype \
+                or not x.is_contiguous():
+            raise ValueError('{} must be a contiguous {} device array of shape {}'.format(
+                name, dtype, shape))
+    _lib.call('elfi_b200_bsl_mh_step_f64', dev.context(), C, p, int(t), n_samples, int(burn_in),
+              int(rows.shape[1]) // C, int(seed), dev.ptr(table), dev.ptr(L), dev.ptr(bnd),
+              dev.ptr(loglik), dev.ptr(prop), dev.ptr(prop_lp), dev.ptr(chains), dev.ptr(logpost),
+              dev.ptr(n_acc), dev.ptr(rows), rows.stride(0), dev.stream_ptr())
+
+
 # ---- BOLFIRE ratio-estimation classifier (elfi/methods/classifier.py) ------------------------------
 LOGREG_D_MAX = 160             # H = X~^T D X~ (packed) and the row tiles in one CTA's shared memory
 LOGREG_PENALTIES = {'l1': 0, 'l2': 1}

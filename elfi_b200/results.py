@@ -186,17 +186,29 @@ class BOLFIRESample(BolfiSample):
 
 class BslSample(Sample):
     """Metropolis-Hastings chain of BSL.sample (elfi/methods/results.py BslSample): `samples_all`
-    holds every iteration per parameter, burn-in included; `samples` those after `burn_in`."""
+    holds every iteration per parameter, burn-in included; `samples` those after `burn_in`.
+
+    Several chains (`chains` (n_chains, n_samples, p) given): `samples_all[p]` is
+    (n_chains, n_samples), `samples` the post-burn-in draws of all chains concatenated chain by
+    chain, `acc_rate` the pooled acceptance rate and `acc_rates` the per-chain ones."""
 
     def __init__(self, method_name, samples_all, parameter_names, burn_in=0, acc_rate=None,
                  **meta):
-        outputs = {k: samples_all[k][burn_in:] for k in samples_all}
+        if meta.get('chains') is not None:
+            outputs = {k: np.reshape(samples_all[k][:, burn_in:], -1) for k in samples_all}
+        else:
+            outputs = {k: samples_all[k][burn_in:] for k in samples_all}
         super().__init__(method_name=method_name, outputs=outputs, parameter_names=parameter_names,
                          samples_all=samples_all, burn_in=burn_in, acc_rate=acc_rate, **meta)
 
     def compute_ess(self):
-        """Effective sample size of the chain after burn-in, per parameter."""
+        """Effective sample size after burn-in, per parameter (over all chains when there are
+        several)."""
         from .mcmc import eff_sample_size
+        chains = self.meta.get('chains')
+        if chains is not None:
+            return {p: eff_sample_size(chains[:, self.burn_in:, i])
+                    for i, p in enumerate(self.parameter_names)}
         return {p: eff_sample_size(self.samples[p]) for p in self.parameter_names}
 
 

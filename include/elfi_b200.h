@@ -770,6 +770,39 @@ int elfi_b200_synlik_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_row, in
                          int32_t estimator, const double* penalties_host, int64_t K,
                          double* loglik, void* stream);
 
+/* elfi_b200_bsl_mh_step_f64: iteration t of C lock-step BSL Metropolis-Hastings chains in
+ * throughput mode (elfi/methods/inference/bsl.py), for p <= 16 parameters.  Device arrays:
+ * loglik (C) the synthetic log-likelihoods of the round (elfi_b200_synlik_f64 with G = C), prop
+ * (C x p) and prop_lp (C) the pending proposals and their joint prior log densities, chains
+ * (C x n_samples x p), logpost (C x n_samples), n_acc (C, int64), rows (column-major C b x p:
+ * column j at rows + j * ld_rows).  Host: spec_host the 7p-word prior table of
+ * elfi_b200_prior_logpdf_cond_f64, chol_host the (p x p, row-major) lower Cholesky factor L of the
+ * proposal covariance, bounds_host NULL or (p x 2) [lower, upper] per parameter.
+ *   t = 0: chain c takes prop[c] as its state, logpost[c, 0] = loglik[c] + prop_lp[c].
+ *   t >= 1: a proposal with a finite log prior is accepted iff u < min(1, exp(clip(r, -700, 700)))
+ *     with r = (J(prop) - J(state)) + (loglik[c] + prop_lp[c] - logpost[c, t - 1]), where J is the
+ *     log Jacobian of the back transform evaluated at the parameters themselves (the reference's
+ *     rule; 0 without bounds), summed left to right, and clip maps NaN to -700.  Otherwise, or for
+ *     a non-finite prop_lp, row t and logpost[c, t] copy row t - 1.  n_acc[c] += 1 for an
+ *     accepted step (t = 0 included) with t >= burn_in.
+ *   t + 1 < n_samples: the proposal of iteration t + 1 is written to prop[c] and its prior log
+ *     density (conditional sources included) to prop_lp[c]: theta~ = logit(state) per parameter,
+ *     log((x - a) / (b - x)), log(1 / (b - x)), log(x - a) or x by which bounds are finite;
+ *     y_a = theta~_a + sum_{k <= a} L[a, k] z_k accumulated in order of k; the back transform of y.
+ *     Rows [c b, (c + 1) b) of every column get the proposal, or the new state when the proposal's
+ *     log prior is not finite.
+ * Random stream: Philox4x32-10 keyed by seed; u = u01(x, y) of counter (t, c, 0, 0x4253434c), and
+ * z_2k, z_2k+1 the two Box-Muller normals of counter (t + 1, c, 1 + k, 0x4253434c), so that no
+ * value depends on C or on the other chains.  Limits: 1 <= C <= 2^22, 1 <= p <= 16, b >= 1,
+ * C b < 2^31, ld_rows >= C b, 0 <= t < n_samples < 2^32.  Asynchronous on `stream`, bit-identical
+ * across calls. */
+int elfi_b200_bsl_mh_step_f64(elfi_b200_ctx* ctx, int64_t C, int64_t p, int64_t t,
+                              int64_t n_samples, int64_t burn_in, int64_t b, uint64_t seed,
+                              const double* spec_host, const double* chol_host,
+                              const double* bounds_host, const double* loglik, double* prop,
+                              double* prop_lp, double* chains, double* logpost, int64_t* n_acc,
+                              double* rows, int64_t ld_rows, void* stream);
+
 /* ---- regression adjustment (elfi/methods/post_processing.py: LinearAdjustment) ------------------
  * The local-linear adjustment of Beaumont et al. (2002) on N rows of q summaries
  * S[i * ldS + j] (ldS >= q), the observed summaries obs (q) and p parameters T[i * ldT + k]
