@@ -1291,6 +1291,73 @@ def lv_summaries(x):
     return S
 
 
+# ---- birth-death-mutation model (elfi/examples/bdm.py) ----------------------------------------
+BDM_N_MAX = 1024              # cluster counts per lane in shared memory as uint16
+BDM_NSUMM = 2                 # T1, T2
+BDM_MAX_EVENTS_LIMIT = 2 ** 32 - 1   # the event index is one 32-bit Philox word
+BDM_BATCH_MAX = 2 ** 31 - 1
+
+
+def _bdm_N(N):
+    if int(N) != N or not 1 <= N <= BDM_N_MAX:
+        raise ValueError('the device BDM model takes an integer 1 <= N <= {}, got {}'.format(
+            BDM_N_MAX, N))
+    return int(N)
+
+
+def sim_bdm(params, N, seed=0, offset=0, max_events=2 ** 24, n=20, want_data=True,
+            want_summaries=True):
+    """Birth-death-mutation simulator on the device: the law of the reference's executable
+    elfi/examples/cpp/bdm.cpp with --mode 1.  params: (batch, 3) columns alpha (birth), delta
+    (death), tau (mutation).  Row i is a pure function of (seed, offset + i).
+
+    Returns (X, S, n_events): X (batch, N) int16 cluster sizes (None unless want_data), S (batch, 2)
+    the summaries T1 and T2 with T2's argument n (None unless want_summaries), bit for bit
+    :func:`bdm_summaries` of X, and n_events (batch,) int64 the events each row ran.  A row with a
+    rate that is negative, NaN or infinite, or with a total rate of 0, gets counts of -1, NaN
+    summaries and n_events = -1; a row still running after max_events events gets counts of -1,
+    NaN summaries and n_events = max_events.  1 <= N <= BDM_N_MAX,
+    1 <= max_events <= BDM_MAX_EVENTS_LIMIT, batch < 2^31."""
+    N = _bdm_N(N)
+    if int(max_events) != max_events or not 1 <= max_events <= BDM_MAX_EVENTS_LIMIT:
+        raise ValueError('max_events must be an integer with 1 <= max_events <= {} (the event '
+                         'index is one Philox word), got {}'.format(BDM_MAX_EVENTS_LIMIT,
+                                                                    max_events))
+    P = _params(params, 'BDM', ('alpha', 'delta', 'tau'))
+    B = P.shape[0]
+    if B > BDM_BATCH_MAX:
+        raise ValueError('the device BDM simulator takes at most {} rows per call, got {}'.format(
+            BDM_BATCH_MAX, B))
+    X = dev.empty((B, N), dtype=torch.int16) if want_data else None
+    S = dev.empty((B, BDM_NSUMM)) if want_summaries else None
+    n_events = dev.empty((B,), dtype=torch.int64)
+    _lib.call('elfi_b200_sim_bdm_f64', dev.context(), dev.ptr(P), _ld(P), B, N, float(n),
+              int(max_events), int(seed), int(offset), dev.ptr(X), N, dev.ptr(S), BDM_NSUMM,
+              dev.ptr(n_events), dev.stream_ptr())
+    return X, S, n_events
+
+
+def bdm_summaries(x, n=20):
+    """T1 and T2 of elfi/examples/bdm.py for device cluster sizes x (batch, N), any strides: a
+    (batch, 2) tensor, bit for bit NumPy's T1(x) and T2(x, n) and :func:`sim_bdm`'s.  int16
+    device data is read in place; anything else is cast to int16 (host data is uploaded first).
+    A row with a negative count (the mark of sim_bdm's invalid and capped rows) gets NaN.
+    1 <= N <= BDM_N_MAX."""
+    if not dev.is_device_array(x):
+        x = dev.to_device(torch.from_numpy(np.ascontiguousarray(x, dtype=np.int16)),
+                          dtype=torch.int16)
+    if x.dtype != torch.int16:
+        x = x.to(torch.int16)
+    if x.dim() == 1:
+        x = x[None, :]
+    _axes(x, 'bdm_summaries', ('batch', 'N'))
+    B, N = int(x.shape[0]), _bdm_N(int(x.shape[1]))
+    S = dev.empty((B, BDM_NSUMM))
+    _lib.call('elfi_b200_bdm_summaries_f64', dev.context(), dev.ptr(x), x.stride(0), x.stride(1),
+              B, N, float(n), dev.ptr(S), BDM_NSUMM, dev.stream_ptr())
+    return S
+
+
 # ---- day care model (elfi/examples/daycare.py) ----------------------------------------------------
 DC_DCC_MAX = 32               # one lane per DCC
 DC_IND_MAX = 64               # the numerators of E_s stay within int64

@@ -1,12 +1,15 @@
 """Graph helpers (mirror of elfi/model/tools.py): ``vectorize`` turns a simulator written for one
-parameter set into one that takes a batch, by calling it once per row.
-
-``external_operation`` (running an outside executable per row) is not provided."""
+parameter set into one that takes a batch, by calling it once per row, and
+``external_operation`` turns a command line (a shell script or an executable) into an operation
+that runs it on a subprocess."""
+import subprocess
 from functools import partial
 
 import numpy as np
 
-__all__ = ['vectorize']
+from .model import get_sub_seed
+
+__all__ = ['vectorize', 'external_operation']
 
 
 def _is_array(x):
@@ -79,3 +82,101 @@ def vectorize(operation, constants=None, dtype=None):
         elfi_b200.Simulator(sim, m['pm'], m['pp'], init_arr, name='sim', observed=obs)
     """
     return partial(run_vectorized, operation, constants=constants, dtype=dtype)
+
+
+def unpack_meta(*inputs, **kwinputs):
+    """Update ``kwinputs`` with the keys and values of its ``meta`` dictionary; keyword inputs
+    given explicitly win over meta keys of the same name."""
+    if 'meta' in kwinputs:
+        new_kwinputs = kwinputs['meta'].copy()
+        new_kwinputs.update(kwinputs)
+        kwinputs = new_kwinputs
+    return inputs, kwinputs
+
+
+def prepare_seed(*inputs, **kwinputs):
+    """Set ``kwinputs['seed']`` from its ``random_state`` (a NumPy RandomState): sub seed
+    ``index_in_batch`` (0 when absent) of the first word of the state, so that every row of a
+    batch gets its own seed."""
+    if 'random_state' in kwinputs:
+        seed = kwinputs['random_state'].get_state()[1][0]
+        kwinputs['seed'] = get_sub_seed(seed, kwinputs.get('index_in_batch') or 0)
+    return inputs, kwinputs
+
+
+def stdout_to_array(stdout, *inputs, sep=' ', dtype=None, **kwinputs):
+    """One row of stdout as a NumPy array (``np.fromstring`` with ``sep``)."""
+    return np.fromstring(stdout, dtype=dtype, sep=sep)
+
+
+def run_external(command, *inputs, process_result=None, prepare_inputs=None, stdout=True,
+                 subprocess_kwargs=None, **kwinputs):
+    """Run ``command`` on a subprocess and return ``process_result`` of what it gave.
+
+    The meta keys are merged into the keyword inputs (:func:`unpack_meta`), a ``seed`` is derived
+    from ``random_state`` (:func:`prepare_seed`), ``prepare_inputs`` may rewrite the inputs, and
+    the command is ``command.format(*inputs, **kwinputs)``.  It runs with
+    ``subprocess.run(shell=True, check=True)`` updated by ``subprocess_kwargs``, so a failing
+    command raises CalledProcessError.  See :func:`external_operation`."""
+    inputs, kwinputs = unpack_meta(*inputs, **kwinputs)
+    inputs, kwinputs = prepare_seed(*inputs, **kwinputs)
+    if prepare_inputs:
+        inputs, kwinputs = prepare_inputs(*inputs, **kwinputs)
+    try:
+        command = command.format(*inputs, **kwinputs)
+    except KeyError as e:
+        raise KeyError('The requested keyword {} was not passed to the external '
+                       'operation: "{}".'.format(str(e), command))
+    kwargs = dict(shell=True, check=True)
+    kwargs.update(subprocess_kwargs or {})
+    completed_process = subprocess.run(command, **kwargs)
+    if stdout:
+        completed_process = completed_process.stdout
+    return process_result(completed_process, *inputs, **kwinputs)
+
+
+def external_operation(command, process_result=None, prepare_inputs=None, sep=' ', stdout=True,
+                       subprocess_kwargs=None):
+    """Wrap an external command (a shell script, an executable) as an operation, e.g. a simulator.
+
+    Parameters
+    ----------
+    command : str
+        The command line, with Python format fields for the inputs, e.g.
+        ``"myscript.sh {0} {batch_size} --seed {seed}"``.  An operation that receives
+        ``random_state`` also gets a ``seed`` keyword (:func:`prepare_seed`), and an operation
+        with ``uses_meta`` the meta keys (``model_name``, ``batch_index``, ``submission_index``,
+        ...).
+    process_result : callable, np.dtype or str, optional
+        ``output = process_result(result, *inputs, **kwinputs)``, where result is the stdout, or
+        the ``subprocess.CompletedProcess`` when ``stdout`` is False.  The default converts
+        stdout with ``np.fromstring(stdout, sep=sep)``; a dtype or its name casts it to that type.
+    prepare_inputs : callable, optional
+        ``inputs, kwinputs = prepare_inputs(*inputs, **kwinputs)``, called before the command is
+        formatted (to write an input file, say).
+    sep : str, optional
+        The separator of the default ``process_result``.
+    stdout : bool, optional
+        Pass ``process_result`` the stdout (True, forced for the default handler) or the
+        ``CompletedProcess``.
+    subprocess_kwargs : dict, optional
+        Options of ``subprocess.run``, over the defaults ``shell=True, check=True``.
+
+    Example::
+
+        op = elfi_b200.tools.external_operation('echo 1 {0}', process_result='int8')
+        sim = elfi_b200.Simulator(op, elfi_b200.Constant(123))
+        sim.generate()      # array([  1, 123], dtype=int8)
+    """
+    if process_result is None or isinstance(process_result, (str, np.dtype)):
+        fromstring_kwargs = dict(sep=sep)
+        if isinstance(process_result, (str, np.dtype)):
+            fromstring_kwargs['dtype'] = str(process_result)
+        process_result = partial(stdout_to_array, **fromstring_kwargs)
+        stdout = True
+    if stdout is True:
+        subprocess_kwargs = dict(subprocess_kwargs or {})
+        subprocess_kwargs['stdout'] = subprocess.PIPE
+    return partial(run_external, command, process_result=process_result,
+                   prepare_inputs=prepare_inputs, stdout=stdout,
+                   subprocess_kwargs=subprocess_kwargs)

@@ -633,6 +633,30 @@ int elfi_b200_lv_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_r
                                int64_t ld_species, int64_t B, int64_t n_obs, double* S,
                                int64_t ldS, void* stream);
 
+/* Birth-death-mutation (BDM) model of elfi/examples/bdm.py, whose reference simulator is the
+ * executable elfi/examples/cpp/bdm.cpp with --mode 1 (throughput mode, statistical parity); law,
+ * stream layout, lane layout and arithmetic in elfi_b200/csrc/bdm.cu and bdm.cuh.
+ * sim_bdm: row i has rates (alpha, delta, tau) = P[i * ldP + 0..2] (ldP >= 3) and population bound
+ *   N (1 <= N <= 1024, B < 2^31).  X[i * ldX + j] (int16, ldX >= N) is the size of cluster j when
+ *   the population first exceeds N (that birth undone) or dies out; S[i * ldS + 0..1] (ldS >= 2)
+ *   are T1 = count(c > 0) / sum(c) (NaN for an extinct row) and T2 = 1 - sum_j (c_j / n_t2)^2 in
+ *   NumPy's pairwise order; either of X and S may be NULL.  n_events[i] (int64) is the number of
+ *   events row i ran.  Event k draws Philox block k of (seed, offset + i): a pure function of the
+ *   row, whatever the launch.  A rate that is negative, NaN or infinite, or a total rate of 0 or
+ *   +inf, gives counts of -1, NaN summaries and n_events = -1; a row still running after
+ *   max_events (1 .. 2^32 - 1) events gives counts of -1, NaN summaries and n_events =
+ *   max_events.  The kernel is persistent: its lanes take new rows as theirs finish.
+ * bdm_summaries: S[i * ldS + 0..1] = T1, T2 (with n) of the row X[i * ld_row + j * ld_col]
+ *   (int16, 1 <= N <= 1024), bit for bit NumPy's and sim_bdm's; a row with a negative count gets
+ *   NaN summaries. */
+int elfi_b200_sim_bdm_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B, int64_t N,
+                          double n_t2, int64_t max_events, uint64_t seed, uint64_t offset,
+                          int16_t* X, int64_t ldX, double* S, int64_t ldS, int64_t* n_events,
+                          void* stream);
+int elfi_b200_bdm_summaries_f64(elfi_b200_ctx* ctx, const int16_t* X, int64_t ld_row,
+                                int64_t ld_col, int64_t B, int64_t N, double n, double* S,
+                                int64_t ldS, void* stream);
+
 /* Day care model of elfi/examples/daycare.py (throughput mode, statistical parity); law, stream
  * layout, lane layout and arithmetic in elfi_b200/csrc/daycare.cu and daycare.cuh.
  * sim_daycare: row i has parameters (t1, t2, t3) = P[i * ldP + 0..2] (ldP >= 3); each of its n_dcc
