@@ -117,6 +117,8 @@ SIGNATURES = {
                                c_ptr, c_i64, c_ptr],
     'elfi_b200_arch_summaries_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr, c_i64,
                                      c_ptr],
+    'elfi_b200_sim_ar1_f64': [c_ptr, c_ptr, c_i64, c_i64, c_u64, c_u64, c_ptr, c_i64, c_ptr, c_ptr,
+                              c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
     'elfi_b200_prior_rvs_f64': [c_ptr, c_ptr, c_i64, c_u64, c_u64, c_ptr, c_ptr],
     'elfi_b200_prior_logpdf_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     'elfi_b200_prior_rvs_cond_f64': [c_ptr, c_ptr, c_i64, c_u64, c_u64, c_ptr, c_ptr, c_ptr, c_ptr],

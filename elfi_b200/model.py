@@ -27,6 +27,7 @@ import scipy.stats as ss
 
 from . import device as dev
 from . import ops
+from .throughput import LazySimulation
 
 # ---- node flags -----------------------------------------------------------------------------
 STOCHASTIC = 1        # consumes the batch RandomState
@@ -723,10 +724,12 @@ class Discrepancy(NodeReference):
 
 def _stack_summaries(summaries):
     """np.column_stack(summaries) of elfi/model/utils.py:39 as a device matrix.
-    A single 2-d parent is used in place (no copy)."""
+    A single 2-d parent is used in place (no copy); lazy simulator output is materialised."""
     import torch
     cols = []
     for s in summaries:
+        if isinstance(s, LazySimulation):
+            s = s.materialize()
         t = s if dev.is_device_array(s) else dev.to_device(np.asarray(s, dtype=np.float64))
         if t.dim() > 2:
             raise ValueError('Incompatible data shape for the distance node. Please check '
@@ -792,7 +795,15 @@ def _device_constant(arr):
 
 
 def device_euclidean_discrepancy(*summaries, observed, w=None, accept=None):
-    """distance_as_discrepancy (elfi/model/utils.py:37-52) for the Euclidean family, on device."""
+    """distance_as_discrepancy (elfi/model/utils.py:37-52) for the Euclidean family, on device.
+    The unweighted distance of lazy simulator output that offers a fused one is computed in the
+    simulator kernel, without writing the data."""
+    if w is None and len(summaries) == 1 and isinstance(summaries[0], LazySimulation) and \
+            summaries[0].euclidean is not None:
+        if _stack_observed(observed).shape[0] != 1:
+            raise ValueError('observed summaries must form a single row')
+        d, idx = summaries[0].euclidean(_observed_on_device(observed), accept)
+        return AcceptedOutput(d, idx) if accept is not None else d
     X = _stack_summaries(summaries)
     if _stack_observed(observed).shape[0] != 1:
         raise ValueError('observed summaries must form a single row')

@@ -68,17 +68,18 @@ def _mask(x, name, layout):
     return _axes(x, name, layout)
 
 
-def _dist_prepare(S, obs, thresholds, K=1, want_indices=True, device_thresholds=False):
-    """What the device distance wrappers share: the matrix, ``obs`` flattened and checked against
-    its width, the K thresholds as a host float64 array (or None) -- or left as a device tensor
-    where the entry point reads them there (``device_thresholds``) -- and the outputs d (B, K),
-    acc_idx and n_acc (both None without thresholds)."""
-    S = _matrix(S)
-    B, D = S.shape
+def _dist_obs(obs, D):
+    """The observed row of a distance as a flat (D,) device vector."""
     obs_t = dev.to_device(obs).reshape(-1)
     if obs_t.numel() != D:
         raise ValueError('XA and XB must have the same number of columns '
                          '(i.e. feature dimension.)')
+    return obs_t
+
+
+def _dist_thresholds(thresholds, K, device_thresholds):
+    """The K thresholds of a distance as a host float64 array (or None), or left as a contiguous
+    float64 device tensor where the entry point reads them there (``device_thresholds``)."""
     thr = None
     if device_thresholds and dev.is_device_array(thresholds):
         thr = thresholds.reshape(-1)
@@ -89,6 +90,18 @@ def _dist_prepare(S, obs, thresholds, K=1, want_indices=True, device_thresholds=
     if thr is not None and thr.shape[0] != K:
         raise ValueError('need one threshold per distance column ({} != {})'.format(
             thr.shape[0], K))
+    return thr
+
+
+def _dist_prepare(S, obs, thresholds, K=1, want_indices=True, device_thresholds=False):
+    """What the device distance wrappers share: the matrix, ``obs`` flattened and checked against
+    its width, the K thresholds as a host float64 array (or None) -- or left as a device tensor
+    where the entry point reads them there (``device_thresholds``) -- and the outputs d (B, K),
+    acc_idx and n_acc (both None without thresholds)."""
+    S = _matrix(S)
+    B, D = S.shape
+    obs_t = _dist_obs(obs, D)
+    thr = _dist_thresholds(thresholds, K, device_thresholds)
     d = dev.empty((B, K))
     acc_idx = n_acc = None
     if thr is not None:
@@ -1525,6 +1538,58 @@ def arch_summaries(y, n_lags=5):
     _lib.call('elfi_b200_arch_summaries_f64', dev.context(), dev.ptr(y), y.stride(0), y.stride(1),
               B, n, n_lags, dev.ptr(S), K, dev.stream_ptr())
     return S
+
+
+# ---- AR(1) model (elfi/examples/ar1.py) -----------------------------------------------------------
+AR1_NOBS_MAX = 1 << 24        # observations per row
+AR1_BATCH_MAX = 2 ** 31 - 1   # accepted rows are int32 indices
+
+
+def sim_ar1(phi, n_obs=200, seed=0, offset=0, obs=None, thresholds=None, want_data=None):
+    """AR(1) simulator on the device (elfi/examples/ar1.py:11-38): x_t = phi x_{t-1} + w_t, x_0 = 0,
+    with the Euclidean distance to an observed series fused.  phi: (batch,) or (batch, 1).  Row i
+    is a pure function of (seed, offset + i).
+
+    obs : None or the observed series, n_obs values
+    thresholds : None, or one threshold (a float, a host array or a device tensor): needs obs
+    want_data : write the series; None writes it only when no obs is given
+
+    Returns (X, d, idx): X (batch, n_obs) the series x_1 .. x_n (None unless want_data), d (batch,)
+    the distance of each series to obs (None without obs), bit for bit :func:`dist_euclid` of X,
+    and idx the ascending indices of the rows with d <= threshold (None without thresholds), as
+    :func:`dist_euclid` returns them.  The distance is computed without writing X.
+    1 <= n_obs <= AR1_NOBS_MAX, batch <= AR1_BATCH_MAX."""
+    if int(n_obs) != n_obs or not 1 <= n_obs <= AR1_NOBS_MAX:
+        raise ValueError('the device AR(1) simulator takes an integer 1 <= n_obs <= {}, got '
+                         '{}'.format(AR1_NOBS_MAX, n_obs))
+    n_obs = int(n_obs)
+    P = _params(phi, 'AR(1)', ('phi',))
+    B = P.shape[0]
+    if B > AR1_BATCH_MAX:
+        raise ValueError('the device AR(1) simulator takes at most {} rows per call, got '
+                         '{}'.format(AR1_BATCH_MAX, B))
+    if thresholds is not None and obs is None:
+        raise ValueError('thresholds need the observed series obs')
+    if want_data is None:
+        want_data = obs is None
+    if not want_data and obs is None:
+        raise ValueError('sim_ar1 asked for neither the data nor a distance')
+    phi_t = P[:, 0].contiguous()
+    obs_t = thr = d = acc_idx = n_acc = None
+    if obs is not None:
+        obs_t = _dist_obs(obs, n_obs)
+        thr = _dist_thresholds(thresholds, 1, device_thresholds=True)
+        d = dev.empty((B,))
+        if thr is not None:
+            n_acc = dev.zeros((1,), dtype=torch.int64)
+            acc_idx = dev.empty((max(B, 1),), dtype=torch.int32)
+    thr_on_device = dev.is_device_array(thr)
+    X = dev.empty((B, n_obs)) if want_data else None
+    _lib.call('elfi_b200_sim_ar1_f64', dev.context(), dev.ptr(phi_t), B, n_obs, int(seed),
+              int(offset), dev.ptr(X), n_obs, dev.ptr(obs_t),
+              None if thr_on_device else dev.ptr(thr), dev.ptr(thr) if thr_on_device else None,
+              dev.ptr(d), dev.ptr(acc_idx), dev.ptr(n_acc), dev.stream_ptr())
+    return X, d, _dist_accepted(acc_idx, n_acc)
 
 
 # ---- M/G/1 queue (elfi/examples/mg1.py) ------------------------------------------------------------

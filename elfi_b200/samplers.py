@@ -30,6 +30,7 @@ from . import model as em
 from . import ops
 from . import sharding
 from .results import DeviceOutputs, Sample, SmcSample
+from .throughput import LazySimulation
 
 logger = logging.getLogger(__name__)
 
@@ -444,6 +445,8 @@ def _batch_key(seed, batch_index):
 
 
 def _to_dev_f64(x):
+    if isinstance(x, LazySimulation):     # a simulator output kept in a sample: its data
+        return x.materialize()
     return x if dev.is_device_array(x) else dev.to_device(np.asarray(x, dtype=np.float64))
 
 

@@ -25,13 +25,19 @@ def batch_columns(values, batch_size):
 class LazySimulation:
     """Simulator output whose summaries are computed in the simulator kernel, so the data is only
     written when ``materialize()`` is called.  ``summarise(kind)`` runs once per kind: the summary
-    nodes of one simulator get columns of the same tensor, which the distance reads in place."""
+    nodes of one simulator get columns of the same tensor, which the distance reads in place.
 
-    def __init__(self, shape, summarise, materialize):
+    ``euclidean``, when given, is the Euclidean distance of the data to an observed row computed in
+    the simulator kernel: ``euclidean(obs, thresholds) -> (d, idx)`` with the contract of
+    ``ops.dist_euclid(materialize(), obs, thresholds=thresholds)``.  A Euclidean ``Distance`` whose
+    single parent is this output uses it; any other consumer of the data materialises it."""
+
+    def __init__(self, shape, summarise, materialize, euclidean=None):
         self.shape = tuple(shape)
         self.ndim = len(self.shape)
         self._summarise = summarise
         self.materialize = materialize
+        self.euclidean = euclidean
         self._summaries = {}
 
     def __len__(self):

@@ -707,6 +707,24 @@ int elfi_b200_arch_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld
                                  int64_t B, int64_t n, int64_t n_lags, double* S, int64_t ldS,
                                  void* stream);
 
+/* AR(1) model of elfi/examples/ar1.py (throughput mode, statistical parity) with the Euclidean
+ * distance to an observed series fused; stream layout, thread layout and arithmetic in
+ * elfi_b200/csrc/ar1.cu and ar1.cuh.  Row i has parameter phi[i] and series
+ * x_t = phi x_{t-1} + w_t (x_0 = 0), X[i * ldX + t - 1] for t = 1 .. n_obs (ldX >= n_obs; X may be
+ * NULL).  Block m of (seed, offset + i) gives the innovations w_{2m+1}, w_{2m+2}: a pure function
+ * of the row, whatever the launch.  0 <= B <= 2^31 - 1, 1 <= n_obs <= 2^24.
+ * With obs (n_obs doubles) the row's distance d_out[i] = sqrt(sum_t (x_t - obs_t)^2), t ascending,
+ * one rounding per operation: bit for bit elfi_b200_dist_euclid_thr_f64 of the written series
+ * (K = 1, no weights), computed without writing X.  With a threshold (one double, thr_host on the
+ * host or thr_dev on the device, not both) rows with d <= threshold are accepted; acc_idx
+ * (B int32, may be NULL) gets their indices ascending and n_acc (one int64 on the device, may be
+ * NULL) their number, the contract of the distance entry points above.  Without obs, d_out,
+ * thresholds, acc_idx and n_acc must be NULL. */
+int elfi_b200_sim_ar1_f64(elfi_b200_ctx* ctx, const double* phi, int64_t B, int64_t n_obs,
+                          uint64_t seed, uint64_t offset, double* X, int64_t ldX,
+                          const double* obs, const double* thr_host, const double* thr_dev,
+                          double* d_out, int32_t* acc_idx, int64_t* n_acc, void* stream);
+
 /* M/G/1 queue of elfi/examples/mg1.py (throughput mode, statistical parity); stream layout, thread
  * layout and arithmetic in elfi_b200/csrc/mg1.cu and mg1.cuh.  Rows where the reference's NumPy
  * raises (1/t3 with its sign bit set, t2 - t1 not finite) give NaN data and NaN quantiles.
