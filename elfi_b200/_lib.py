@@ -38,6 +38,11 @@ SIGNATURES = {
                                           c_ptr, c_ptr, c_ptr, c_ptr],
     'elfi_b200_topn_merge_f64': [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_i64, c_ptr, c_i64, c_i64, c_i64,
                                  c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
+    'elfi_b200_topn_merge_seg_f64': [c_ptr, c_i64, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64, c_i64,
+                                     c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
+                                     c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
+    'elfi_b200_dist_seg_f64': [c_ptr, ctypes.c_int32, c_dbl, c_ptr, c_i64, c_i64, c_i64, c_i64,
+                               c_ptr, c_i64, c_ptr, c_ptr],
     'elfi_b200_summary_autocov_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr, c_i64,
                                       c_ptr],
     'elfi_b200_summary_meanvar_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64,

@@ -629,6 +629,109 @@ static int launch_metric(elfi_b200_ctx* ctx, int metric, const double* S, int64_
     }
 }
 
+// ---- segmented distances (Testbench: R repetitions of a rejection batch in one launch) -----------
+// Rows [r B, (r + 1) B) of S are measured against observed row r.  The per-row arithmetic is that
+// of MetricConsumer / metric_direct_kernel (for 'euclidean': EuclidConsumer / dist_direct_kernel),
+// so every segment is bit-identical to the one-observation entry points on that segment.  A tile
+// of 32 rows may straddle two segments: each lane looks its observed row up from its own row.
+struct SegParams : DistParams {
+    double pexp;
+    int64_t seg_rows;   // B
+    int64_t R;
+    int64_t ld_obs;
+};
+
+__device__ __forceinline__ int64_t seg_of(const SegParams& p, int64_t row) {
+    const int64_t r = row / p.seg_rows;
+    return r < p.R ? r : p.R - 1;   // rows past the end (zero-filled tile) read the last row
+}
+
+// Shared consumer area: the R observed rows, each padded to Dp doubles with zeros.
+template <int METRIC>
+struct SegConsumer {
+    typedef SegParams Params;
+    static constexpr int PASSES = 1;
+    static constexpr bool RS_TILE_INFO = true;
+    const Params& p;
+    const double* obs_s;
+    const double* my_obs;
+    int Dp;
+    double acc;
+
+    static __device__ void setup_shared(uint8_t* aux, const Params& p, int D) {
+        const int Dp = rs_padded_cols(D);
+        double* obs_s = reinterpret_cast<double*>(aux);
+        for (int64_t t = threadIdx.x; t < p.R * Dp; t += blockDim.x) {
+            const int64_t r = t / Dp;
+            const int j = int(t - r * Dp);
+            obs_s[t] = j < D ? p.obs[r * p.ld_obs + j] : 0.0;
+        }
+    }
+    __device__ SegConsumer(const Params& p_, const uint8_t* aux, int D, int)
+        : p(p_), obs_s(reinterpret_cast<const double*>(aux)), my_obs(obs_s), acc(0.0) {
+        Dp = rs_padded_cols(D);
+    }
+    __device__ __forceinline__ void begin_row() { acc = 0.0; }
+    __device__ __forceinline__ void set_tile(int64_t row0, int64_t) {
+        my_obs = obs_s + seg_of(p, row0 + (threadIdx.x & 31)) * Dp;
+    }
+    __device__ __forceinline__ void consume(int, int cg, const uint8_t* box_row, int sw) {
+        const double2* o = reinterpret_cast<const double2*>(my_obs + cg * RS_BOX_COLS);
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            const double2 v = *reinterpret_cast<const double2*>(box_row + ((c ^ sw) << 4));
+            const double2 ob = o[c];
+            acc = metric_term<METRIC>(acc, __dsub_rn(v.x, ob.x), p.pexp);
+            acc = metric_term<METRIC>(acc, __dsub_rn(v.y, ob.y), p.pexp);
+        }
+    }
+    __device__ __forceinline__ void end_row(int64_t row, int64_t B, int lane) {
+        dist_record<true, 1>(p, 1, row, B, lane,
+                             [&](int) { return metric_value<METRIC>(acc, p.pexp); });
+    }
+};
+
+template <int METRIC>
+__global__ void __launch_bounds__(256)
+seg_direct_kernel(const double* __restrict__ S, int64_t ld, int64_t n, int D, SegParams p) {
+    const int64_t row = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    dist_record<false, 1>(p, 1, row, n, threadIdx.x & 31, [&](int) {
+        const double* r = S + row * ld;
+        const double* ob = p.obs + seg_of(p, row) * p.ld_obs;
+        double acc = 0.0;
+        for (int j = 0; j < D; ++j)
+            acc = metric_term<METRIC>(acc, __dsub_rn(__ldg(r + j), __ldg(ob + j)), p.pexp);
+        return metric_value<METRIC>(acc, p.pexp);
+    });
+}
+
+template <int METRIC>
+static int launch_seg_t(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t n, int64_t D,
+                        const SegParams& p, cudaStream_t stream) {
+    const size_t aux = size_t(rs_padded_cols(D)) * 8 * size_t(p.R);
+    if (rs_streams(ctx, S, ldS, D, aux))
+        return rowstream_launch<SegConsumer<METRIC>>(ctx, S, ldS, n, D, aux, p, stream);
+    seg_direct_kernel<METRIC><<<unsigned((n + 255) / 256), 256, 0, stream>>>(S, ldS, n, int(D), p);
+    ELFI_CUDA_OK(cudaGetLastError());
+    return ELFI_B200_OK;
+}
+
+static int launch_seg(elfi_b200_ctx* ctx, int metric, const double* S, int64_t ldS, int64_t n,
+                      int64_t D, const SegParams& p, cudaStream_t stream) {
+    switch (metric) {
+        case ELFI_B200_METRIC_EUCLIDEAN:
+            return launch_seg_t<ELFI_B200_METRIC_EUCLIDEAN>(ctx, S, ldS, n, D, p, stream);
+        case ELFI_B200_METRIC_SQEUCLIDEAN:
+            return launch_seg_t<ELFI_B200_METRIC_SQEUCLIDEAN>(ctx, S, ldS, n, D, p, stream);
+        case ELFI_B200_METRIC_CITYBLOCK:
+            return launch_seg_t<ELFI_B200_METRIC_CITYBLOCK>(ctx, S, ldS, n, D, p, stream);
+        case ELFI_B200_METRIC_CHEBYSHEV:
+            return launch_seg_t<ELFI_B200_METRIC_CHEBYSHEV>(ctx, S, ldS, n, D, p, stream);
+        default:
+            return launch_seg_t<ELFI_B200_METRIC_MINKOWSKI>(ctx, S, ldS, n, D, p, stream);
+    }
+}
+
 static int check_dist_args(const void* S, int64_t ldS, int64_t B, int64_t D, const void* obs,
                            const void* W, int64_t K, const void* thr, const void* acc_idx) {
     ELFI_REQUIRE(B >= 0 && D >= 1, "dist: bad shape B=%lld D=%lld", (long long)B, (long long)D);
@@ -864,6 +967,32 @@ int elfi_b200_dist_seuclidean_thr_f64(elfi_b200_ctx* ctx, const double* S, int64
                          return launch_metric(ctx, METRIC_SEUCLIDEAN, S, ldS, B, D,
                                               MetricParams{p, 0.0, V}, stream);
                      });
+}
+
+int elfi_b200_dist_seg_f64(elfi_b200_ctx* ctx, int32_t metric, double pexp, const double* S,
+                           int64_t ldS, int64_t R, int64_t B, int64_t D, const double* obs,
+                           int64_t ld_obs, double* d_out, void* stream_) {
+    using namespace elfi;
+    ELFI_REQUIRE(ctx != nullptr, "dist_seg: ctx is NULL");
+    ELFI_REQUIRE(metric >= ELFI_B200_METRIC_EUCLIDEAN && metric <= ELFI_B200_METRIC_MINKOWSKI,
+                 "dist_seg: unknown metric code %d", int(metric));
+    ELFI_REQUIRE(metric != ELFI_B200_METRIC_MINKOWSKI || (pexp > 0.0 && pexp < 1e308),
+                 "dist_seg: Minkowski exponent must be positive and finite");
+    ELFI_REQUIRE(R >= 1 && B >= 0 && D >= 1 && ldS >= D && ld_obs >= D,
+                 "dist_seg: bad shape R=%lld B=%lld D=%lld ldS=%lld ld_obs=%lld", (long long)R,
+                 (long long)B, (long long)D, (long long)ldS, (long long)ld_obs);
+    ELFI_REQUIRE(B == 0 || R <= ((int64_t(1) << 31) - 1) / B, "dist_seg: R * B must fit int32");
+    if (B == 0) return ELFI_B200_OK;
+    ELFI_REQUIRE(S != nullptr && obs != nullptr && d_out != nullptr, "dist_seg: NULL argument");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
+    SegParams p;
+    static_cast<DistParams&>(p) = dist_params(obs, nullptr, 1, nullptr, nullptr, d_out, nullptr);
+    p.pexp = pexp;
+    p.seg_rows = B;
+    p.R = R;
+    p.ld_obs = ld_obs;
+    return launch_seg(ctx, int(metric), S, ldS, R * B, D, p, stream);
 }
 
 }  // extern "C"

@@ -305,6 +305,61 @@ merge_keys_kernel(const double* __restrict__ keysA, int64_t ldA, int64_t nA,
     }
 }
 
+// ---- segmented top-n merge (Testbench: R repetitions' best-n buffers in one call) ----------------
+// Segment r's virtual concatenation [A_r (nA rows); B_r (nB rows)] occupies global positions
+// [r n, (r + 1) n), n = nA + nB.  The 8 key passes sort all R n keys stably; the segment index is
+// then sorted as the most significant digit(s) by further stable passes over the permutation, so
+// within segment r the order is (key, position in [A_r; B_r]) -- exactly the order of
+// elfi_b200_topn_merge_f64 on that segment.
+__global__ void __launch_bounds__(256)
+merge_keys_seg_kernel(const double* __restrict__ keysA, int64_t ldA, int64_t segA, int64_t nA,
+                      const double* __restrict__ keysB, int64_t ldB, int64_t segB, int64_t nB,
+                      int64_t total, double* __restrict__ out) {
+    const int64_t n = nA + nB;
+    const int64_t stride = int64_t(gridDim.x) * blockDim.x;
+    for (int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; t < total; t += stride) {
+        const int64_t r = t / n, i = t - r * n;
+        out[t] = i < nA ? keysA[r * segA + i * ldA] : keysB[r * segB + (i - nA) * ldB];
+    }
+}
+
+// ukeys[t] = segment of the row at sorted position t, and the 8 x 256 digit histograms.
+__global__ void __launch_bounds__(256)
+seg_digits_kernel(const int32_t* __restrict__ vals, int64_t total, int64_t n,
+                  uint64_t* __restrict__ ukeys, uint32_t* __restrict__ ghist) {
+    __shared__ uint32_t h[8 * 256];
+    for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) h[i] = 0;
+    __syncthreads();
+    const int64_t stride = int64_t(gridDim.x) * blockDim.x;
+    for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const uint64_t u = uint64_t(vals[i] / n);
+        ukeys[i] = u;
+#pragma unroll
+        for (int p = 0; p < 8; ++p) atomicAdd(&h[p * 256 + ((u >> (8 * p)) & 255)], 1u);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x)
+        if (h[i]) atomicAdd(&ghist[i], h[i]);
+}
+
+// dst_r[i, 0:width] = row perm[r n + i] - r n of [A_r; B_r], for i < n_keep and every segment r.
+__global__ void __launch_bounds__(256)
+gather2_seg_kernel(const double* __restrict__ A, int64_t ldA, int64_t segA, int64_t nA,
+                   const double* __restrict__ Bm, int64_t ldB, int64_t segB, int64_t n,
+                   const int32_t* __restrict__ perm, int64_t R, int64_t n_keep, int64_t width,
+                   double* __restrict__ dst, int64_t ld_dst, int64_t seg_dst) {
+    const int64_t per = n_keep * width;
+    const int64_t total = R * per;
+    const int64_t stride = int64_t(gridDim.x) * blockDim.x;
+    for (int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; t < total; t += stride) {
+        const int64_t r = t / per, rem = t - r * per;
+        const int64_t i = rem / width, j = rem - i * width;
+        const int64_t q = int64_t(perm[r * n + i]) - r * n;
+        dst[r * seg_dst + i * ld_dst + j] =
+            q < nA ? A[r * segA + q * ldA + j] : Bm[r * segB + (q - nA) * ldB + j];
+    }
+}
+
 // ---- weighted quantile ---------------------------------------------------------------------
 // The reference normalises with np.sum (pairwise order) and accumulates with np.cumsum
 // (strictly sequential); with equal weights and round alphas (e.g. SMC round 0, alpha = 0.5)
@@ -763,6 +818,77 @@ int elfi_b200_topn_merge_f64(elfi_b200_ctx* ctx, const double* keysA, int64_t ld
         gather2_rows_kernel<<<unsigned(gb), 256, 0, stream>>>(A_host[k], ldA_host[k], nA, B_host[k],
                                                               ldB_host[k], mapB, perm, n_keep, width,
                                                               dst_host[k], ld_dst_host[k]);
+    }
+    ELFI_CUDA_OK(cudaGetLastError());
+    return ELFI_B200_OK;
+}
+
+int elfi_b200_topn_merge_seg_f64(elfi_b200_ctx* ctx, int64_t R, const double* keysA,
+                                 int64_t ld_keysA, int64_t seg_keysA, int64_t nA,
+                                 const double* keysB, int64_t ld_keysB, int64_t seg_keysB,
+                                 int64_t nB, int64_t n_keep, int64_t n_out,
+                                 const double* const* A_host, const int64_t* ldA_host,
+                                 const int64_t* segA_host, const double* const* B_host,
+                                 const int64_t* ldB_host, const int64_t* segB_host,
+                                 const int64_t* width_host, double* const* dst_host,
+                                 const int64_t* ld_dst_host, const int64_t* seg_dst_host,
+                                 void* stream_) {
+    using namespace elfi;
+    ELFI_REQUIRE(ctx != nullptr, "topn_merge_seg: ctx is NULL");
+    ELFI_REQUIRE(R >= 1 && nA >= 0 && nB >= 0 && n_keep >= 0 && n_keep <= nA + nB && n_out >= 0,
+                 "topn_merge_seg: bad sizes (R=%lld nA=%lld nB=%lld n_keep=%lld)", (long long)R,
+                 (long long)nA, (long long)nB, (long long)n_keep);
+    const int64_t n = nA + nB;
+    ELFI_REQUIRE(n == 0 || R <= ((int64_t(1) << 31) - 1) / n, "topn_merge_seg: R * (nA + nB) must fit int32");
+    if (n == 0 || n_keep == 0) return ELFI_B200_OK;
+    const int64_t total = R * n;
+    ELFI_REQUIRE((nA == 0 || keysA) && (nB == 0 || keysB), "topn_merge_seg: keys are NULL");
+    ELFI_REQUIRE(n_out == 0 || (A_host && ldA_host && segA_host && B_host && ldB_host && segB_host &&
+                                width_host && dst_host && ld_dst_host && seg_dst_host),
+                 "topn_merge_seg: output descriptors are NULL");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
+    const size_t sort_bytes = sort_scratch_bytes(total);
+    uint8_t* base = static_cast<uint8_t*>(ctx_scratch(ctx, sort_bytes + align256(size_t(total) * 8) + 256));
+    if (!base) return ELFI_B200_ERR_NOMEM;
+    SortScratch s = carve_sort(base, total);
+    double* keys = reinterpret_cast<double*>(base + sort_bytes);
+    int blocks = int((total + 255) / 256);
+    if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
+    merge_keys_seg_kernel<<<blocks, 256, 0, stream>>>(keysA, ld_keysA, seg_keysA, nA, keysB, ld_keysB,
+                                                      seg_keysB, nB, total, keys);
+    int rc = sort_pairs_device(keys, total, s, ctx->sm_count, stream);
+    if (rc) return rc;
+    // key order is in s.k[0] / s.v[0]; now the segment digits (one pass per byte of R - 1)
+    int kc = 1, vc = 0;
+    if (R > 1) {
+        ELFI_CUDA_OK(cudaMemsetAsync(s.ghist, 0, 8 * 256 * 4, stream));
+        int pblocks = int((total + 256 * 8 - 1) / (256 * 8));
+        if (pblocks > ctx->sm_count * 4) pblocks = ctx->sm_count * 4;
+        seg_digits_kernel<<<pblocks, 256, 0, stream>>>(s.v[0], total, n, s.k[1], s.ghist);
+        const unsigned wblocks = unsigned((s.nw + SORT_WARPS - 1) / SORT_WARPS);
+        for (int pass = 0; pass < 8 && (uint64_t(R - 1) >> (8 * pass)) != 0; ++pass) {
+            sort_upsweep_kernel<<<wblocks, SORT_WARPS * 32, 0, stream>>>(s.k[kc], total, pass, s.nw,
+                                                                         s.ghist, s.whist);
+            sort_scan_kernel<<<256, 1024, 0, stream>>>(s.k[kc], total, pass, s.nw, s.ghist, s.whist);
+            sort_scatter_kernel<<<wblocks, SORT_WARPS * 32, 0, stream>>>(
+                s.k[kc], s.v[vc], total, pass, s.nw, s.ghist, s.whist, s.k[kc ^ 1], s.v[vc ^ 1]);
+            kc ^= 1;
+            vc ^= 1;
+        }
+    }
+    const int32_t* perm = s.v[vc];
+    for (int64_t k = 0; k < n_out; ++k) {
+        const int64_t width = width_host[k];
+        ELFI_REQUIRE(width >= 1 && dst_host[k] && ld_dst_host[k] >= width &&
+                     (nA == 0 || (A_host[k] && ldA_host[k] >= width)) &&
+                     (nB == 0 || (B_host[k] && ldB_host[k] >= width)),
+                     "topn_merge_seg: bad descriptor of output %lld", (long long)k);
+        int64_t gb = (R * n_keep * width + 255) / 256;
+        if (gb > int64_t(ctx->sm_count) * 16) gb = int64_t(ctx->sm_count) * 16;
+        gather2_seg_kernel<<<unsigned(gb), 256, 0, stream>>>(
+            A_host[k], ldA_host[k], segA_host[k], nA, B_host[k], ldB_host[k], segB_host[k], n, perm,
+            R, n_keep, width, dst_host[k], ld_dst_host[k], seg_dst_host[k]);
     }
     ELFI_CUDA_OK(cudaGetLastError());
     return ELFI_B200_OK;

@@ -375,6 +375,92 @@ def merge_topn(state, batch, key_state, key_batch, map_b, n_keep):
     return [o.reshape((n_keep,) + tuple(t.shape[1:])) for o, t in zip(outs, batch)]
 
 
+def _seg_rows(t, R):
+    """(R, rows, width) view of a segmented device array (R, rows, *shape), in place when its
+    trailing dimensions are contiguous: (pointer, leading dimension, segment stride, width)."""
+    if t.dim() < 2 or t.shape[0] != R:
+        raise ValueError('expected an (R={}, rows, ...) array, got shape {}'.format(
+            R, tuple(t.shape)))
+    rows = int(t.shape[1])
+    width = 1
+    for extent in t.shape[2:]:
+        width *= int(extent)
+    v = t.reshape(R, rows, width)
+    if v.stride(2) != 1 and width > 1:
+        v = v.contiguous()
+    ld = v.stride(1) if rows > 1 else width
+    return v, ld, v.stride(0), width
+
+
+def merge_topn_seg(state, batch, key_state, key_batch, n_keep):
+    """R independent :func:`merge_topn` calls (map_b None) in one library call: segment r ranks
+    [state[k][r]; batch[k][r]] by [key_state[r]; key_batch[r]] and keeps its n_keep smallest rows.
+    state[k] is (R, nA, ...), batch[k] (R, nB, ...), key_state (R, nA) and key_batch (R, nB) (views
+    such as a column of a distance matrix are read in place).  Returns new (R, n_keep, ...) device
+    arrays, each segment bit-identical to merge_topn on that segment."""
+    R = int(key_batch.shape[0])
+    n_a, n_b = int(key_state.shape[1]), int(key_batch.shape[1])
+    a3 = [_seg_rows(t, R) for t in state]
+    b3 = [_seg_rows(dev.to_device(t), R) for t in batch]
+    widths = [w for _, _, _, w in b3]
+    outs = [dev.empty((R, n_keep, w)) for w in widths]
+    n = len(outs)
+    if n_keep and n:
+        arr_p, arr_i = ctypes.c_void_p * n, ctypes.c_int64 * n
+        pa = arr_p(*[v.data_ptr() if n_a else 0 for v, _, _, _ in a3])
+        la = arr_i(*[ld if n_a else w for (_, ld, _, _), w in zip(a3, widths)])
+        sa = arr_i(*[s for _, _, s, _ in a3])
+        pb = arr_p(*[v.data_ptr() for v, _, _, _ in b3])
+        lb = arr_i(*[ld for _, ld, _, _ in b3])
+        sb = arr_i(*[s for _, _, s, _ in b3])
+        wd = arr_i(*widths)
+        pd = arr_p(*[t.data_ptr() for t in outs])
+        ld = arr_i(*widths)
+        sd = arr_i(*[n_keep * w for w in widths])
+        cast = lambda a: ctypes.cast(a, ctypes.c_void_p)   # noqa: E731
+        _lib.call('elfi_b200_topn_merge_seg_f64', dev.context(), R,
+                  dev.ptr(key_state) if n_a else None, key_state.stride(1) if n_a > 1 else 1,
+                  key_state.stride(0) if n_a else 0, n_a, dev.ptr(key_batch),
+                  key_batch.stride(1) if n_b > 1 else 1, key_batch.stride(0), n_b, n_keep, n,
+                  cast(pa), cast(la), cast(sa), cast(pb), cast(lb), cast(sb), cast(wd), cast(pd),
+                  cast(ld), cast(sd), dev.stream_ptr())
+    return [o.reshape((R, n_keep) + tuple(t.shape[2:])) for o, t in zip(outs, batch)]
+
+
+SEG_METRICS = ('euclidean', 'sqeuclidean', 'cityblock', 'chebyshev', 'minkowski')
+
+
+def dist_seg(S, obs, metric='euclidean', p=2.0):
+    """Segmented distances: S (R B, D) in R segments of B rows, segment r against observed row r
+    of obs (R, D); returns d (R B,).  Each segment is bit-identical to dist_euclid (unweighted) or
+    dist_metric on that segment; Minkowski with p = 1, 2, inf is routed as dist_metric does."""
+    if metric == 'minkowski':
+        if p == 1:
+            metric = 'cityblock'
+        elif p == 2:
+            metric = 'euclidean'
+        elif np.isinf(p):
+            metric = 'chebyshev'
+        elif not p > 0:
+            raise ValueError('p must be greater than 0')
+    if metric not in SEG_METRICS:
+        raise ValueError('dist_seg supports {}, not {!r}'.format(', '.join(SEG_METRICS), metric))
+    code = 0 if metric == 'euclidean' else METRIC_CODES[metric]
+    S = _matrix(S)
+    O = _matrix(obs)
+    R, D = O.shape
+    n = S.shape[0]
+    if S.shape[1] != D:
+        raise ValueError('XA and XB must have the same number of columns '
+                         '(i.e. feature dimension.)')
+    if n % R:
+        raise ValueError('{} rows do not form {} equal segments'.format(n, R))
+    d = dev.empty((n,))
+    _lib.call('elfi_b200_dist_seg_f64', dev.context(), code, float(p), dev.ptr(S), _ld(S), R,
+              n // R, D, dev.ptr(O), _ld(O), dev.ptr(d), dev.stream_ptr())
+    return d
+
+
 class CandidateBuffer:
     """Packed (capacity, width) device buffer of accepted rows + device-side row count: the tail
     of the reference's sample buffers (samplers.py:196-230) filled without host round trips."""

@@ -238,6 +238,28 @@ int elfi_b200_topn_merge_f64(elfi_b200_ctx* ctx, const double* keysA, int64_t ld
                              const int64_t* ldB_host, const int64_t* width_host,
                              double* const* dst_host, const int64_t* ld_dst_host, void* stream);
 
+/* elfi_b200_topn_merge_seg_f64: R independent elfi_b200_topn_merge_f64 calls in one (the lock-step
+ * Rejection repetitions of elfi_b200.Testbench).  Segment r = 0 .. R-1 ranks its virtual
+ * concatenation [A_r (nA rows); B_r (nB rows)] by keys keysA + r seg_keysA (leading dimension
+ * ld_keysA) and keysB + r seg_keysB, and gathers its n_keep smallest rows of each output k into
+ * dst_host[k] + r seg_dst_host[k]; sources are A_host[k] + r segA_host[k] and
+ * B_host[k] + r segB_host[k].  Segment strides and leading dimensions count doubles.  Each
+ * segment's result is bit-identical to elfi_b200_topn_merge_f64 (mapB = NULL) on that segment:
+ * stable, NaN last.  The 8 key passes run over all R (nA + nB) keys at once, then one more stable
+ * 8-bit pass per byte of R - 1 sorts by segment.  Limits: R >= 1, R (nA + nB) < 2^31.  The ten
+ * descriptor arrays are HOST arrays of length n_out; destinations must not alias sources.
+ * Asynchronous on `stream`, deterministic. */
+int elfi_b200_topn_merge_seg_f64(elfi_b200_ctx* ctx, int64_t R, const double* keysA,
+                                 int64_t ld_keysA, int64_t seg_keysA, int64_t nA,
+                                 const double* keysB, int64_t ld_keysB, int64_t seg_keysB,
+                                 int64_t nB, int64_t n_keep, int64_t n_out,
+                                 const double* const* A_host, const int64_t* ldA_host,
+                                 const int64_t* segA_host, const double* const* B_host,
+                                 const int64_t* ldB_host, const int64_t* segB_host,
+                                 const int64_t* width_host, double* const* dst_host,
+                                 const int64_t* ld_dst_host, const int64_t* seg_dst_host,
+                                 void* stream);
+
 /* elfi_b200_wquantile_f64: weighted_sample_quantile (elfi/methods/utils.py:379-411).
  *   x (n), w (n) or NULL (equal weights), 0 <= alpha <= 1.
  *   out[0] = alpha-quantile (an element of x), out[1] = its rank in sorted order (as double).
@@ -954,10 +976,24 @@ int elfi_b200_rowsort_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, int6
  * row is read from HBM once for all C.  No scratch, no atomics: repeated calls give the same bits.
  * Asynchronous on `stream`. */
 #define ELFI_B200_METRIC_EUCLIDEAN 0
+
 int elfi_b200_subset_distance_f64(elfi_b200_ctx* ctx, int32_t metric, const double* S, int64_t ldS,
                                   int64_t B, int64_t W, const double* obs, const int32_t* ranges,
                                   const int32_t* comb, int64_t C, double* d_out, int64_t ld_out,
                                   void* stream);
+
+/* elfi_b200_dist_seg_f64: R segments of B rows of S (leading dimension ldS), segment r against
+ * observed row r of obs (R rows, leading dimension ld_obs): d_out[r B + i] = cdist(S[r B + i],
+ * obs[r], metric).  metric is ELFI_B200_METRIC_EUCLIDEAN, _SQEUCLIDEAN, _CITYBLOCK, _CHEBYSHEV or
+ * _MINKOWSKI (pexp); each segment is bit-identical to elfi_b200_dist_euclid_thr_f64 (unweighted)
+ * or elfi_b200_dist_metric_thr_f64 on that segment.  No thresholds.  Limits: R >= 1, D >= 1,
+ * R B < 2^31.  The row-stream kernel keeps all R observed rows in shared memory; when D < 16,
+ * S is not TMA-addressable, or R ceil(D / 16) 16 doubles do not fit beside a two-slot ring (about
+ * R ceil(D / 16) 16 <= 20000 on an H100), a thread per row reads them from global memory instead,
+ * with the same arithmetic.  Asynchronous on `stream`. */
+int elfi_b200_dist_seg_f64(elfi_b200_ctx* ctx, int32_t metric, double pexp, const double* S,
+                           int64_t ldS, int64_t R, int64_t B, int64_t D, const double* obs,
+                           int64_t ld_obs, double* d_out, void* stream);
 
 /* elfi_b200_knn_entropy_f64: the nearest-neighbour part of the minimum-entropy criterion
  * (diagnostics.py:214-253) for C point sets of n points in q dimensions at once.
