@@ -32,6 +32,26 @@ def _ld(t):
     return t.stride(0) if t.shape[0] > 1 else t.shape[1]
 
 
+def _out(out, shape, name):
+    """A caller's ``out=`` for an entry point that writes rows of ``shape[1]`` adjacent doubles
+    ``stride(0)`` apart (or, for a 1-d shape, one double per row): float64 device data of exactly
+    ``shape`` whose rows do not overlap.  A transposed or column-strided view would be written in
+    the wrong places, so it is refused."""
+    if out is None:
+        return dev.empty(shape)
+    if not (dev.is_device_array(out) and out.dtype == torch.float64):
+        raise ValueError('{}: out must be a float64 device tensor'.format(name))
+    if tuple(out.shape) != tuple(shape):
+        raise ValueError('{}: out must have shape {}, got {}'.format(name, tuple(shape),
+                                                                     tuple(out.shape)))
+    rows = shape[0]
+    width = shape[1] if len(shape) > 1 else 1
+    if (len(shape) > 1 and width > 1 and out.stride(1) != 1) or (rows > 1 and out.stride(0) < width):
+        raise ValueError('{}: out must have unit column stride and non-overlapping rows, got '
+                         'strides {}'.format(name, tuple(out.stride())))
+    return out
+
+
 def _params(params, model, names):
     """The (batch, p) parameter matrix of a model whose p parameters are ``names``."""
     P = _matrix(params)
@@ -267,8 +287,7 @@ def autocov(x, lags=(1,), out=None):
     for lag in lags_arr:
         if not 1 <= lag < n:
             raise ValueError('lag {} outside [1, {})'.format(lag, n))
-    if out is None:
-        out = dev.empty((B, len(lags_arr)))
+    out = _out(out, (B, len(lags_arr)), 'autocov')
     _lib.call('elfi_b200_summary_autocov_f64', dev.context(), dev.ptr(x), _ld(x), B, n,
               dev.ptr(lags_arr), len(lags_arr), dev.ptr(out), out.stride(0) if B > 1 else
               out.shape[1], dev.stream_ptr())
@@ -281,8 +300,7 @@ def meanvar(y, out=None):
     Returns a (B, 2) tensor [np.mean(y, axis=1), np.var(y, axis=1)], bit for bit."""
     y = _matrix(y)
     B, n = y.shape
-    if out is None:
-        out = dev.empty((B, 2))
+    out = _out(out, (B, 2), 'meanvar')
     _lib.call('elfi_b200_summary_meanvar_f64', dev.context(), dev.ptr(y), _ld(y), B, n,
               dev.ptr(out), out.stride(0) if B > 1 else out.shape[1], 0, 1, dev.stream_ptr())
     return out
@@ -1142,10 +1160,9 @@ def count_zeros(y, out=None):
     of y (B, n), as float64 (B,) (or into the column view ``out``)."""
     y = _matrix(y)
     B, n = y.shape
-    if out is None:
-        out = dev.empty((B,))
+    out = _out(out, (B,), 'count_zeros')
     _lib.call('elfi_b200_count_zeros_f64', dev.context(), dev.ptr(y), _ld(y), B, n, dev.ptr(out),
-              out.stride(0), dev.stream_ptr())
+              out.stride(0) if B > 1 else 1, dev.stream_ptr())
     return out
 
 

@@ -104,6 +104,9 @@ int elfi_b200_dist_euclid_thr_dev_f64(elfi_b200_ctx* ctx, const double* S, int64
  * batch to add_data (elfi_model.py:1104-1125); the reference reads S K + 1 times for that.
  * moments (2, D) device: row 0 = column means of the batch, row 1 = M2 = sum_i (x_ij - mean_j)^2
  * (what elfi_b200_colmoments_f64 returns; Chan-merged into (n, mean, M2) by the caller).
+ * Accuracy of the moments (the distances stay bit-identical): as elfi_b200_colmoments_f64, with
+ * the fused kernel's summation depth h = 8 rows per lane + 2 shuffle levels + ceil(B / 32 / nwarps)
+ * tiles per warp + ceil(nwarps / 32) + 31 in the flush, nwarps = 8 or 12 per SM in use.
  * Thresholds: thr_host or thr_dev (at most one non-NULL; both NULL = no acceptance test).
  * W may be NULL only when the stand-alone moments pass is acceptable (the fused kernel is the
  * weighted / nested row stream; pass a row of ones for plain Euclidean distances). */
@@ -279,6 +282,14 @@ int elfi_b200_wquantile_f64(elfi_b200_ctx* ctx, const double* x, const double* w
  * which is algebraically AdaptiveDistance.add_data (elfi/model/elfi_model.py:1104-1125);
  * parity is tolerance-level (the reference itself only promises np.std agreement,
  * tests/unit/test_elfi_model.py:185-253).
+ *   Accuracy: the sums run over d_i = x_ij - x_0j (shift = first row), so with u = 2^-53,
+ *   gamma_k = k u / (1 - k u) and summation depth h = ceil(R / 8) + 7 + ceil(B / R), where
+ *   R = max(64, ceil(B / ceil(8 sm_count / ceil(D / 32)))) rows go to one block:
+ *     |M2^ - M2|     <= 4 gamma_{h+3} sum_i d_i^2 <= 4 gamma_{h+3} (B + 1) M2,
+ *     |mean^ - mean| <= u |mean| + gamma_{h+2} sum_i |d_i| / B.
+ *   sum_i d_i^2 <= (B + 1) M2 because x_0 is one of the data: the cancellation is bounded
+ *   whatever the offset of the column.  A constant column gives M2 = 0.0 exactly.  The derivation
+ *   and the checks are in tests/rowstream_cases.py.
  *
  * elfi_b200_weighted_stats_f64: weighted_var and its ingredients (elfi/methods/utils.py:108-139):
  *   stats = [V1 = sum w, V2 = sum w^2, xbar_0..p-1 = np.average(x, weights=w),

@@ -266,12 +266,36 @@ def wquantile_f64(ctx, x, w, n, alpha, out, stream):
     res[1] = float(np.searchsorted(np.sort(x), q))
 
 
+SM_COUNT = 132   # the multiprocessors colmoments_f64 sizes its grid by (an H100 SXM)
+
+
 def colmoments_f64(ctx, S, ldS, B, D, out, stream):
-    S = _mat(S, B, D, ldS)
+    """colmoments_partial_kernel + colmoments_final_kernel (smc.cu) in their float64 order: shift
+    by the first row; each block of R rows has 8 sequential chains (rows r0 + t, r0 + t + 8, ...),
+    added t = 0 .. 7; the blocks are added in order; mean = x_0 + s1 / B, M2 = s2 - s1^2 / B.
+    (The kernel's fma(d, d, s2) is a rounded product and add here: within the same bound.)"""
+    S = np.ascontiguousarray(_mat(S, B, D, ldS))
     res = _mat(out, 2, D)
-    mean = S.mean(axis=0)
-    res[0] = mean
-    res[1] = ((S - mean) ** 2).sum(axis=0)
+    colgroups = -(-D // 32)
+    slabs = -(-(SM_COUNT * 8) // colgroups)
+    rows = max(-(-B // slabs), 64)
+    with np.errstate(invalid='ignore', over='ignore'):
+        d = S - S[0]
+        s1 = np.zeros(D)
+        s2 = np.zeros(D)
+        for r0 in range(0, B, rows):
+            blk = d[r0:r0 + rows]
+            b1 = np.zeros(D)
+            b2 = np.zeros(D)
+            for t in range(8):
+                chain = blk[t::8]
+                if len(chain):
+                    b1 = b1 + np.cumsum(chain, axis=0)[-1]
+                    b2 = b2 + np.cumsum(chain * chain, axis=0)[-1]
+            s1 = s1 + b1
+            s2 = s2 + b2
+        res[0] = S[0] + s1 / B
+        res[1] = s2 - s1 * s1 / B
 
 
 def weighted_stats_f64(ctx, x, ldx, w, N, p, stats, stream):
