@@ -96,6 +96,7 @@ SIGNATURES = {
                                  c_i64, c_ptr, c_i64, c_ptr, c_i64, c_ptr],
     'elfi_b200_count_zeros_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr],
     'elfi_b200_chi_squared_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
+    'elfi_b200_ricker_wood_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_i64, c_ptr],
     'elfi_b200_sim_lorenz_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_dbl, c_dbl, c_dbl,
                                  c_dbl, c_u64, c_u64, c_ptr, c_ptr, c_i64, c_ptr],
     'elfi_b200_lorenz_summaries_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr,

@@ -1195,6 +1195,30 @@ def chi_squared(S, obs):
     return out
 
 
+RICKER_WOOD_NOBS_MIN, RICKER_WOOD_NOBS_MAX = 7, 2048   # the shared-memory sort of the differences
+RICKER_WOOD_WIDTH = 13
+
+
+def wood_summaries(y, design):
+    """Wood's 13 Ricker statistics (ss_wood of elfi_b200.examples.ricker) of each row of y (B, n),
+    7 <= n <= RICKER_WOOD_NOBS_MAX, on the device.  design: the (3, n - 1) pseudo-inverse of the
+    observed series' cubic design (ricker.wood_design), a host array or, to avoid a copy per call,
+    a device tensor.  Returns a (B, 13) device tensor; accuracy in include/elfi_b200.h."""
+    y = _matrix(y)
+    B, n = y.shape
+    if not RICKER_WOOD_NOBS_MIN <= n <= RICKER_WOOD_NOBS_MAX:
+        raise ValueError("Wood's statistics on the device take {} <= n_obs <= {}, got {}".format(
+            RICKER_WOOD_NOBS_MIN, RICKER_WOOD_NOBS_MAX, n))
+    if tuple(design.shape) != (3, n - 1):
+        raise ValueError('the cubic design of a series of {} values is (3, {}), got shape {}'.format(
+            n, n - 1, tuple(design.shape)))
+    P = dev.to_device(design)
+    out = dev.empty((B, RICKER_WOOD_WIDTH))
+    _lib.call('elfi_b200_ricker_wood_f64', dev.context(), dev.ptr(y), _ld(y), B, n, dev.ptr(P),
+              dev.ptr(out), RICKER_WOOD_WIDTH, dev.stream_ptr())
+    return out
+
+
 # ---- Lorenz forecast model (elfi/examples/lorenz.py) ----------------------------------------------
 LORENZ_NOBS_MIN, LORENZ_NOBS_MAX = 4, 128     # variables of the ring on the device
 LORENZ_SUMM_NOBS_MIN = 2     # one variable: NumPy sums over time pairwise, not row by row

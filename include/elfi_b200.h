@@ -584,6 +584,27 @@ int elfi_b200_count_zeros_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, 
 int elfi_b200_chi_squared_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B, int64_t K,
                               const double* obs, double* out, void* stream);
 
+/* The 13 Ricker statistics of Wood (2010, Nature 466:1102) in this project's reading (ss_wood of
+ * elfi_b200/examples/ricker.py defines them in NumPy); layout in elfi_b200/csrc/ricker_wood.cu.
+ * Row i of Y (B, n; ldY >= n), 7 <= n <= 2048, gives out[i * ld_out + 0..12] (ld_out >= 13):
+ *   0 mean; 1 number of zeros; 2..7 autocovariances sum_t (y_t - m)(y_{t+k} - m) / n, k = 0..5;
+ *   8..10 P e, e the sorted differences y_{t+1} - y_t and P (3 x (n-1), row-major, on the device)
+ *   the pseudo-inverse of [o, o^2, o^3] for the sorted observed differences o;
+ *   11..12 the minimum-norm least-squares (a1, a2) of y_{t+1}^0.3 = a1 y_t^0.3 + a2 y_t^0.6.
+ * Rank rule of (a1, a2), with N the distinct nonzero values among y_0 .. y_{n-2}: N empty gives
+ * (0, 0); N = {k} gives s (k^0.3, k^0.6) / (k^0.6 + k^1.2), s the mean of y_{t+1}^0.3 over the t
+ * with y_t = k; otherwise the normal equations of the two columns.
+ * Accuracy against the host definition on the same row:
+ *   * columns 0..7 are bit-identical for every n (NumPy's pairwise summation order, also above
+ *     128 terms);
+ *   * column 8 + j is within 2 (n-1) 2^-53 sum_t |P_jt e_t|;
+ *   * the branch of the rank rule is the same, and on rows of full column rank (a1, a2) is within
+ *     1e3 2^-53 cond([u v])^2 relative (u, v the two regressor columns).
+ * A row with a non-finite value gives 13 NaN.  Results are bit-identical across calls and do not
+ * depend on B or on the other rows; B = 0 is a no-op. */
+int elfi_b200_ricker_wood_f64(elfi_b200_ctx* ctx, const double* Y, int64_t ldY, int64_t B, int64_t n,
+                              const double* P, double* out, int64_t ld_out, void* stream);
+
 /* Lorenz forecast model of elfi/examples/lorenz.py (throughput mode, statistical parity); stream
  * layout, lane layout and arithmetic in elfi_b200/csrc/lorenz.cu and lorenz.cuh.
  * sim_lorenz: row i has parameters (theta1, theta2) = P[i * ldP], P[i * ldP + 1] (ldP >= 2) and
