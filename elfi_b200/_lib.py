@@ -141,9 +141,14 @@ SIGNATURES = {
                                               c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr],
     'elfi_b200_synlik_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr, c_ptr,
                              ctypes.c_int32, c_ptr, c_i64, c_ptr, c_ptr],
+    'elfi_b200_synlik_obs_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr, c_i64,
+                                 c_ptr, ctypes.c_int32, c_ptr, c_i64, c_ptr, c_ptr],
     'elfi_b200_bsl_mh_step_f64': [c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_u64, c_ptr,
                                   c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
                                   c_i64, c_ptr],
+    'elfi_b200_bsl_mh_step_keyed_f64': [c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr,
+                                        c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr,
+                                        c_ptr, c_ptr, c_ptr, c_i64, c_ptr],
     'elfi_b200_regadj_mask_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_i64, c_i64,
                                   c_ptr, c_ptr, c_ptr],
     'elfi_b200_regadj_moments_f64': [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_i64, c_i64,

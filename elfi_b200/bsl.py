@@ -191,6 +191,16 @@ class BSL(ModelBased):
         proposals and uniforms from RandomState(seed), chain c >= 1 from
         RandomState(get_sub_seed(seed, c)).  Returns a BslSample; with n_chains > 1 it also holds
         `chains` (n_chains, n_samples, p) and the per-chain `acc_rates`."""
+        self._set_up(n_samples, sigma_proposals, params0, param_names, burn_in,
+                     logit_transform_bound, n_chains)
+        return self.infer(n_samples)
+
+    def _set_up(self, n_samples, sigma_proposals, params0=None, param_names=None, burn_in=0,
+                logit_transform_bound=None, n_chains=1, device_state=None):
+        """Everything `sample` does before its rounds: the prior, the chains, the initial state and,
+        in throughput mode, the device chains (in `device_state` when given, see
+        _init_device_chains).  A Testbench sets up several samplers this way and runs their rounds
+        together."""
         n_chains = int(n_chains)
         if n_chains < 1:
             raise ValueError('n_chains must be at least 1, got {}'.format(n_chains))
@@ -203,8 +213,7 @@ class BSL(ModelBased):
         self.logit_transform_bound = None if logit_transform_bound is None else \
             np.array(logit_transform_bound)
         self._set_chains(n_chains)
-        self._init_state(n_samples, params0)
-        return self.infer(n_samples)
+        self._init_state(n_samples, params0, device_state)
 
     def _set_chains(self, C):
         if C != self.n_chains:
@@ -234,7 +243,7 @@ class BSL(ModelBased):
                 params0[outside][0] if C > 1 else params0[0], where))
         return params0
 
-    def _init_state(self, n_samples, params0=None):
+    def _init_state(self, n_samples, params0=None, device_state=None):
         self.state['n_batches'] = 0
         self.state['n_sim'] = 0
         self.state['round'] = 0
@@ -252,7 +261,7 @@ class BSL(ModelBased):
         self._logprior[:, 0] = np.reshape(self.prior.logpdf(params0), -1)
         self._share_state()
         if self.device_proposal is not None:
-            self._init_device_chains(n_samples, params0)
+            self._init_device_chains(n_samples, params0, device_state)
 
     def _share_state(self):
         one = (lambda a: a[0]) if self.n_chains == 1 else (lambda a: a)
@@ -260,10 +269,12 @@ class BSL(ModelBased):
         self.state['logprior'] = one(self._logprior)
         self.state['logposterior'] = one(self._logpost)
 
-    def _init_device_chains(self, n_samples, params0):
+    def _init_device_chains(self, n_samples, params0, device_state=None):
         """Device state of throughput mode: the chains, their log posteriors and acceptance
         counters, the pending proposals (params0 at iteration 0) and the (p, C b) parameters of
-        the next batch."""
+        the next batch.  `device_state` may hold zero-filled views of caller-owned buffers of
+        these shapes under the keys 'chains', 'logpost', 'n_acc', 'prop', 'prop_lp' and 'rows'
+        (a column block of a wider (p, .) matrix); otherwise this sampler allocates its own."""
         dp = self.device_proposal
         names = list(self.parameter_names)
         if list(dp.parameter_names) != names:
@@ -273,12 +284,22 @@ class BSL(ModelBased):
         sources = dp.sources if getattr(dp, '_cond', False) else None
         self._tables = ops.bsl_mh_tables(dp.specs, self.sigma_proposals, sources,
                                          self.logit_transform_bound)
-        self._prop = dev.to_device(params0).contiguous()
-        self._prop_lp = dp.logpdf(self._prop)
-        self._chains_dev = dev.zeros((C, n_samples, p))
-        self._logpost_dev = dev.zeros((C, n_samples))
-        self._n_acc_dev = dev.zeros((C,), dtype=torch.int64)
-        self._rows = dev.empty((p, C * b))
+        if device_state is None:
+            self._prop = dev.to_device(params0).contiguous()
+            self._prop_lp = dp.logpdf(self._prop)
+            self._chains_dev = dev.zeros((C, n_samples, p))
+            self._logpost_dev = dev.zeros((C, n_samples))
+            self._n_acc_dev = dev.zeros((C,), dtype=torch.int64)
+            self._rows = dev.empty((p, C * b))
+        else:
+            self._prop = device_state['prop']
+            self._prop.copy_(dev.to_device(params0))
+            self._prop_lp = device_state['prop_lp']
+            self._prop_lp.copy_(dp.logpdf(self._prop))
+            self._chains_dev = device_state['chains']
+            self._logpost_dev = device_state['logpost']
+            self._n_acc_dev = device_state['n_acc']
+            self._rows = device_state['rows']
         self._rows.view(p, C, b).copy_(self._prop.t()[:, :, None].expand(p, C, b))
 
     def prepare_new_batch(self, batch_index):
@@ -318,8 +339,12 @@ class BSL(ModelBased):
                 where))
 
     def _process_simulated(self):
+        self._step(self._loglikelihoods())
+
+    def _step(self, ll):
+        """The Metropolis-Hastings step of the round, from the (C,) log-likelihoods of
+        `_loglikelihoods` (or the same values computed by a caller)."""
         n = self.state['n_samples']
-        ll = self._loglikelihoods()
         if self.device_proposal is not None:
             if n == 0:
                 self._check_first_round(dev.to_host(ll))   # the one read of throughput mode

@@ -6,11 +6,13 @@
 // One CTA per chain.  Thread 0 makes the chain's decision for iteration t and draws the proposal of
 // iteration t + 1; then the CTA writes the chain's b rows of the next batch's parameters.
 //
-// Random stream (Philox4x32-10 keyed by the sampler's seed; include/elfi_b200.h has the contract):
-//   counter (t, c, 0, SALT_BSL):      u = u01(x, y), the uniform of chain c's decision at iteration t
-//   counter (t, c, 1 + k, SALT_BSL):  z_2k, z_2k+1 (Box-Muller, boxmuller.cuh) of chain c's
+// Random stream (Philox4x32-10 keyed by the sampler's seed, or by keys[c] in the keyed entry point;
+// include/elfi_b200.h has the contract).  With lane l = c, or lanes[c] in the keyed entry point:
+//   counter (t, l, 0, SALT_BSL):      u = u01(x, y), the uniform of chain c's decision at iteration t
+//   counter (t, l, 1 + k, SALT_BSL):  z_2k, z_2k+1 (Box-Muller, boxmuller.cuh) of chain c's
 //                                     proposal for iteration t, k = 0 .. ceil(p / 2) - 1
-// so no value depends on C, on the other chains or on the launch shape.
+// so no value depends on C, on the other chains or on the launch shape, and the chains of several
+// samplers (a Testbench's repetitions) can step in one launch.
 #include "boxmuller.cuh"
 #include "common.cuh"
 #include "philox.cuh"
@@ -76,7 +78,8 @@ __device__ __forceinline__ double bsl_jacobian(const BslStepParams& P, const dou
 template <int PMAX>
 __global__ void __launch_bounds__(BSL_THREADS)
 bsl_mh_step_kernel(const BslStepParams P, int p, int64_t t, int64_t n_samples, int64_t burn_in,
-                   int64_t b, uint64_t seed, const double* __restrict__ loglik,
+                   int64_t b, uint64_t seed, const uint64_t* __restrict__ keys,
+                   const uint32_t* __restrict__ lanes, const double* __restrict__ loglik,
                    double* __restrict__ prop, double* __restrict__ prop_lp,
                    double* __restrict__ chains, double* __restrict__ logpost,
                    int64_t* __restrict__ n_acc, double* __restrict__ rows, int64_t ld_rows) {
@@ -84,7 +87,9 @@ bsl_mh_step_kernel(const BslStepParams P, int p, int64_t t, int64_t n_samples, i
     const int64_t c = blockIdx.x;
     const bool next = t + 1 < n_samples;
     if (threadIdx.x == 0) {
-        const Philox ph(seed);
+        // NULL keys and lanes: the sampler's seed and lane c
+        const Philox ph(keys ? keys[c] : seed);
+        const uint32_t lane = lanes ? lanes[c] : uint32_t(c);
         double* pc = prop + c * p;
         double* state = chains + (c * n_samples + t) * p;
         double* lpost = logpost + c * n_samples + t;
@@ -103,7 +108,7 @@ bsl_mh_step_kernel(const BslStepParams P, int p, int64_t t, int64_t n_samples, i
                 const double res = (bsl_jacobian<PMAX>(P, s, p) - bsl_jacobian<PMAX>(P, prev, p))
                                    + (lp_new - lpost[-1]);
                 const double prob = fmin(1.0, exp(fmin(700.0, fmax(-700.0, res))));
-                const uint4 r = ph(uint32_t(t), uint32_t(c), 0u, SALT_BSL);
+                const uint4 r = ph(uint32_t(t), lane, 0u, SALT_BSL);
                 accept = u01(r.x, r.y) < prob;
             }
             if (!accept) {
@@ -127,7 +132,7 @@ bsl_mh_step_kernel(const BslStepParams P, int p, int64_t t, int64_t n_samples, i
             for (int k = 0; k < PMAX; k += 2) {
                 if (k >= p) break;
                 double z0, z1;
-                normal2(ph(uint32_t(t + 1), uint32_t(c), 1u + uint32_t(k / 2), SALT_BSL), z0, z1);
+                normal2(ph(uint32_t(t + 1), lane, 1u + uint32_t(k / 2), SALT_BSL), z0, z1);
 #pragma unroll
                 for (int a = k; a < PMAX; ++a) {
                     if (a >= p) break;
@@ -162,6 +167,7 @@ bsl_mh_step_kernel(const BslStepParams P, int p, int64_t t, int64_t n_samples, i
 
 static int bsl_mh_step_launch(elfi_b200_ctx* ctx, int64_t C, int64_t p, int64_t t,
                               int64_t n_samples, int64_t burn_in, int64_t b, uint64_t seed,
+                              const uint64_t* keys, const uint32_t* lanes,
                               const double* spec_host, const double* chol_host,
                               const double* bounds_host, const double* loglik, double* prop,
                               double* prop_lp, double* chains, double* logpost, int64_t* n_acc,
@@ -206,8 +212,8 @@ static int bsl_mh_step_launch(elfi_b200_ctx* ctx, int64_t C, int64_t p, int64_t 
     return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
         with_pow2<2, PRIOR_MAX_PARAMS>(int(p), [&](auto pm) {
             bsl_mh_step_kernel<decltype(pm)::value><<<unsigned(C), BSL_THREADS, 0, stream>>>(
-                P, int(p), t, n_samples, burn_in, b, seed, loglik, prop, prop_lp, chains, logpost,
-                n_acc, rows, ld_rows);
+                P, int(p), t, n_samples, burn_in, b, seed, keys, lanes, loglik, prop, prop_lp,
+                chains, logpost, n_acc, rows, ld_rows);
             return 0;
         });
         return ELFI_B200_OK;
@@ -224,9 +230,22 @@ int elfi_b200_bsl_mh_step_f64(elfi_b200_ctx* ctx, int64_t C, int64_t p, int64_t 
                               const double* bounds_host, const double* loglik, double* prop,
                               double* prop_lp, double* chains, double* logpost, int64_t* n_acc,
                               double* rows, int64_t ld_rows, void* stream) {
-    return elfi::bsl_mh_step_launch(ctx, C, p, t, n_samples, burn_in, b, seed, spec_host,
-                                    chol_host, bounds_host, loglik, prop, prop_lp, chains,
-                                    logpost, n_acc, rows, ld_rows, stream);
+    return elfi::bsl_mh_step_launch(ctx, C, p, t, n_samples, burn_in, b, seed, nullptr, nullptr,
+                                    spec_host, chol_host, bounds_host, loglik, prop, prop_lp,
+                                    chains, logpost, n_acc, rows, ld_rows, stream);
+}
+
+int elfi_b200_bsl_mh_step_keyed_f64(elfi_b200_ctx* ctx, int64_t C, int64_t p, int64_t t,
+                                    int64_t n_samples, int64_t burn_in, int64_t b,
+                                    const uint64_t* keys, const uint32_t* lanes,
+                                    const double* spec_host, const double* chol_host,
+                                    const double* bounds_host, const double* loglik, double* prop,
+                                    double* prop_lp, double* chains, double* logpost,
+                                    int64_t* n_acc, double* rows, int64_t ld_rows, void* stream) {
+    ELFI_REQUIRE(keys && lanes, "bsl_mh_step_keyed: NULL keys or lanes");
+    return elfi::bsl_mh_step_launch(ctx, C, p, t, n_samples, burn_in, b, 0, keys, lanes,
+                                    spec_host, chol_host, bounds_host, loglik, prop, prop_lp,
+                                    chains, logpost, n_acc, rows, ld_rows, stream);
 }
 
 }  // extern "C"

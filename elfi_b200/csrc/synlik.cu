@@ -14,8 +14,10 @@
 //      1 / (n - 1), mirrored to a full symmetric Sigma.
 //   4. whitening: W Sigma W^T as two batched NT products through scratch (synlik_gemm_nt_kernel).
 //   5. synlik_factor_kernel: one CTA per (group, penalty).  It shrinks Sigma into shared memory,
-//      appends the right-hand side b = y - mu (or W (y - mu)) as row d, and runs a right-looking
-//      Cholesky over the d + 1 rows: row d then holds z = L^{-1} b, so one factorisation gives
+//      appends the right-hand side b = y_g - mu (or W (y_g - mu)) as row d, where y_g is the
+//      group's observation (one row shared by every group, or one row per group), and runs a
+//      right-looking Cholesky over the d + 1 rows: row d then holds z = L^{-1} b, so one
+//      factorisation gives
 //      log det Sigma = 2 sum log L_jj and m = |z|^2.
 #include <cfloat>
 #include <cmath>
@@ -187,10 +189,11 @@ __host__ __device__ constexpr int64_t synlik_factor_doubles(int d) {
 }
 
 // loglik[g * max(K, 1) + k] for group g and penalty k (lambda = 0 when K = 0).  Sig holds the
-// group's covariance at Sig[g * d * d + i * d + j], i >= j read, times scale.
+// group's covariance at Sig[g * d * d + i * d + j], i >= j read, times scale; the group's
+// observation is y + g * ld_y (ld_y = 0: one row for every group).
 __global__ void __launch_bounds__(512)
 synlik_factor_kernel(const double* __restrict__ Sig, double scale, const double* __restrict__ mu,
-                     const double* __restrict__ y, const double* __restrict__ W,
+                     const double* __restrict__ y, int64_t ld_y, const double* __restrict__ W,
                      const double* __restrict__ pen, int K, int d, int estimator, double n,
                      double c_unbiased, double* __restrict__ loglik) {
     extern __shared__ double sm[];
@@ -206,6 +209,7 @@ synlik_factor_kernel(const double* __restrict__ Sig, double scale, const double*
     const double lam = K ? pen[k] : 0.0;
     const double* Sg = Sig + g * int64_t(d) * d;
     const double* mug = mu + g * d;
+    const double* yg = y + g * ld_y;
     double* out = loglik + g * (K ? K : 1) + k;
 
     // a non-finite input makes its column sum, so its mean, non-finite
@@ -222,7 +226,7 @@ synlik_factor_kernel(const double* __restrict__ Sig, double scale, const double*
             L[i * ld + j] = v;
         }
     }
-    for (int j = tid; j < d; j += nthr) col[j] = y[j] - mug[j];
+    for (int j = tid; j < d; j += nthr) col[j] = yg[j] - mug[j];
     __syncthreads();
     for (int i = tid; i < d; i += nthr) {
         double b = col[i];
@@ -288,16 +292,15 @@ static double log_c(int64_t k, double nu) {
 
 static size_t align256(size_t bytes) { return (bytes + 255) / 256 * 256; }
 
-}  // namespace elfi
-
-extern "C" {
-
-int elfi_b200_synlik_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_row, int64_t ld_group,
-                         int64_t G, int64_t n, int64_t d, const double* y, const double* W,
-                         int32_t estimator, const double* penalties_host, int64_t K,
-                         double* loglik, void* stream_) {
-    using namespace elfi;
+// both entry points: group g's observation is y + g * ld_y (ld_y = 0: one row for every group)
+static int synlik_launch(elfi_b200_ctx* ctx, const double* S, int64_t ld_row, int64_t ld_group,
+                         int64_t G, int64_t n, int64_t d, const double* y, int64_t ld_y,
+                         const double* W, int32_t estimator, const double* penalties_host,
+                         int64_t K, double* loglik, void* stream_) {
     ELFI_REQUIRE(ctx && (G == 0 || (S && y && loglik)), "synlik: NULL argument");
+    ELFI_REQUIRE(ld_y == 0 || ld_y >= d,
+                 "synlik: the observation stride must be 0 or at least d (ld_y=%lld d=%lld)",
+                 (long long)ld_y, (long long)d);
     ELFI_REQUIRE(d >= 1 && d <= SL_D_MAX && n >= 2 && n < (int64_t(1) << 31) && G >= 0 &&
                      G <= (int64_t(1) << 22) && ld_row >= d && ld_group >= 0,
                  "synlik: bad shape (1 <= d <= %d, 2 <= n < 2^31, G <= 2^22, ld_row >= d, "
@@ -373,10 +376,31 @@ int elfi_b200_synlik_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_row, in
                                           cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           int(synlik_factor_doubles(SL_D_MAX) * 8)));
         synlik_factor_kernel<<<dim3(unsigned(G), unsigned(K ? K : 1)), factor_threads, factor_smem,
-                               stream>>>(sig, sig_scale, mu, y, W, pen, int(K), di, int(estimator),
-                                         double(n), c_unb, loglik);
+                               stream>>>(sig, sig_scale, mu, y, ld_y, W, pen, int(K), di,
+                                         int(estimator), double(n), c_unb, loglik);
         return ELFI_B200_OK;
     });
+}
+
+}  // namespace elfi
+
+extern "C" {
+
+int elfi_b200_synlik_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_row, int64_t ld_group,
+                         int64_t G, int64_t n, int64_t d, const double* y, const double* W,
+                         int32_t estimator, const double* penalties_host, int64_t K,
+                         double* loglik, void* stream) {
+    return elfi::synlik_launch(ctx, S, ld_row, ld_group, G, n, d, y, 0, W, estimator,
+                               penalties_host, K, loglik, stream);
+}
+
+int elfi_b200_synlik_obs_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_row,
+                             int64_t ld_group, int64_t G, int64_t n, int64_t d, const double* Y,
+                             int64_t ld_y, const double* W, int32_t estimator,
+                             const double* penalties_host, int64_t K, double* loglik,
+                             void* stream) {
+    return elfi::synlik_launch(ctx, S, ld_row, ld_group, G, n, d, Y, ld_y, W, estimator,
+                               penalties_host, K, loglik, stream);
 }
 
 }  // extern "C"

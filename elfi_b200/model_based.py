@@ -112,9 +112,24 @@ class ModelBased(ParameterInference):
         self._merge_batch(batch)
         if self.state['n_sim_round'] == self.n_sim_round:
             self._process_simulated()
-            self.state['round'] += 1
-            if self.state['round'] < self.objective['round']:
-                self._init_round()
+            self._end_round()
+
+    def _end_round(self):
+        self.state['round'] += 1
+        if self.state['round'] < self.objective['round']:
+            self._init_round()
+
+    def _simulate_round(self):
+        """Run the batches of the current round (as `iterate` does) and stop when its features
+        are complete, without processing them: the caller evaluates the round and then calls
+        `_end_round`.  A Testbench evaluates the rounds of several samplers in one call."""
+        while self.state['n_sim_round'] < self.n_sim_round:
+            batch_index = self._next_batch_index
+            values = self.prepare_new_batch(batch_index)
+            self._next_batch_index += 1
+            batch = self._run_batch(batch_index, values)
+            super().update(batch, batch_index)
+            self._merge_batch(batch)
 
     def _init_round(self):
         self.state['n_sim_round'] = 0

@@ -1903,7 +1903,9 @@ SYNLIK_ESTIMATORS = {'standard': 0, 'unbiased': 1}
 
 def synlik(S, y, estimator='standard', penalties=None, whitening=None):
     """Gaussian synthetic log-likelihood of the observed summaries y (d,) under each group of
-    simulated summaries S, (n, d) or (G, n, d), host or device, any row and group strides.
+    simulated summaries S, (n, d) or (G, n, d), host or device, any row and group strides.  A y of
+    shape (G, d), G > 1, gives each group its own observation (any row stride, 0 included); group
+    g's value is then the one S[g] alone would give against y[g].
 
     estimator 'standard' is gaussian_syn_likelihood (Warton shrinkage at each of the penalties, and
     whitening by the (d, d) matrix W, both optional); 'unbiased' is
@@ -1927,9 +1929,19 @@ def synlik(S, y, estimator='standard', penalties=None, whitening=None):
         raise ValueError('synlik takes n >= 2 simulations per group, got n = {}'.format(n))
     if X.stride(2) != 1 or X.stride(1) < d or X.stride(0) < 0:
         X = X.contiguous()
-    yv = dev.to_device(y).reshape(-1).contiguous()
-    if yv.numel() != d:
-        raise ValueError('y has {} values, S has d = {} summaries'.format(yv.numel(), d))
+    yv = y if dev.is_device_array(y) and y.dtype == torch.float64 else dev.to_device(y)
+    # d values in any shape are the one observation of every group, as before per-group rows
+    per_group = yv.dim() == 2 and yv.numel() != d
+    if per_group:
+        if tuple(yv.shape) != (G, d):
+            raise ValueError('y has shape {}, S has G = {} groups of d = {} summaries'.format(
+                tuple(yv.shape), G, d))
+        if yv.stride(1) != 1 or 0 < yv.stride(0) < d or yv.stride(0) < 0:
+            yv = yv.contiguous()        # stride 0 (an expanded row) is kept: ld_y = 0
+    else:
+        yv = yv.reshape(-1).contiguous()
+        if yv.numel() != d:
+            raise ValueError('y has {} values, S has d = {} summaries'.format(yv.numel(), d))
     W = None
     if whitening is not None:
         W = dev.to_device(whitening).contiguous()
@@ -1945,10 +1957,15 @@ def synlik(S, y, estimator='standard', penalties=None, whitening=None):
         if not np.all((pen >= 0) & (pen <= 1)):
             raise ValueError('Warton penalties must lie in [0, 1], got {}'.format(pen))
     out = dev.empty((G, K) if K else (G,))
-    _lib.call('elfi_b200_synlik_f64', dev.context(), dev.ptr(X), X.stride(1), X.stride(0), G, n,
-              d, dev.ptr(yv), dev.ptr(W), SYNLIK_ESTIMATORS[estimator],
-              None if pen is None else ctypes.c_void_p(pen.ctypes.data), K, dev.ptr(out),
-              dev.stream_ptr())
+    tail = (dev.ptr(W), SYNLIK_ESTIMATORS[estimator],
+            None if pen is None else ctypes.c_void_p(pen.ctypes.data), K, dev.ptr(out),
+            dev.stream_ptr())
+    if per_group:
+        _lib.call('elfi_b200_synlik_obs_f64', dev.context(), dev.ptr(X), X.stride(1),
+                  X.stride(0), G, n, d, dev.ptr(yv), yv.stride(0), *tail)
+    else:
+        _lib.call('elfi_b200_synlik_f64', dev.context(), dev.ptr(X), X.stride(1), X.stride(0), G,
+                  n, d, dev.ptr(yv), *tail)
     return out
 
 
@@ -1979,7 +1996,8 @@ def bsl_mh_tables(specs, sigma_proposals, sources=None, bounds=None):
     return table, L, bnd
 
 
-def bsl_mh_step(tables, t, loglik, prop, prop_lp, chains, logpost, n_acc, rows, seed, burn_in=0):
+def bsl_mh_step(tables, t, loglik, prop, prop_lp, chains, logpost, n_acc, rows, seed, burn_in=0,
+                lanes=None):
     """Iteration t of C lock-step BSL chains on the device (include/elfi_b200.h states the step
     and its Philox stream): the decision of every chain from the round's log-likelihoods
     ``loglik`` (C,) and the pending proposals ``prop`` (C, p) with their log priors ``prop_lp``
@@ -1987,7 +2005,10 @@ def bsl_mh_step(tables, t, loglik, prop, prop_lp, chains, logpost, n_acc, rows, 
     counted in ``n_acc`` (C,) int64 from ``burn_in``; then, unless t is the last iteration, the
     proposals of iteration t + 1 into ``prop`` / ``prop_lp`` and the next batch's parameters into
     ``rows`` (p, C b), chain c's block in columns [c b, (c + 1) b).  ``tables`` is
-    :func:`bsl_mh_tables`.  Asynchronous; nothing is read back."""
+    :func:`bsl_mh_tables`.  ``seed`` is an int (every chain's Philox key, chain c on lane c), or
+    a (C,) int64 device tensor of per-chain keys with ``lanes`` an optional (C,) integer device
+    tensor of lanes (default 0 .. C - 1), so that the chains of several samplers step in one
+    launch.  Asynchronous; nothing is read back."""
     table, L, bnd = tables
     C, n_samples, p = (int(v) for v in chains.shape)
     if not 1 <= C <= BSL_MAX_CHAINS:
@@ -2005,10 +2026,28 @@ def bsl_mh_step(tables, t, loglik, prop, prop_lp, chains, logpost, n_acc, rows, 
                 or not x.is_contiguous():
             raise ValueError('{} must be a contiguous {} device array of shape {}'.format(
                 name, dtype, shape))
-    _lib.call('elfi_b200_bsl_mh_step_f64', dev.context(), C, p, int(t), n_samples, int(burn_in),
-              int(rows.shape[1]) // C, int(seed), dev.ptr(table), dev.ptr(L), dev.ptr(bnd),
-              dev.ptr(loglik), dev.ptr(prop), dev.ptr(prop_lp), dev.ptr(chains), dev.ptr(logpost),
-              dev.ptr(n_acc), dev.ptr(rows), rows.stride(0), dev.stream_ptr())
+    tail = (dev.ptr(table), dev.ptr(L), dev.ptr(bnd), dev.ptr(loglik), dev.ptr(prop),
+            dev.ptr(prop_lp), dev.ptr(chains), dev.ptr(logpost), dev.ptr(n_acc), dev.ptr(rows),
+            rows.stride(0), dev.stream_ptr())
+    b = int(rows.shape[1]) // C
+    if not dev.is_device_array(seed):
+        if lanes is not None:
+            raise ValueError('lanes go with per-chain keys: a (C,) int64 device tensor seed')
+        _lib.call('elfi_b200_bsl_mh_step_f64', dev.context(), C, p, int(t), n_samples,
+                  int(burn_in), b, int(seed), *tail)
+        return
+    if tuple(seed.shape) != (C,) or seed.dtype != torch.int64:
+        raise ValueError('keys (seed) must be a ({},) int64 device tensor, got {} {}'.format(
+            C, tuple(seed.shape), seed.dtype))
+    keys = seed.contiguous()
+    if lanes is None:
+        lanes = torch.arange(C, dtype=torch.int32, device=keys.device)
+    elif not dev.is_device_array(lanes) or tuple(lanes.shape) != (C,) or \
+            lanes.dtype not in (torch.int32, torch.int64):
+        raise ValueError('lanes must be a ({},) int32 or int64 device tensor'.format(C))
+    lanes = lanes.to(torch.int32).contiguous()      # the bits of uint32 lanes
+    _lib.call('elfi_b200_bsl_mh_step_keyed_f64', dev.context(), C, p, int(t), n_samples,
+              int(burn_in), b, dev.ptr(keys), dev.ptr(lanes), *tail)
 
 
 # ---- BOLFIRE ratio-estimation classifier (elfi/methods/classifier.py) ------------------------------

@@ -5,12 +5,24 @@ simulated from the reference parameters, and reports per-parameter sample-mean e
 arguments, result layouts and the seeding order are the reference's, quirks included (DESIGN.md
 section 7, "Testbench").
 
-Rejection in quantile or n_sim mode consumes the same number of batches in every repetition, so
-`run()` steps the R repetitions of such a method together: per batch index, each repetition runs
-its own plan with its own seed, the summaries of all R go into one (R B, D) device matrix, one
-segmented distance launch (ops.dist_seg) measures every block against its own observation, and
-one segmented top-n merge (ops.merge_topn_seg) updates all R best-n buffers.  Repetition r's
-Sample is bit-identical to the serial Rejection(model_r, seed=seed_r).sample(...).
+`run()` steps the R repetitions of two kinds of method together (lock-step); every other method
+runs its repetitions one after the other.  Each repetition keeps its own model copy, observation,
+seed and plan, and its result is bit-identical to its serial run, method(model_r, seed=seed_r)
+.sample(...).
+
+* Rejection in quantile or n_sim mode consumes the same number of batches in every repetition.
+  Per batch index, the summaries of all R go into one (R B, D) device matrix, one segmented
+  distance launch (ops.dist_seg) measures every block against its own observation, and one
+  segmented top-n merge (ops.merge_topn_seg) updates all R best-n buffers.
+* BSL with a device likelihood (any n_chains, with or without device_proposal).  Per iteration
+  every unfinished repetition simulates its own round into its block of one (R C, n_sim_round, d)
+  device feature buffer, one ops.synlik call evaluates the R C groups against their own
+  observations, and one device-to-host read of R C values feeds each repetition's host
+  Metropolis-Hastings step.  Repetitions whose proposals all leave the prior support skip rounds,
+  so they progress raggedly; a finished repetition's group is evaluated and ignored.  In
+  throughput mode (device_proposal) the chains of all repetitions live in stacked device buffers
+  and one keyed ops.bsl_mh_step steps them all, each with its own seed as Philox key: no read
+  happens between the first round's check and the end.
 """
 import functools
 import logging
@@ -19,6 +31,7 @@ import sys
 import numpy as np
 import torch
 
+from . import bsl
 from . import device as dev
 from . import model as em
 from . import ops
@@ -146,9 +159,10 @@ class Testbench:
         self.method_seed_list.append(self._get_seeds(n_rep=self.repetitions))
 
     def run(self, lockstep=True):
-        """Run Testbench.  With `lockstep`, a Rejection method in quantile or n_sim mode runs its
-        repetitions together (see the module docstring); every other method, and every method
-        with ``lockstep=False``, runs its repetitions one after the other."""
+        """Run Testbench.  With `lockstep`, a Rejection method in quantile or n_sim mode and a BSL
+        method with a device likelihood run their repetitions together (see the module
+        docstring); every other method, and every method with ``lockstep=False``, runs its
+        repetitions one after the other."""
         self.testbench_results = []
         for method_index, method in enumerate(self.method_list):
             logger.info('Running {} in testbench.'.format(method.attributes['name']))
@@ -158,11 +172,14 @@ class Testbench:
 
             seeds = self.method_seed_list[method_index]
             metric = self._lockstep_metric(method) if lockstep else None
-            if metric is None:
-                result = self._repeat_inference(method, seeds)
-            else:
+            if metric is not None:
                 result = self._collect_results(method.attributes['name'],
                                                self._lockstep_rejection(method, seeds, *metric))
+            elif lockstep and self._lockstep_bsl_applies(method):
+                result = self._collect_results(method.attributes['name'],
+                                               self._lockstep_bsl(method, seeds))
+            else:
+                result = self._repeat_inference(method, seeds)
             self.testbench_results.append(result)
 
     def _repeat_inference(self, method, seed_list):
@@ -312,6 +329,82 @@ class Testbench:
             rej._n_valid = nv
             results.append(rej.extract_result())
         return results
+
+    # -- lock-step BSL -----------------------------------------------------------------------
+    @staticmethod
+    def _lockstep_bsl_applies(method):
+        """Whether `method` is this package's BSL, without fit kwargs or a pool, with a device
+        likelihood (standard or unbiased)."""
+        a = method.attributes
+        mk = a['method_kwargs']
+        return (a['callable'] is bsl.BSL and not a['fit_kwargs'] and mk.get('pool') is None
+                and bsl._device_likelihood(mk.get('likelihood')) is not None)
+
+    def _lockstep_bsl(self, method, seed_list):
+        a = method.attributes
+        sk = a['sample_kwargs']
+        R = self.repetitions
+        model = self.model.copy()
+        reps = []
+        for i in range(R):
+            model.observed[self.simulator_name] = np.atleast_2d(self.observations[i])
+            reps.append(bsl.BSL(model, **a['method_kwargs'], seed=seed_list[i]))
+        first = reps[0]
+        n_samples = int(sk['n_samples'])
+        C = int(sk.get('n_chains', 1))
+        d, b = first.observed.size, first._rows_per_chain
+        state = None
+        if first.device_proposal is not None:
+            p = len(sk.get('param_names') or first.model.parameter_names)
+            state = dict(chains=dev.zeros((R * C, n_samples, p)),
+                         logpost=dev.zeros((R * C, n_samples)),
+                         n_acc=dev.zeros((R * C,), dtype=torch.int64),
+                         prop=dev.zeros((R * C, p)), prop_lp=dev.zeros((R * C,)),
+                         rows=dev.zeros((p, R * C * b)))
+        feats = dev.zeros((R * C, first.n_sim_round, d))
+        for r, rep in enumerate(reps):
+            block = slice(r * C, (r + 1) * C)
+            rep._set_up(**sk, device_state=None if state is None else dict(
+                {k: v[block] for k, v in state.items() if k != 'rows'},
+                rows=state['rows'][:, r * C * b:(r + 1) * C * b]))
+            rep.set_objective(n_samples)
+            rep._sim = feats[block] if C > 1 else feats[r * C]
+        obs = dev.to_device(np.repeat(np.concatenate([rep.observed.reshape(1, d) for rep in reps]),
+                                      C, axis=0))
+        lik = first._device_lik
+        if state is not None:
+            keys = dev.to_device(np.repeat(np.asarray(seed_list[:R], dtype=np.int64), C),
+                                 dtype=torch.int64)
+            lanes = dev.to_device(np.tile(np.arange(C, dtype=np.int32), R), dtype=torch.int32)
+        while True:
+            live = [rep for rep in reps if not rep.finished]
+            if not live:
+                break
+            if self.progress_bar:
+                self.progress_bar.update_progressbar(
+                    max(rep.state['n_samples'] for rep in live) + 1, n_samples)
+            for rep in live:
+                rep._simulate_round()
+            ll = lik.device(feats, obs)
+            if state is None:
+                ll = dev.to_host(ll)          # the one device-to-host read of the iteration
+                for r, rep in enumerate(reps):
+                    if rep in live:
+                        rep._step(ll[r * C:(r + 1) * C])
+            else:
+                t = first.state['n_samples']          # every repetition runs every round
+                if t == 0:
+                    host = dev.to_host(ll)            # the one read of throughput mode
+                    for r, rep in enumerate(reps):
+                        rep._check_first_round(host[r * C:(r + 1) * C])
+                ops.bsl_mh_step(first._tables, t, ll, state['prop'], state['prop_lp'],
+                                state['chains'], state['logpost'], state['n_acc'], state['rows'],
+                                keys, first.burn_in, lanes=lanes)
+                for rep in live:
+                    rep.state['n_samples'] += 1
+            for rep in live:
+                rep._end_round()
+        return [rep.extract_result() for rep in reps]
 
 
 class TestbenchMethod:

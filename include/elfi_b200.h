@@ -866,6 +866,20 @@ int elfi_b200_synlik_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_row, in
                          int32_t estimator, const double* penalties_host, int64_t K,
                          double* loglik, void* stream);
 
+/* elfi_b200_synlik_obs_f64: elfi_b200_synlik_f64 with an observation per group: group g's
+ * observed summaries are Y[g * ld_y + j], j < d (device), and ld_y = 0 gives every group the one
+ * row Y.  ld_y must be 0 or at least d.  Every promise of elfi_b200_synlik_f64 holds per group:
+ * the -inf rules, whitening (W y_g replaces y), the Warton penalties, the unbiased estimator,
+ * bit-identity across calls, and independence of a group's value from G, K and the other groups
+ * and their observations.  So group g gives the bits of elfi_b200_synlik_f64 on group g alone with
+ * y = Y + g * ld_y, and a Testbench's repetitions, each with its own observation, share one call.
+ * Same limits, scratch and stream behaviour. */
+int elfi_b200_synlik_obs_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_row,
+                             int64_t ld_group, int64_t G, int64_t n, int64_t d, const double* Y,
+                             int64_t ld_y, const double* W, int32_t estimator,
+                             const double* penalties_host, int64_t K, double* loglik,
+                             void* stream);
+
 /* elfi_b200_bsl_mh_step_f64: iteration t of C lock-step BSL Metropolis-Hastings chains in
  * throughput mode (elfi/methods/inference/bsl.py), for p <= 16 parameters.  Device arrays:
  * loglik (C) the synthetic log-likelihoods of the round (elfi_b200_synlik_f64 with G = C), prop
@@ -898,6 +912,21 @@ int elfi_b200_bsl_mh_step_f64(elfi_b200_ctx* ctx, int64_t C, int64_t p, int64_t 
                               const double* bounds_host, const double* loglik, double* prop,
                               double* prop_lp, double* chains, double* logpost, int64_t* n_acc,
                               double* rows, int64_t ld_rows, void* stream);
+
+/* elfi_b200_bsl_mh_step_keyed_f64: elfi_b200_bsl_mh_step_f64 with a Philox key and a lane per
+ * chain slot: keys (C, uint64) and lanes (C, uint32), device, both required.  Slot c draws its
+ * uniform from counter (t, lanes[c], 0, 0x4253434c) and its proposal normals from
+ * (t + 1, lanes[c], 1 + k, 0x4253434c) of Philox4x32-10 keyed by keys[c]; everything else is the
+ * contract above.  elfi_b200_bsl_mh_step_f64 is the case keys[c] = seed, lanes[c] = c, so slot c
+ * of a keyed call gives the bits of an unkeyed call in which the same chain sits at slot lanes[c]
+ * under seed keys[c]: the chains of several samplers, each with its own seed, step in one launch. */
+int elfi_b200_bsl_mh_step_keyed_f64(elfi_b200_ctx* ctx, int64_t C, int64_t p, int64_t t,
+                                    int64_t n_samples, int64_t burn_in, int64_t b,
+                                    const uint64_t* keys, const uint32_t* lanes,
+                                    const double* spec_host, const double* chol_host,
+                                    const double* bounds_host, const double* loglik, double* prop,
+                                    double* prop_lp, double* chains, double* logpost,
+                                    int64_t* n_acc, double* rows, int64_t ld_rows, void* stream);
 
 /* ---- regression adjustment (elfi/methods/post_processing.py: LinearAdjustment) ------------------
  * The local-linear adjustment of Beaumont et al. (2002) on N rows of q summaries
