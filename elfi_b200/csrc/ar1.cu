@@ -24,8 +24,8 @@ namespace elfi {
 
 constexpr uint32_t SALT_AR1 = 0x41523120u;   // "AR1 "
 constexpr int AR1_THREADS = 128;
-constexpr int64_t AR1_NOBS_MAX = int64_t(1) << 24;
-constexpr int64_t AR1_BATCH_MAX = (int64_t(1) << 31) - 1;
+constexpr int64_t AR1_NOBS_MAX = ELFI_B200_AR1_NOBS_MAX;
+constexpr int64_t AR1_BATCH_MAX = ELFI_B200_AR1_BATCH_MAX;
 
 // Row i: parameter phi[i], series X[i * ldX + t] (X may be NULL), distance to p.obs (p.obs may be
 // NULL: then no distance and no mask).  Threads of rows >= B run to the epilogue: its ballot needs

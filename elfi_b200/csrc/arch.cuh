@@ -18,13 +18,15 @@
 #include <stdint.h>
 
 #include "hd.cuh"
+#include "../../include/elfi_b200.h"
 #include "leafsum.cuh"
 
 namespace elfi {
 
-constexpr int ARCH_NOBS_MIN = 2;
-constexpr int ARCH_NOBS_MAX = LEAF_MAX_TERMS;   // one pairwise leaf per reduction
-constexpr int ARCH_LAGS_MAX = 8;
+constexpr int ARCH_NOBS_MIN = ELFI_B200_ARCH_NOBS_MIN;
+constexpr int ARCH_NOBS_MAX = ELFI_B200_ARCH_NOBS_MAX;
+static_assert(ARCH_NOBS_MAX == LEAF_MAX_TERMS, "one pairwise leaf per reduction");
+constexpr int ARCH_LAGS_MAX = ELFI_B200_ARCH_LAGS_MAX;
 
 ELFI_HD double arch_div(double a, double b) {
 #if defined(__CUDA_ARCH__)

@@ -162,12 +162,12 @@ int elfi_b200_sim_bdm_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int6
                           void* stream_) {
     using namespace elfi;
     ELFI_REQUIRE(ctx && (B == 0 || (P && n_events)), "sim_bdm: NULL argument");
-    ELFI_REQUIRE(B >= 0 && B <= 0x7fffffff && ldP >= 3 && N >= 1 && N <= BDM_N_MAX &&
+    ELFI_REQUIRE(B >= 0 && B <= ELFI_B200_BDM_BATCH_MAX && ldP >= 3 && N >= 1 && N <= BDM_N_MAX &&
                      (!X || ldX >= N) && (!S || ldS >= BDM_NSUMM),
                  "sim_bdm: bad shape (1 <= N <= %d, B < 2^31, ldP >= 3, ldX >= N, ldS >= 2; "
                  "B=%lld N=%lld ldP=%lld ldX=%lld ldS=%lld)", BDM_N_MAX, (long long)B,
                  (long long)N, (long long)ldP, (long long)ldX, (long long)ldS);
-    ELFI_REQUIRE(max_events >= 1 && max_events <= int64_t(0xffffffffu),
+    ELFI_REQUIRE(max_events >= 1 && max_events <= ELFI_B200_BDM_MAX_EVENTS_LIMIT,
                  "sim_bdm: 1 <= max_events <= 2^32 - 1 (the event is one Philox word), got %lld",
                  (long long)max_events);
     if (B == 0) return ELFI_B200_OK;

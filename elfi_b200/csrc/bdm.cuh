@@ -27,13 +27,15 @@
 
 #include "gnkstats.cuh"
 #include "hd.cuh"
+#include "../../include/elfi_b200.h"
 #include "leafsum.cuh"
 #include "treesum.cuh"
 
 namespace elfi {
 
-constexpr int BDM_N_MAX = 1024;       // a count stays below N + 2 <= 2^16 (uint16 in shared memory)
-constexpr int BDM_NSUMM = 2;          // T1, T2
+// a count stays below N + 2 <= 2^16 (uint16 in shared memory)
+constexpr int BDM_N_MAX = ELFI_B200_BDM_N_MAX;
+constexpr int BDM_NSUMM = ELFI_B200_BDM_NSUMM;          // T1, T2
 constexpr int BDM_PW_DEPTH = 4;       // TreeSum<4> sums up to 1928 terms in NumPy's order
 
 // The state of one row between events; the counts are c[j * stride] in the caller's storage.

@@ -22,7 +22,7 @@ namespace elfi {
 
 constexpr uint32_t SALT_BSL = 0x4253434cu;   // "BSCL"
 constexpr int BSL_THREADS = 128;
-constexpr int64_t BSL_MAX_CHAINS = int64_t(1) << 22;
+constexpr int64_t BSL_MAX_CHAINS = ELFI_B200_BSL_MAX_CHAINS;
 constexpr int BSL_TRI = PRIOR_MAX_PARAMS * (PRIOR_MAX_PARAMS + 1) / 2;
 
 // logit kinds of a parameter, by which of its bounds (a, b) are finite

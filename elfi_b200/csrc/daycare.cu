@@ -165,8 +165,8 @@ int elfi_b200_sim_daycare_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, 
                               void* stream_) {
     using namespace elfi;
     ELFI_REQUIRE(ctx && (B == 0 || (P && freq && K)), "sim_daycare: NULL argument");
-    ELFI_REQUIRE(B >= 0 && B <= 0x7fffffff && ldP >= 3 && n_dcc >= 1 && n_dcc <= DC_DCC_MAX &&
-                     n_ind >= 2 && n_ind <= DC_IND_MAX && n_strains >= 1 &&
+    ELFI_REQUIRE(B >= 0 && B <= ELFI_B200_DC_BATCH_MAX && ldP >= 3 && n_dcc >= 1 &&
+                     n_dcc <= DC_DCC_MAX && n_ind >= 2 && n_ind <= DC_IND_MAX && n_strains >= 1 &&
                      n_strains <= DC_STRAINS_MAX && n_obs >= 1 && n_obs <= n_ind &&
                      (!S || ldS >= DC_NSUMM * n_dcc),
                  "sim_daycare: bad shape (1 <= n_dcc <= %d, 2 <= n_ind <= %d, 1 <= n_strains <= "
@@ -206,8 +206,8 @@ int elfi_b200_daycare_summaries_f64(elfi_b200_ctx* ctx, const uint8_t* X, int64_
                                     int64_t ldS, void* stream_) {
     using namespace elfi;
     ELFI_REQUIRE(ctx && (B == 0 || (X && S)), "daycare_summaries: NULL argument");
-    ELFI_REQUIRE(B >= 0 && n_dcc >= 1 && n_obs >= 1 && n_strains >= 1 && n_strains <= 64 &&
-                     ldS >= DC_NSUMM * n_dcc,
+    ELFI_REQUIRE(B >= 0 && n_dcc >= 1 && n_obs >= 1 && n_strains >= 1 &&
+                     n_strains <= ELFI_B200_DC_SUMM_STRAINS_MAX && ldS >= DC_NSUMM * n_dcc,
                  "daycare_summaries: bad shape (n_dcc, n_obs >= 1, 1 <= n_strains <= 64, "
                  "ldS >= 4 n_dcc; n_dcc=%lld n_obs=%lld n_strains=%lld ldS=%lld)",
                  (long long)n_dcc, (long long)n_obs, (long long)n_strains, (long long)ldS);

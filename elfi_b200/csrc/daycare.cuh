@@ -28,15 +28,18 @@
 #include <stdint.h>
 
 #include "hd.cuh"
+#include "../../include/elfi_b200.h"
 #include "lotka_volterra.cuh"   // lv_leaf_sum: NumPy's pairwise order for <= 128 terms
 
 namespace elfi {
 
-constexpr int DC_DCC_MAX = 32;        // one lane per DCC
-constexpr int DC_IND_MAX = 64;        // num_s * 64 stays within int64 for n_strains <= 40
-constexpr int DC_STRAINS_MAX = 40;    // lcm(1 .. 40) = 5.3e15 < 2^53
-constexpr int DC_NSUMM = 4;           // Shannon, n_strains, prevalence, multi
-constexpr int DC_DIST_TERMS_MAX = 128;   // n_ss * n_dcc of the distance (one pairwise leaf)
+constexpr int DC_DCC_MAX = ELFI_B200_DC_DCC_MAX;        // one lane per DCC
+// num_s * 64 stays within int64 for n_strains <= 40
+constexpr int DC_IND_MAX = ELFI_B200_DC_IND_MAX;
+constexpr int DC_STRAINS_MAX = ELFI_B200_DC_STRAINS_MAX;    // lcm(1 .. 40) = 5.3e15 < 2^53
+constexpr int DC_NSUMM = ELFI_B200_DC_NSUMM;           // Shannon, n_strains, prevalence, multi
+// n_ss * n_dcc of the distance (one pairwise leaf)
+constexpr int DC_DIST_TERMS_MAX = ELFI_B200_DC_DIST_TERMS_MAX;
 constexpr double DC_EVENTS_MAX = 4294967295.0;   // transitions per row: the stream's event word
 
 ELFI_HD int dc_popc(uint64_t m) {

@@ -23,8 +23,9 @@ namespace elfi {
 
 constexpr uint32_t SALT_SIM_GNK = 0x474e4b30u;     // sim_gnk_kernel's stream (simulate.cu)
 constexpr uint32_t SALT_SIM_BIGNK = 0x42474e4bu;   // one block per (row, observation)
-constexpr int GNK_REGS_MAX = 512;                  // 32 lanes x 16 keys
-constexpr int GNK_SERIES_MAX = 2048;
+constexpr int GNK_REGS_MAX = ELFI_B200_GNK_FUSED_MAX;
+static_assert(GNK_REGS_MAX == 32 * 16, "the register sort holds 32 lanes x 16 keys");
+constexpr int GNK_SERIES_MAX = ELFI_B200_GNK_SERIES_MAX;
 
 // sort one series held in registers, then lane 0 writes its summary to out[j * step]
 template <int KPL>

@@ -22,11 +22,11 @@
 
 namespace elfi {
 
-constexpr int LR_D_MAX = 160;
+constexpr int LR_D_MAX = ELFI_B200_LOGREG_D_MAX;
 constexpr int LR_THREADS = 256;
 constexpr int LR_WARPS = LR_THREADS / 32;
 constexpr int LR_TILE = 32;
-constexpr int LR_HEAD = 8;              // header doubles of the result block
+constexpr int LR_HEAD = ELFI_B200_LOGREG_HEAD;   // header doubles of the result block
 constexpr int LR_MAX_SWEEPS = 1000;     // coordinate-descent sweeps per Newton step
 constexpr int LR_MAX_HALVINGS = 40;     // line-search step halvings
 constexpr double LR_ARMIJO = 0.01;      // sufficient-decrease fraction of the predicted decrease

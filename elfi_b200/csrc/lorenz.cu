@@ -35,9 +35,9 @@
 namespace elfi {
 
 constexpr uint32_t SALT_LORENZ = 0x4c4f525au;   // "LORZ"
-constexpr int LORENZ_M_MIN = 4;
-constexpr int LORENZ_M_MAX = 128;
-constexpr int64_t LORENZ_T_MAX = int64_t(1) << 26;   // s << 6 fits the 32-bit block word
+constexpr int LORENZ_M_MIN = ELFI_B200_LORENZ_NOBS_MIN;
+constexpr int LORENZ_M_MAX = ELFI_B200_LORENZ_NOBS_MAX;
+constexpr int64_t LORENZ_T_MAX = ELFI_B200_LORENZ_T_MAX;   // s << 6 fits the 32-bit block word
 constexpr int LORENZ_THREADS = 128;
 constexpr int LORENZ_WARPS = LORENZ_THREADS / 32;
 constexpr int LORENZ_FUSED_BLOCKS_PER_SM = 4;
@@ -425,8 +425,8 @@ int elfi_b200_lorenz_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t 
                                    int64_t n_obs, double* S, int64_t ldS, void* stream_) {
     using namespace elfi;
     ELFI_REQUIRE(ctx && (B == 0 || (X && S)), "lorenz_summaries: NULL argument");
-    ELFI_REQUIRE(B >= 0 && n_obs >= 2 && n_obs <= LORENZ_M_MAX && n_timestep >= 2 &&
-                     n_timestep * n_obs <= LORENZ_SUMM_MAX_TERMS && ldS >= 6,
+    ELFI_REQUIRE(B >= 0 && n_obs >= ELFI_B200_LORENZ_SUMM_NOBS_MIN && n_obs <= LORENZ_M_MAX &&
+                     n_timestep >= 2 && n_timestep * n_obs <= LORENZ_SUMM_MAX_TERMS && ldS >= 6,
                  "lorenz_summaries: bad shape (2 <= n_obs <= %d, 2 <= n_timestep, n_timestep * "
                  "n_obs <= %lld; n_timestep=%lld n_obs=%lld)",
                  LORENZ_M_MAX, (long long)LORENZ_SUMM_MAX_TERMS, (long long)n_timestep,

@@ -20,6 +20,7 @@
 #include <stdint.h>
 
 #include "hd.cuh"
+#include "../../include/elfi_b200.h"
 #include "leafsum.cuh"
 
 namespace elfi {
@@ -27,7 +28,9 @@ namespace elfi {
 constexpr int LORENZ_SUMM_MAXD = 8;   // open splits of PairwiseLeaves
 // longest flattened run PairwiseLeaves takes (TreeSum's bound: a right part has up to n/2 + 7
 // terms); the summaries need n_timestep * n_obs <= this
-constexpr int64_t LORENZ_SUMM_MAX_TERMS = (int64_t(120) << LORENZ_SUMM_MAXD) + 8;
+constexpr int64_t LORENZ_SUMM_MAX_TERMS = ELFI_B200_LORENZ_SUMM_MAX_TERMS;
+static_assert(LORENZ_SUMM_MAX_TERMS == (int64_t(120) << LORENZ_SUMM_MAXD) + 8,
+              "the summaries' bound is the longest run PairwiseLeaves takes");
 
 ELFI_HD double lorenz_div(double a, double b) {
 #if defined(__CUDA_ARCH__)

@@ -165,7 +165,7 @@ int elfi_b200_sim_lotka_volterra_f64(elfi_b200_ctx* ctx, const double* P, int64_
                  "ldP=%lld)", LV_NOBS_MAX, (long long)B, (long long)n_obs, (long long)ldP);
     ELFI_REQUIRE(time_end > 0.0 && time_end < INFINITY,
                  "sim_lotka_volterra: time_end must be finite and > 0");
-    ELFI_REQUIRE(max_events >= 1 && max_events <= int64_t(0xffffffffu),
+    ELFI_REQUIRE(max_events >= 1 && max_events <= ELFI_B200_LV_MAX_EVENTS_LIMIT,
                  "sim_lotka_volterra: 1 <= max_events <= 2^32 - 1 (the event is one Philox word), "
                  "got %lld", (long long)max_events);
     if (B == 0) return ELFI_B200_OK;

@@ -32,14 +32,18 @@
 #include <stdint.h>
 
 #include "hd.cuh"
+#include "../../include/elfi_b200.h"
 #include "gnkstats.cuh"
 
 namespace elfi {
 
-constexpr int LV_NOBS_MAX = 1024;          // observation times staged in shared memory
-constexpr int LV_SUMM_NOBS_MIN = 3;        // the lag-2 autocorrelation needs one product
-constexpr int LV_SUMM_NOBS_MAX = 128;      // one leaf of NumPy's pairwise sum (LEAF_MAX_TERMS)
-constexpr int LV_NSUMM = 9;
+// observation times staged in shared memory
+constexpr int LV_NOBS_MAX = ELFI_B200_LV_NOBS_MAX;
+// the lag-2 autocorrelation needs one product
+constexpr int LV_SUMM_NOBS_MIN = ELFI_B200_LV_SUMM_NOBS_MIN;
+// one leaf of NumPy's pairwise sum (LEAF_MAX_TERMS)
+constexpr int LV_SUMM_NOBS_MAX = ELFI_B200_LV_SUMM_NOBS_MAX;
+constexpr int LV_NSUMM = ELFI_B200_LV_NSUMM;
 constexpr double LV_INT32_LOW = -2147483649.0;   // the open interval of doubles whose truncation
 constexpr double LV_INT32_HIGH = 2147483648.0;   // fits int32
 

@@ -23,14 +23,16 @@
 #include <stdint.h>
 
 #include "hd.cuh"
+#include "../../include/elfi_b200.h"
 #include "gnkstats.cuh"
 #include "toad.cuh"
 
 namespace elfi {
 
-constexpr int MG1_NOBS_MIN = 2;
-constexpr int MG1_NOBS_MAX = 512;   // one warp sorts a row in registers (32 lanes x 16 keys)
-constexpr int MG1_NQ_MAX = 32;      // one quantile per lane
+constexpr int MG1_NOBS_MIN = ELFI_B200_MG1_NOBS_MIN;
+// one warp sorts a row in registers (32 lanes x 16 keys)
+constexpr int MG1_NOBS_MAX = ELFI_B200_MG1_NOBS_MAX;
+constexpr int MG1_NQ_MAX = ELFI_B200_MG1_NQ_MAX;      // one quantile per lane
 
 // false where the reference raises: the row is NaN
 ELFI_HD bool mg1_params_ok(double inv_t3, double range) {

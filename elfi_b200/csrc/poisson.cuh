@@ -36,10 +36,11 @@
 #include "philox.cuh"
 
 #include "hd.cuh"
+#include "../../include/elfi_b200.h"
 
 namespace elfi {
 
-constexpr double POISSON_LAM_MAX = 9.223372006484771e18;   // NumPy's POISSON_LAM_MAX
+constexpr double POISSON_LAM_MAX = ELFI_B200_POISSON_LAM_MAX;   // NumPy's POISSON_LAM_MAX
 constexpr double POISSON_SWITCH = 10.0;                    // inversion below, PTRS at and above
 constexpr int POISSON_INV_MAX = 64;
 constexpr int POISSON_MAX_TRIALS = 32;

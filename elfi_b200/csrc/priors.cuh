@@ -36,14 +36,17 @@
 #include <stdio.h>
 
 #include "hd.cuh"
+#include "../../include/elfi_b200.h"
 
 namespace elfi {
 
 enum PriorKind { PRIOR_UNIFORM = 0, PRIOR_NORM = 1, PRIOR_TRUNCNORM = 2, PRIOR_EXPON = 3,
                  PRIOR_GAMMA = 4, PRIOR_BETA = 5 };
-constexpr int PRIOR_SPEC_WORDS = 5;      // [kind, p0, p1, p2, p3] per parameter
-constexpr int PRIOR_COND_SPEC_WORDS = 7; // [kind, p0, p1, p2, p3, loc_src, scale_src]
-constexpr int PRIOR_MAX_PARAMS = 16;
+// [kind, p0, p1, p2, p3] per parameter
+constexpr int PRIOR_SPEC_WORDS = ELFI_B200_PRIOR_SPEC_WORDS;
+// [kind, p0, p1, p2, p3, loc_src, scale_src]
+constexpr int PRIOR_COND_SPEC_WORDS = ELFI_B200_PRIOR_COND_SPEC_WORDS;
+constexpr int PRIOR_MAX_PARAMS = ELFI_B200_MAX_PRIOR_PARAMS;
 constexpr int PRIOR_MAX_TRIALS = 64;     // Marsaglia-Tsang trials per gamma component
 constexpr double PRIOR_NORM_LOGC = 0.91893853320467274178;   // log(sqrt(2 pi))
 

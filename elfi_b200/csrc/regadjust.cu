@@ -28,7 +28,7 @@
 
 namespace elfi {
 
-constexpr int RA_D_MAX = 256;
+constexpr int RA_D_MAX = ELFI_B200_REGADJ_D_MAX;
 constexpr int RA_THREADS = 256;
 constexpr int RA_TILE = 64;                  // lower tiles of the cross-product
 constexpr int RA_SLAB = 32;                  // rows staged in shared memory per step
@@ -336,7 +336,7 @@ static int ra_group_args(const double* S, int64_t ldS, int64_t N, int64_t q, con
                          const double* T, int64_t ldT, int64_t p, const uint8_t* flags,
                          const int32_t* cols_host, int64_t pg, int64_t sel, const char* who) {
     ELFI_REQUIRE(S && obs && T && flags && cols_host, "%s: NULL argument", who);
-    ELFI_REQUIRE(q >= 1 && p >= 1 && q + p <= RA_D_MAX && N >= 1 && N < (int64_t(1) << 31) &&
+    ELFI_REQUIRE(q >= 1 && p >= 1 && q + p <= RA_D_MAX && N >= 1 && N <= ELFI_B200_REGADJ_N_MAX &&
                      ldS >= q && ldT >= p,
                  "%s: bad shape (q, p >= 1, q + p <= %d, 1 <= N < 2^31, ldS >= q, ldT >= p; "
                  "N=%lld q=%lld p=%lld ldS=%lld ldT=%lld)", who, RA_D_MAX, (long long)N,
@@ -360,7 +360,7 @@ int elfi_b200_regadj_mask_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, 
                               uint8_t* flags, int64_t* counts, void* stream_) {
     using namespace elfi;
     ELFI_REQUIRE(ctx && S && obs && T && flags && counts, "regadj_mask: NULL argument");
-    ELFI_REQUIRE(q >= 1 && p >= 1 && q + p <= RA_D_MAX && N >= 1 && N < (int64_t(1) << 31) &&
+    ELFI_REQUIRE(q >= 1 && p >= 1 && q + p <= RA_D_MAX && N >= 1 && N <= ELFI_B200_REGADJ_N_MAX &&
                      ldS >= q && ldT >= p,
                  "regadj_mask: bad shape (q, p >= 1, q + p <= %d, 1 <= N < 2^31, ldS >= q, "
                  "ldT >= p; N=%lld q=%lld p=%lld ldS=%lld ldT=%lld)", RA_D_MAX, (long long)N,

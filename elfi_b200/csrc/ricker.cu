@@ -30,9 +30,11 @@ namespace elfi {
 
 constexpr uint32_t SALT_POISSON = 0x504f4953u;   // "POIS"
 constexpr uint32_t SALT_RICKER = 0x5249434bu;    // "RICK"
-constexpr int RICKER_FUSED_MAX = 128;            // LEAF_MAX_TERMS
+constexpr int RICKER_FUSED_MAX = ELFI_B200_RICKER_FUSED_MAX;
+static_assert(RICKER_FUSED_MAX == LEAF_MAX_TERMS, "the fused summaries sum one pairwise leaf");
 constexpr int RICKER_THREADS = 128;
-constexpr int64_t RICKER_NOBS_MAX = int64_t(1) << 24;   // t << 8 fits the 32-bit block word
+// t << 8 fits the 32-bit block word
+constexpr int64_t RICKER_NOBS_MAX = ELFI_B200_RICKER_NOBS_MAX;
 
 __global__ void __launch_bounds__(256)
 poisson_kernel(const double* __restrict__ lam, int64_t n, uint64_t seed, uint64_t offset,

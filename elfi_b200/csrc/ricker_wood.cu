@@ -26,9 +26,10 @@
 
 namespace elfi {
 
-constexpr int WOOD_NOBS_MIN = 7;
-constexpr int WOOD_NOBS_MAX = 2048;   // the shared-memory sort of gnk_summaries has the same bound
-constexpr int WOOD_WIDTH = 13;
+constexpr int WOOD_NOBS_MIN = ELFI_B200_RICKER_WOOD_NOBS_MIN;
+// the shared-memory sort of gnk_summaries has the same bound
+constexpr int WOOD_NOBS_MAX = ELFI_B200_RICKER_WOOD_NOBS_MAX;
+constexpr int WOOD_WIDTH = ELFI_B200_RICKER_WOOD_WIDTH;
 constexpr int WOOD_WARPS = 4;
 constexpr int WOOD_LAGS = 6;          // autocovariances at lags 0 .. 5
 constexpr int WOOD_SLOTS = 16;        // per-warp result slots (13 used)

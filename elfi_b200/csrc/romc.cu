@@ -13,11 +13,12 @@
 
 namespace elfi {
 
-constexpr int ROMC_MAX_P = 16;
+constexpr int ROMC_MAX_P = ELFI_B200_ROMC_MAX_P;
 constexpr int ROMC_THREADS = 128;
 constexpr uint32_t ROMC_SALT = 0x524f4d43u;   // "ROMC": the fourth counter word of the box draws
 
 enum { NM_INIT = 0, NM_REFLECT, NM_EXPAND, NM_CONTRACT_OUT, NM_CONTRACT_IN, NM_SHRINK, NM_DONE };
+static_assert(NM_DONE == ELFI_B200_ROMC_NM_DONE, "the header states a finished problem's code");
 
 __host__ __device__ constexpr int64_t nm_state_size(int64_t N) { return (N + 1) * (N + 1) + 3 * N + 2; }
 

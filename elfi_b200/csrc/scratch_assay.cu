@@ -185,9 +185,10 @@ int elfi_b200_sim_scratch_assay_f64(elfi_b200_ctx* ctx, const double* P, int64_t
                                     void* stream_) {
     using namespace elfi;
     ELFI_REQUIRE(ctx && (B == 0 || (P && init)), "sim_scratch_assay: NULL argument");
-    ELFI_REQUIRE(B >= 0 && B <= 0x7fffffff && ldP >= SA_NPARAMS && nrows >= 1 && ncols >= 1 &&
-                     nrows <= SA_SITES_MAX && ncols <= SA_SITES_MAX &&
-                     nrows * ncols <= SA_SITES_MAX && num_iter >= 0 && num_iter <= 0x7fffffff &&
+    ELFI_REQUIRE(B >= 0 && B <= ELFI_B200_SA_BATCH_MAX && ldP >= SA_NPARAMS && nrows >= 1 &&
+                     ncols >= 1 && nrows <= SA_SITES_MAX && ncols <= SA_SITES_MAX &&
+                     nrows * ncols <= SA_SITES_MAX && num_iter >= 0 &&
+                     num_iter <= ELFI_B200_SA_ITER_MAX &&
                      obs_interval >= 1 && (S == nullptr || ldS >= num_iter / obs_interval + 1),
                  "sim_scratch_assay: bad shape (1 <= nrows * ncols <= %d, 0 <= num_iter < 2^31, "
                  "obs_interval >= 1, ldS >= num_iter / obs_interval + 1, B < 2^31; B=%lld "

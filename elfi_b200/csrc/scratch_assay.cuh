@@ -39,13 +39,15 @@
 #include <stdint.h>
 
 #include "hd.cuh"
+#include "../../include/elfi_b200.h"
 #include "leafsum.cuh"
 #include "philox.cuh"
 
 namespace elfi {
 
 constexpr uint32_t SALT_SCRATCH = 0x53434131u;   // "SCA1"; slot s adds s (s < SA_SITES_MAX)
-constexpr int SA_SITES_MAX = 4096;               // lattice sites: list entries fit uint16
+// lattice sites: list entries fit uint16
+constexpr int SA_SITES_MAX = ELFI_B200_SA_SITES_MAX;
 constexpr int SA_WORDS_MAX = SA_SITES_MAX / 32;
 constexpr int SA_NPARAMS = 2;                    // pm, pp
 

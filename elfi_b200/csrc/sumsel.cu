@@ -13,7 +13,7 @@ namespace elfi {
 // ---- all-combination distances ------------------------------------------------------------------
 constexpr int SS_ROWS = 32;        // rows staged per CTA: one per lane
 constexpr int SS_THREADS = 256;    // 8 warps take the combinations in turn
-constexpr int SS_MAX_W = 512;
+constexpr int SS_MAX_W = ELFI_B200_SUBSET_MAX_WIDTH;
 
 // Rows are staged at an odd stride (W | 1 doubles), so the 32 lanes of a warp, each reading
 // column j of its own row, hit different banks; obs[j] is one broadcast.
@@ -69,8 +69,8 @@ static int launch_subset_distance(elfi_b200_ctx* ctx, const double* S, int64_t l
 // ---- k-th nearest neighbour radii ----------------------------------------------------------------
 constexpr int KN_QUERIES = 128;    // query points (threads) per CTA
 constexpr int KN_TILE = 256;       // set points per shared tile
-constexpr int KN_MAX_Q = 16;
-constexpr int KN_MAX_K = 32;
+constexpr int KN_MAX_Q = ELFI_B200_KNN_MAX_Q;
+constexpr int KN_MAX_K = ELFI_B200_KNN_MAX_K;
 constexpr int RED_THREADS = 256;
 
 // best[] holds the KMAX smallest values seen, ascending.  Only the top k slots take part: the
@@ -177,7 +177,7 @@ int elfi_b200_subset_distance_f64(elfi_b200_ctx* ctx, int32_t metric, const doub
     ELFI_REQUIRE(ctx && obs && ranges && comb && d_out && (B == 0 || S),
                  "subset_distance: NULL argument");
     ELFI_REQUIRE(W >= 1 && W <= SS_MAX_W && ldS >= W && B >= 0 && B < (int64_t(1) << 31) &&
-                     C >= 1 && C < (int64_t(1) << 24) && ld_out >= B,
+                     C >= 1 && C <= ELFI_B200_SUBSET_MAX_COMBINATIONS && ld_out >= B,
                  "subset_distance: bad shape (1 <= W <= %d, ldS >= W, 0 <= B < 2^31, "
                  "1 <= C < 2^24, ld_out >= B; W=%lld ldS=%lld B=%lld C=%lld ld_out=%lld)",
                  SS_MAX_W, (long long)W, (long long)ldS, (long long)B, (long long)C,
@@ -211,7 +211,7 @@ int elfi_b200_knn_entropy_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, 
     using namespace elfi;
     ELFI_REQUIRE(ctx && X && R && logsum, "knn_entropy: NULL argument");
     ELFI_REQUIRE(q >= 1 && q <= KN_MAX_Q && ldX >= q && k >= 1 && k <= KN_MAX_K && n >= 1 &&
-                     n <= (int64_t(1) << 20) && C >= 1 && C < (int64_t(1) << 16),
+                     n <= ELFI_B200_KNN_MAX_N && C >= 1 && C <= ELFI_B200_KNN_MAX_SETS,
                  "knn_entropy: bad shape (1 <= q <= %d, ldX >= q, 1 <= k <= %d, 1 <= n <= 2^20, "
                  "1 <= C < 2^16; q=%lld ldX=%lld k=%lld n=%lld C=%lld)", KN_MAX_Q, KN_MAX_K,
                  (long long)q, (long long)ldX, (long long)k, (long long)n, (long long)C);

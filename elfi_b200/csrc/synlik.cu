@@ -26,7 +26,7 @@
 
 namespace elfi {
 
-constexpr int SL_D_MAX = 160;
+constexpr int SL_D_MAX = ELFI_B200_SYNLIK_D_MAX;
 constexpr int SL_TILE = 32;
 constexpr int SL_CHUNK = 256;          // rows of one chunk sum: fixes the summation order
 constexpr int SL_THREADS = 256;

@@ -23,16 +23,19 @@
 #include <stdint.h>
 
 #include "hd.cuh"
+#include "../../include/elfi_b200.h"
 #include "gnkstats.cuh"
 #include "stable.cuh"
 
 namespace elfi {
 
-constexpr int TOAD_DISP_MAX = 4096;        // displacements of one lag: n_toads * (n_days - lag)
-constexpr int TOAD_NP_MAX = 32;            // quantile levels
-constexpr int TOAD_LAGS_MAX = 8;           // lags of the fused summaries
+// displacements of one lag: n_toads * (n_days - lag)
+constexpr int TOAD_DISP_MAX = ELFI_B200_TOAD_DISP_MAX;
+constexpr int TOAD_NP_MAX = ELFI_B200_TOAD_NP_MAX;            // quantile levels
+constexpr int TOAD_LAGS_MAX = ELFI_B200_TOAD_LAGS_MAX;           // lags of the fused summaries
 constexpr int TOAD_MEDIAN_SMALL = 600;     // below: np.ma.median; from here: np.median
-constexpr int64_t TOAD_CELLS_MAX = int64_t(1) << 31;   // n_days * n_toads: (cell << 1) | h < 2^32
+// n_days * n_toads: (cell << 1) | h < 2^32
+constexpr int64_t TOAD_CELLS_MAX = ELFI_B200_TOAD_CELLS_MAX;
 constexpr double TOAD_GAP_FLOOR = 0x1.1b48655f37267p-29;   // np.exp(-20)
 
 ELFI_HD double toad_log(double x) { return log(x); }

@@ -11,7 +11,7 @@ import torch
 from . import _lib
 from . import device as dev
 
-MAX_NESTED = 32
+MAX_NESTED = _lib.CONSTANTS['MAX_NESTED']
 
 
 def _matrix(S):
@@ -204,7 +204,10 @@ def dist_euclid(S, obs, w=None, thresholds=None, want_indices=True, sync=True, m
     return (d, acc_idx, mom) if moments else (d, acc_idx)
 
 
-METRIC_CODES = {'sqeuclidean': 1, 'cityblock': 2, 'chebyshev': 3, 'minkowski': 4}
+# the header's ELFI_B200_METRIC_<NAME> codes by value: name -> code
+_METRICS = {k[len('METRIC_'):].lower(): v for k, v in sorted(
+    _lib.CONSTANTS.items(), key=lambda kv: kv[1]) if k.startswith('METRIC_')}
+METRIC_CODES = {k: v for k, v in _METRICS.items() if k != 'euclidean'}
 
 
 def dist_metric(S, obs, metric, p=2.0, threshold=None, want_indices=True):
@@ -766,9 +769,9 @@ def gm_rvs(means, cov, weights, size, seed, offset=0, support=0, box=None, cdf=N
 PRIOR_KINDS = ('uniform', 'norm', 'truncnorm', 'expon', 'gamma', 'beta')
 PRIOR_SHAPES = {'uniform': (), 'norm': (), 'truncnorm': ('a', 'b'), 'expon': (), 'gamma': ('a',),
                 'beta': ('a', 'b')}
-MAX_PRIOR_PARAMS = 16
-PRIOR_SPEC_WORDS = 5
-PRIOR_COND_SPEC_WORDS = 7      # [kind, p0, p1, p2, p3, loc_src, scale_src]
+MAX_PRIOR_PARAMS = _lib.CONSTANTS['MAX_PRIOR_PARAMS']
+PRIOR_SPEC_WORDS = _lib.CONSTANTS['PRIOR_SPEC_WORDS']
+PRIOR_COND_SPEC_WORDS = _lib.CONSTANTS['PRIOR_COND_SPEC_WORDS']
 
 
 def _prior_spec_error(spec, loc_src=-1, scale_src=-1):
@@ -971,8 +974,8 @@ def rowsort(x):
 # ---- robust / octile g-and-k summaries (elfi/examples/gnk.py:164-248, bignk.py) ------------------
 GNK_KINDS = {'ss_robust': 0, 'ss_octile': 1}
 GNK_WIDTH = {'ss_robust': 4, 'ss_octile': 7}
-GNK_SERIES_MAX = 2048     # series length of gnk_summaries (the shared-memory sort)
-GNK_FUSED_MAX = 512       # n_obs of the fused simulators (the register sort)
+GNK_SERIES_MAX = _lib.CONSTANTS['GNK_SERIES_MAX']
+GNK_FUSED_MAX = _lib.CONSTANTS['GNK_FUSED_MAX']
 _GNK_OCTILES = np.linspace(12.5, 87.5, 7)
 
 
@@ -1097,9 +1100,9 @@ def euclidean_multiss(S, obs):
 
 
 # ---- Ricker model (elfi/examples/ricker.py) -------------------------------------------------------
-POISSON_LAM_MAX = 9.223372006484771e18   # NumPy's limit; larger rates give NaN
-RICKER_FUSED_MAX = 128    # n_obs of the fused summaries (one leaf of NumPy's pairwise sum)
-RICKER_NOBS_MAX = 1 << 24
+POISSON_LAM_MAX = _lib.CONSTANTS['POISSON_LAM_MAX']
+RICKER_FUSED_MAX = _lib.CONSTANTS['RICKER_FUSED_MAX']
+RICKER_NOBS_MAX = _lib.CONSTANTS['RICKER_NOBS_MAX']
 
 
 def poisson(lam, seed, offset=0):
@@ -1195,8 +1198,9 @@ def chi_squared(S, obs):
     return out
 
 
-RICKER_WOOD_NOBS_MIN, RICKER_WOOD_NOBS_MAX = 7, 2048   # the shared-memory sort of the differences
-RICKER_WOOD_WIDTH = 13
+RICKER_WOOD_NOBS_MIN = _lib.CONSTANTS['RICKER_WOOD_NOBS_MIN']
+RICKER_WOOD_NOBS_MAX = _lib.CONSTANTS['RICKER_WOOD_NOBS_MAX']
+RICKER_WOOD_WIDTH = _lib.CONSTANTS['RICKER_WOOD_WIDTH']
 
 
 def wood_summaries(y, design):
@@ -1220,10 +1224,11 @@ def wood_summaries(y, design):
 
 
 # ---- Lorenz forecast model (elfi/examples/lorenz.py) ----------------------------------------------
-LORENZ_NOBS_MIN, LORENZ_NOBS_MAX = 4, 128     # variables of the ring on the device
-LORENZ_SUMM_NOBS_MIN = 2     # one variable: NumPy sums over time pairwise, not row by row
-LORENZ_T_MAX = 1 << 26                        # n_timestep of the simulator (the stream's step word)
-LORENZ_SUMM_MAX_TERMS = 30728                 # n_timestep * n_obs of the summaries
+LORENZ_NOBS_MIN = _lib.CONSTANTS['LORENZ_NOBS_MIN']
+LORENZ_NOBS_MAX = _lib.CONSTANTS['LORENZ_NOBS_MAX']
+LORENZ_SUMM_NOBS_MIN = _lib.CONSTANTS['LORENZ_SUMM_NOBS_MIN']
+LORENZ_T_MAX = _lib.CONSTANTS['LORENZ_T_MAX']
+LORENZ_SUMM_MAX_TERMS = _lib.CONSTANTS['LORENZ_SUMM_MAX_TERMS']
 LORENZ_NSUMM = 6
 
 
@@ -1288,10 +1293,10 @@ def lorenz_summaries(x):
 
 
 # ---- Toad movement model (elfi/examples/toad.py) --------------------------------------------------
-TOAD_DISP_MAX = 4096          # displacements of one lag, n_toads * (n_days - lag), sorted per CTA
-TOAD_LAGS_MAX = 8             # lags of the fused summaries
-TOAD_NP_MAX = 32              # quantile levels
-TOAD_CELLS_MAX = 1 << 31      # n_days * n_toads (the stream's block word)
+TOAD_DISP_MAX = _lib.CONSTANTS['TOAD_DISP_MAX']
+TOAD_LAGS_MAX = _lib.CONSTANTS['TOAD_LAGS_MAX']
+TOAD_NP_MAX = _lib.CONSTANTS['TOAD_NP_MAX']
+TOAD_CELLS_MAX = _lib.CONSTANTS['TOAD_CELLS_MAX']
 
 
 def _toad_p(p):
@@ -1373,11 +1378,11 @@ def toad_summaries(x, lag, p=np.linspace(0, 1, 11), thd=10.):
 
 
 # ---- Lotka-Volterra model (elfi/examples/lotka_volterra.py) ----------------------------------------
-LV_NOBS_MAX = 1024            # observation times staged in shared memory
-LV_SUMM_NOBS_MIN = 3          # the lag-2 autocorrelation needs one product
-LV_SUMM_NOBS_MAX = 128        # one leaf of NumPy's pairwise sum
-LV_NSUMM = 9
-LV_MAX_EVENTS_LIMIT = 2 ** 32 - 1   # the event index is one 32-bit Philox word
+LV_NOBS_MAX = _lib.CONSTANTS['LV_NOBS_MAX']
+LV_SUMM_NOBS_MIN = _lib.CONSTANTS['LV_SUMM_NOBS_MIN']
+LV_SUMM_NOBS_MAX = _lib.CONSTANTS['LV_SUMM_NOBS_MAX']
+LV_NSUMM = _lib.CONSTANTS['LV_NSUMM']
+LV_MAX_EVENTS_LIMIT = _lib.CONSTANTS['LV_MAX_EVENTS_LIMIT']
 
 
 def sim_lotka_volterra(params, n_obs=16, time_end=30., seed=0, offset=0, max_events=2 ** 20):
@@ -1432,10 +1437,10 @@ def lv_summaries(x):
 
 
 # ---- birth-death-mutation model (elfi/examples/bdm.py) ----------------------------------------
-BDM_N_MAX = 1024              # cluster counts per lane in shared memory as uint16
-BDM_NSUMM = 2                 # T1, T2
-BDM_MAX_EVENTS_LIMIT = 2 ** 32 - 1   # the event index is one 32-bit Philox word
-BDM_BATCH_MAX = 2 ** 31 - 1
+BDM_N_MAX = _lib.CONSTANTS['BDM_N_MAX']
+BDM_NSUMM = _lib.CONSTANTS['BDM_NSUMM']
+BDM_MAX_EVENTS_LIMIT = _lib.CONSTANTS['BDM_MAX_EVENTS_LIMIT']
+BDM_BATCH_MAX = _lib.CONSTANTS['BDM_BATCH_MAX']
 
 
 def _bdm_N(N):
@@ -1499,13 +1504,13 @@ def bdm_summaries(x, n=20):
 
 
 # ---- day care model (elfi/examples/daycare.py) ----------------------------------------------------
-DC_DCC_MAX = 32               # one lane per DCC
-DC_IND_MAX = 64               # the numerators of E_s stay within int64
-DC_STRAINS_MAX = 40           # lcm(1 .. n_strains) < 2^53
-DC_SUMM_STRAINS_MAX = 64      # one 64-bit strain mask per child
-DC_NSUMM = 4                  # Shannon, n_strains, prevalence, multi
-DC_DIST_TERMS_MAX = 128       # n_ss * n_dcc of the distance: one leaf of NumPy's pairwise sum
-DC_BATCH_MAX = 2 ** 31 - 1    # one CTA per row
+DC_DCC_MAX = _lib.CONSTANTS['DC_DCC_MAX']
+DC_IND_MAX = _lib.CONSTANTS['DC_IND_MAX']
+DC_STRAINS_MAX = _lib.CONSTANTS['DC_STRAINS_MAX']
+DC_SUMM_STRAINS_MAX = _lib.CONSTANTS['DC_SUMM_STRAINS_MAX']
+DC_NSUMM = _lib.CONSTANTS['DC_NSUMM']
+DC_DIST_TERMS_MAX = _lib.CONSTANTS['DC_DIST_TERMS_MAX']
+DC_BATCH_MAX = _lib.CONSTANTS['DC_BATCH_MAX']
 
 
 def sim_daycare(params, n_dcc=29, n_ind=53, n_strains=33, freq_strains_commun=None, n_obs=36,
@@ -1614,8 +1619,9 @@ def daycare_distance(S, observed, n_dcc):
 
 
 # ---- ARCH(1) model (elfi/examples/arch.py) --------------------------------------------------------
-ARCH_NOBS_MIN, ARCH_NOBS_MAX = 2, 128   # one leaf of NumPy's pairwise sum per reduction
-ARCH_LAGS_MAX = 8
+ARCH_NOBS_MIN = _lib.CONSTANTS['ARCH_NOBS_MIN']
+ARCH_NOBS_MAX = _lib.CONSTANTS['ARCH_NOBS_MAX']
+ARCH_LAGS_MAX = _lib.CONSTANTS['ARCH_LAGS_MAX']
 
 
 def arch_nsumm(n_lags):
@@ -1668,8 +1674,8 @@ def arch_summaries(y, n_lags=5):
 
 
 # ---- AR(1) model (elfi/examples/ar1.py) -----------------------------------------------------------
-AR1_NOBS_MAX = 1 << 24        # observations per row
-AR1_BATCH_MAX = 2 ** 31 - 1   # accepted rows are int32 indices
+AR1_NOBS_MAX = _lib.CONSTANTS['AR1_NOBS_MAX']
+AR1_BATCH_MAX = _lib.CONSTANTS['AR1_BATCH_MAX']
 
 
 def sim_ar1(phi, n_obs=200, seed=0, offset=0, obs=None, thresholds=None, want_data=None):
@@ -1720,9 +1726,9 @@ def sim_ar1(phi, n_obs=200, seed=0, offset=0, obs=None, thresholds=None, want_da
 
 
 # ---- M/G/1 queue (elfi/examples/mg1.py) ------------------------------------------------------------
-MG1_NOBS_MIN = 2
-MG1_NOBS_MAX = 512            # a row is sorted by one warp in registers
-MG1_NQ_MAX = 32               # quantile levels
+MG1_NOBS_MIN = _lib.CONSTANTS['MG1_NOBS_MIN']
+MG1_NOBS_MAX = _lib.CONSTANTS['MG1_NOBS_MAX']
+MG1_NQ_MAX = _lib.CONSTANTS['MG1_NQ_MAX']
 
 
 def _mg1_q(q):
@@ -1815,9 +1821,9 @@ def svm_summaries(x):
 
 
 # ---- scratch assay (elfi/examples/scratch_assay.py) -----------------------------------------------
-SA_SITES_MAX = 4096            # lattice sites: the snapshot list is uint16, one warp's state in smem
-SA_ITER_MAX = 2 ** 31 - 1      # iteration counters of the Philox streams
-SA_BATCH_MAX = 2 ** 31 - 1     # one warp per row
+SA_SITES_MAX = _lib.CONSTANTS['SA_SITES_MAX']
+SA_ITER_MAX = _lib.CONSTANTS['SA_ITER_MAX']
+SA_BATCH_MAX = _lib.CONSTANTS['SA_BATCH_MAX']
 
 
 def scratch_assay_steps(obs_period=12, obs_interval=1 / 12, tau=1 / 24):
@@ -1897,7 +1903,7 @@ def scratch_assay_summaries(x):
 
 
 # ---- Bayesian synthetic likelihood (elfi/methods/bsl/pdf_methods.py) ------------------------------
-SYNLIK_D_MAX = 160             # Sigma, its factor and the right-hand side in one CTA's shared memory
+SYNLIK_D_MAX = _lib.CONSTANTS['SYNLIK_D_MAX']
 SYNLIK_ESTIMATORS = {'standard': 0, 'unbiased': 1}
 
 
@@ -1969,7 +1975,7 @@ def synlik(S, y, estimator='standard', penalties=None, whitening=None):
     return out
 
 
-BSL_MAX_CHAINS = 1 << 22
+BSL_MAX_CHAINS = _lib.CONSTANTS['BSL_MAX_CHAINS']
 
 
 def bsl_mh_tables(specs, sigma_proposals, sources=None, bounds=None):
@@ -2051,9 +2057,9 @@ def bsl_mh_step(tables, t, loglik, prop, prop_lp, chains, logpost, n_acc, rows, 
 
 
 # ---- BOLFIRE ratio-estimation classifier (elfi/methods/classifier.py) ------------------------------
-LOGREG_D_MAX = 160             # H = X~^T D X~ (packed) and the row tiles in one CTA's shared memory
+LOGREG_D_MAX = _lib.CONSTANTS['LOGREG_D_MAX']
 LOGREG_PENALTIES = {'l1': 0, 'l2': 1}
-LOGREG_HEAD = 8                # header doubles of a fit block (include/elfi_b200.h)
+LOGREG_HEAD = _lib.CONSTANTS['LOGREG_HEAD']
 LOGREG_STATUS = {1: 'converged', 0: 'not converged', -1: 'bad labels', -2: 'non-finite input'}
 
 
@@ -2200,13 +2206,13 @@ def logreg_predict(fit, X, class_min=0.0, out=None):
 
 
 # ---- summary-statistic selection (TwoStageSelection, elfi/methods/diagnostics.py) ---------------
-SUBSET_METRIC_CODES = {'euclidean': 0, 'sqeuclidean': 1, 'cityblock': 2, 'chebyshev': 3}
-SUBSET_MAX_WIDTH = 512
-SUBSET_MAX_COMBINATIONS = 2 ** 24 - 1
-KNN_MAX_Q = 16
-KNN_MAX_K = 32
-KNN_MAX_N = 2 ** 20
-KNN_MAX_SETS = 2 ** 16 - 1
+SUBSET_METRIC_CODES = {k: v for k, v in _METRICS.items() if v <= _METRICS['chebyshev']}
+SUBSET_MAX_WIDTH = _lib.CONSTANTS['SUBSET_MAX_WIDTH']
+SUBSET_MAX_COMBINATIONS = _lib.CONSTANTS['SUBSET_MAX_COMBINATIONS']
+KNN_MAX_Q = _lib.CONSTANTS['KNN_MAX_Q']
+KNN_MAX_K = _lib.CONSTANTS['KNN_MAX_K']
+KNN_MAX_N = _lib.CONSTANTS['KNN_MAX_N']
+KNN_MAX_SETS = _lib.CONSTANTS['KNN_MAX_SETS']
 
 
 class SubsetLayout:
@@ -2324,9 +2330,9 @@ def mrsse(T, P, out=None):
 
 
 # ---- robust optimisation Monte Carlo (ROMC, elfi/methods/inference/romc.py) ---------------------
-ROMC_MAX_P = 16
-ROMC_NM_INTS = 8
-ROMC_NM_DONE = 6
+ROMC_MAX_P = _lib.CONSTANTS['ROMC_MAX_P']
+ROMC_NM_INTS = _lib.CONSTANTS['ROMC_NM_INTS']
+ROMC_NM_DONE = _lib.CONSTANTS['ROMC_NM_DONE']
 
 
 def romc_nm_doubles(p):
@@ -2500,8 +2506,8 @@ def romc_posterior_unnorm(theta, prior, eps, center=None, rot_inv=None, limits=N
 
 
 # ---- regression adjustment (elfi/methods/post_processing.py: LinearAdjustment) ----------------------
-REGADJ_D_MAX = 256             # q + p: the mean and the tile rows of one group in shared memory
-REGADJ_N_MAX = 2 ** 31 - 1     # rows: int32 row ranks in the kernels' compaction
+REGADJ_D_MAX = _lib.CONSTANTS['REGADJ_D_MAX']
+REGADJ_N_MAX = _lib.CONSTANTS['REGADJ_N_MAX']
 
 
 def _regadj_shape(x):

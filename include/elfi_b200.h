@@ -458,10 +458,11 @@ int elfi_b200_gm_rvs_cdf_f64(elfi_b200_ctx* ctx, const double* means, int64_t ld
  *                               per gamma component.  If all 64 are rejected (probability below
  *                               1e-80 for every valid shape) the component's value is
  *                               d = a - 1/3 (a >= 1) or a + 2/3 (a < 1), a point of the support
- *   elfi_b200_prior_logpdf_f64  joint log density of p <= 16 independent parameters at the rows of
- *                               x (B, p; leading dimension ldx): the sum, left to right, of
- *                               scipy.stats.<kind>.logpdf, -inf outside the closed support and
- *                               scipy's values on its edges (spec_host: 5p words)
+ *   elfi_b200_prior_logpdf_f64  joint log density of p <= ELFI_B200_MAX_PRIOR_PARAMS independent
+ *                               parameters at the rows of x (B, p; leading dimension ldx): the sum,
+ *                               left to right, of scipy.stats.<kind>.logpdf, -inf outside the
+ *                               closed support and scipy's values on its edges (spec_host: 5p
+ *                               words)
  *
  * Conditional loc / scale (a hierarchical prior such as t2 ~ U(t1, t1 + 10)): the 7-word form
  * [kind, p0, p1, p2, p3, loc_src, scale_src] takes the loc and / or the scale of a parameter from
@@ -484,6 +485,9 @@ int elfi_b200_gm_rvs_cdf_f64(elfi_b200_ctx* ctx, const double* means, int64_t ld
  *   elfi_b200_gm_rvs(_cdf)_f64 with support = 4: box_host is the 7p-word table; the draws use the
  *                                    blocks of support 3, so with every source -1 they are its bits
  */
+#define ELFI_B200_MAX_PRIOR_PARAMS 16       /* parameters p of one prior table */
+#define ELFI_B200_PRIOR_SPEC_WORDS 5        /* [kind, p0, p1, p2, p3] per parameter */
+#define ELFI_B200_PRIOR_COND_SPEC_WORDS 7   /* [kind, p0, p1, p2, p3, loc_src, scale_src] */
 int elfi_b200_prior_rvs_f64(elfi_b200_ctx* ctx, const double* spec_host, int64_t B, uint64_t seed,
                             uint64_t offset, double* out, void* stream);
 int elfi_b200_prior_logpdf_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int64_t B, int64_t p,
@@ -527,17 +531,21 @@ int elfi_b200_logprior_box_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx,
  * NaN rules as NumPy's: a NaN in a series makes all its octiles NaN; an infinity at a picked
  * position with t = 0 gives NaN through (inf - a) * 0; ss_B = 0 becomes eps.
  * gnk_summaries: series (i, a) of a data matrix is X[i * ld_row + j * ld_obs + a], j < n,
- *   1 <= n <= 2048, d in {1, 2}.
+ *   1 <= n <= ELFI_B200_GNK_SERIES_MAX, d in {1, 2}.
  * sim_gnk_summaries: the summaries of the rows elfi_b200_sim_gnk_f64 would simulate, without
- *   writing them (1 <= n_obs <= 512); equal to sim_gnk followed by gnk_summaries.
+ *   writing them (1 <= n_obs <= ELFI_B200_GNK_FUSED_MAX); equal to sim_gnk followed by
+ *   gnk_summaries.
  * sim_bignk: bivariate g-and-k (elfi/examples/bignk.py:12-108).  P[i * ldP + 0..8] = A1, A2, B1, B2,
  *   g1, g2, k1, k2, rho.  Observation j of row i: Philox block (seed, offset + i, j) gives n0, n1;
  *   z1 = n0, z2 = rho n0 + sqrt(1 - rho^2) n1, y_a = the g-and-k quantile of (A_a, B_a, g_a, k_a, c)
  *   at z_a.  |rho| > 1 or NaN gives NaN rows.  Y (B, n_obs, 2) with leading dimension ldY (may be
- *   NULL); S (B, 2 * width) fused summaries of kind `kind` (may be NULL, needs n_obs <= 512).
+ *   NULL); S (B, 2 * width) fused summaries of kind `kind` (may be NULL, needs
+ *   n_obs <= ELFI_B200_GNK_FUSED_MAX).
  * euclidean_multiss (gnk.py:115-142) on (B, K, 1) summaries stored as (B, K) with leading dimension
  *   ldS, K <= 128, obs (K) on the device: out[i] = sqrt(sum_j (S[i, j] - obs[j])^2), summed in
  *   NumPy's pairwise order. */
+#define ELFI_B200_GNK_SERIES_MAX 2048   /* series length of gnk_summaries: the shared-memory sort */
+#define ELFI_B200_GNK_FUSED_MAX 512     /* n_obs of the fused summaries: 32 lanes x 16 keys */
 int elfi_b200_gnk_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_row, int64_t ld_obs,
                                 int64_t B, int64_t n, int64_t d, int32_t kind,
                                 const double* picks_host, double* out, int64_t ld_out, void* stream);
@@ -557,22 +565,26 @@ int elfi_b200_euclidean_multiss_f64(elfi_b200_ctx* ctx, const double* S, int64_t
  * algorithms and limits in elfi_b200/csrc/ricker.cu and poisson.cuh.
  * poisson: out[i] ~ Poisson(lam[i]) (device vectors of n doubles), a pure function of
  *   (seed, offset + i).  Inversion for lam < 10, PTRS (Hoermann 1993) with a cancellation-free
- *   log-pmf test above.  lam == 0 gives 0; lam < 0, NaN or lam > 9.223372006484771e18 (NumPy's
- *   POISSON_LAM_MAX, where NumPy raises) give NaN.  PTRS takes at most 32 trials (each rejected
+ *   log-pmf test above.  lam == 0 gives 0; lam < 0, NaN or lam > ELFI_B200_POISSON_LAM_MAX
+ *   (NumPy's limit, where NumPy raises) give NaN.  PTRS takes at most 32 trials (each rejected
  *   with probability below 0.12); if all 32 are rejected the draw is floor(lam).  The inversion
  *   search stops at 64.  Counts are doubles.
  * sim_ricker: one row per parameter row P[i * ldP + ..]: n_params 3 = (r, sigma, phi), the
  *   stochastic model N_t = N_{t-1} exp((r - N_{t-1}) + sigma e_t) from N_{-1} = stock_init and
  *   Y_t ~ Poisson(phi N_t), t < n_obs; n_params 1 = (r), the deterministic model Y_0 = stock_init,
- *   Y_t = Y_{t-1} exp(r - Y_{t-1}) (N = Y).  1 <= n_obs <= 2^24.  Y (B, n_obs; ldY), N (B, n_obs;
- *   ldN) and S (B, 3; ldS) may each be NULL.  S = [np.mean(Y), np.var(Y), number of zeros of Y]
- *   per row, computed in the simulator without writing Y (needs n_obs <= 128); equal bit for bit
- *   to summary_meanvar and count_zeros of Y.
+ *   Y_t = Y_{t-1} exp(r - Y_{t-1}) (N = Y).  1 <= n_obs <= ELFI_B200_RICKER_NOBS_MAX.
+ *   Y (B, n_obs; ldY), N (B, n_obs; ldN) and S (B, 3; ldS) may each be NULL.
+ *   S = [np.mean(Y), np.var(Y), number of zeros of Y] per row, computed in the simulator without
+ *   writing Y (needs n_obs <=
+ *   ELFI_B200_RICKER_FUSED_MAX); equal bit for bit to summary_meanvar and count_zeros of Y.
  * count_zeros: out[i * ld_out] = the number of entries of row i of X (B, n; ldX) equal to 0, as a
  *   double (num_zeros of ricker.py).
  * chi_squared (ricker.py:147-161) on summaries S (B, K; ldS), K <= 128, obs (K) on the device:
  *   out[i] = sum_j (S[i, j] - obs[j])^2 / obs[j] summed in NumPy's pairwise order; obs[j] = 0
  *   gives NumPy's inf / NaN terms. */
+#define ELFI_B200_POISSON_LAM_MAX 9.223372006484771e18   /* NumPy's POISSON_LAM_MAX */
+#define ELFI_B200_RICKER_NOBS_MAX 16777216   /* 2^24: t << 8 fits the 32-bit block word */
+#define ELFI_B200_RICKER_FUSED_MAX 128       /* fused summaries: one leaf of NumPy's pairwise sum */
 int elfi_b200_poisson_f64(elfi_b200_ctx* ctx, const double* lam, int64_t n, uint64_t seed,
                           uint64_t offset, double* out, void* stream);
 int elfi_b200_sim_ricker_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t n_params,
@@ -586,7 +598,9 @@ int elfi_b200_chi_squared_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, 
 
 /* The 13 Ricker statistics of Wood (2010, Nature 466:1102) in this project's reading (ss_wood of
  * elfi_b200/examples/ricker.py defines them in NumPy); layout in elfi_b200/csrc/ricker_wood.cu.
- * Row i of Y (B, n; ldY >= n), 7 <= n <= 2048, gives out[i * ld_out + 0..12] (ld_out >= 13):
+ * Row i of Y (B, n; ldY >= n), ELFI_B200_RICKER_WOOD_NOBS_MIN <= n <=
+ * ELFI_B200_RICKER_WOOD_NOBS_MAX, gives out[i * ld_out + 0..12] (ld_out >=
+ * ELFI_B200_RICKER_WOOD_WIDTH):
  *   0 mean; 1 number of zeros; 2..7 autocovariances sum_t (y_t - m)(y_{t+k} - m) / n, k = 0..5;
  *   8..10 P e, e the sorted differences y_{t+1} - y_t and P (3 x (n-1), row-major, on the device)
  *   the pseudo-inverse of [o, o^2, o^3] for the sorted observed differences o;
@@ -602,6 +616,9 @@ int elfi_b200_chi_squared_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, 
  *     1e3 2^-53 cond([u v])^2 relative (u, v the two regressor columns).
  * A row with a non-finite value gives 13 NaN.  Results are bit-identical across calls and do not
  * depend on B or on the other rows; B = 0 is a no-op. */
+#define ELFI_B200_RICKER_WOOD_NOBS_MIN 7
+#define ELFI_B200_RICKER_WOOD_NOBS_MAX 2048   /* the shared-memory sort of the differences */
+#define ELFI_B200_RICKER_WOOD_WIDTH 13
 int elfi_b200_ricker_wood_f64(elfi_b200_ctx* ctx, const double* Y, int64_t ldY, int64_t B, int64_t n,
                               const double* P, double* out, int64_t ld_out, void* stream);
 
@@ -612,16 +629,24 @@ int elfi_b200_ricker_wood_f64(elfi_b200_ctx* ctx, const double* Y, int64_t ldY, 
  *   normals, a pure function of (seed, offset + i, s, k): Box-Muller normal (k & 1) of Philox block
  *   (s << 6) | (k >> 1)), sets eta = phi * eta + e * s_phi and takes one RK4 step of length dt.
  *   s_phi = sqrt(1 - phi^2) and dt = total_duration / n_timestep are computed by the caller
- *   (phi > 1 gives NaN rows, as in the reference).  4 <= n_obs <= 128, 2 <= n_timestep <= 2^26.
+ *   (phi > 1 gives NaN rows, as in the reference).
+ *   ELFI_B200_LORENZ_NOBS_MIN <= n_obs <= ELFI_B200_LORENZ_NOBS_MAX, 2 <= n_timestep <=
+ *   ELFI_B200_LORENZ_T_MAX.
  *   X (B, n_timestep, n_obs), C-contiguous, may be NULL; S (B, 6; ldS >= 6) may be NULL and needs
- *   n_timestep * n_obs <= 30728.  With S and without X the summaries are computed in the simulator
- *   from a per-warp scratch slab (up to 512 MiB of the context's scratch, independent of B); with
- *   both, X is written and summarised.  Either way S equals lorenz_summaries of X bit for bit.
+ *   n_timestep * n_obs <= ELFI_B200_LORENZ_SUMM_MAX_TERMS.  With S and without X the summaries are
+ *   computed in the simulator from a per-warp scratch slab (up to 512 MiB of the context's scratch,
+ *   independent of B); with both, X is written and summarised.  Either way S equals
+ *   lorenz_summaries of X bit for bit.
  * lorenz_summaries: S[i * ldS + 0..5] = [Mean, Var, Autocov, Cov, CrosscovPrev, CrosscovNext]
  *   (lorenz.py:231-320) of the row X[i * ld_row + t * ld_t + k * ld_k] (n_timestep, n_obs), bit for
- *   bit NumPy's on a C-contiguous array; 2 <= n_obs <= 128 (with one variable NumPy sums over time
- *   pairwise), n_timestep >= 2,
- *   n_timestep * n_obs <= 30728.  NaN and inf propagate as in NumPy. */
+ *   bit NumPy's on a C-contiguous array; ELFI_B200_LORENZ_SUMM_NOBS_MIN <= n_obs <=
+ *   ELFI_B200_LORENZ_NOBS_MAX (with one variable NumPy sums over time pairwise), n_timestep >= 2,
+ *   n_timestep * n_obs <= ELFI_B200_LORENZ_SUMM_MAX_TERMS.  NaN and inf propagate as in NumPy. */
+#define ELFI_B200_LORENZ_NOBS_MIN 4             /* variables of the ring of sim_lorenz */
+#define ELFI_B200_LORENZ_NOBS_MAX 128
+#define ELFI_B200_LORENZ_SUMM_NOBS_MIN 2
+#define ELFI_B200_LORENZ_T_MAX 67108864         /* 2^26: s << 6 fits the 32-bit block word */
+#define ELFI_B200_LORENZ_SUMM_MAX_TERMS 30728   /* (120 << 8) + 8, what PairwiseLeaves<8> sums */
 int elfi_b200_sim_lorenz_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
                              int64_t n_obs, int64_t n_timestep, const double* init, double f,
                              double phi, double s_phi, double dt, uint64_t seed, uint64_t offset,
@@ -638,18 +663,25 @@ int elfi_b200_lorenz_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t 
  *   (SciPy's levy_stable, S1, beta = 0).  The draws of (d, k) are a pure function of
  *   (seed, offset + i, d, k): Philox blocks (c << 1) | 0 and (c << 1) | 1 with c = d * n_toads + k.
  *   alpha outside (0, 2] or gamma < 0 or NaN (where the reference raises) give a row of NaN.
- *   n_toads >= 1, n_days >= 1, n_days * n_toads <= 2^31.
+ *   n_toads >= 1, n_days >= 1, n_days * n_toads <= ELFI_B200_TOAD_CELLS_MAX.
  *   X (B, n_days, n_toads), C-contiguous, may be NULL.  S (B, n_lags * (n_p + 1); ldS) may be NULL;
- *   it holds toad_summaries of each lag lags[l] (host array, 1 <= lags[l] < n_days, n_lags <= 8) in
- *   columns l * (n_p + 1) .. and needs n_toads * (n_days - 1) <= 4096 and 1 <= n_p <= 32 (p a host
- *   array).  With S and without X the row is simulated into shared memory and summarised there;
- *   with both, X is written and summarised.  Either way S equals toad_summaries of X bit for bit.
+ *   it holds toad_summaries of each lag lags[l] (host array, 1 <= lags[l] < n_days,
+ *   n_lags <= ELFI_B200_TOAD_LAGS_MAX) in columns l * (n_p + 1) .. and needs
+ *   n_toads * (n_days - 1) <= ELFI_B200_TOAD_DISP_MAX and 1 <= n_p <= ELFI_B200_TOAD_NP_MAX (p a
+ *   host array).  With S and without X the row is simulated into shared memory and summarised
+ *   there; with both, X is written and summarised.  Either way S equals toad_summaries of X bit for
+ *   bit.
  * toad_summaries: S[i * ldS + 0 .. n_p] = compute_summaries(X, lag, p, thd) (toad.py:73-132) of the
  *   row X[d * ld_day + k * ld_toad + i * ld_row] (n_days, n_toads): the number of |displacements|
  *   < thd, the median of the others (NaN dropped) and the n_p - 1 logs of the gaps between their p
  *   quantiles floored at exp(-20), through nan_to_num(nan=inf); bit for bit NumPy's except for
- *   the logs, which use the device's log.  1 <= lag < n_days, n_toads * (n_days - lag) <= 4096,
- *   1 <= n_p <= 32 levels in [0, 1] (host array p). */
+ *   the logs, which use the device's log.  1 <= lag < n_days,
+ *   n_toads * (n_days - lag) <= ELFI_B200_TOAD_DISP_MAX, 1 <= n_p <= ELFI_B200_TOAD_NP_MAX levels
+ *   in [0, 1] (host array p). */
+#define ELFI_B200_TOAD_CELLS_MAX 2147483648LL   /* 2^31 n_days * n_toads: (cell << 1) | h < 2^32 */
+#define ELFI_B200_TOAD_DISP_MAX 4096   /* displacements of one lag, sorted per CTA */
+#define ELFI_B200_TOAD_LAGS_MAX 8      /* lags of the fused summaries */
+#define ELFI_B200_TOAD_NP_MAX 32       /* quantile levels */
 int elfi_b200_sim_toad_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
                            int64_t n_toads, int64_t n_days, uint64_t seed, uint64_t offset,
                            double* X, int64_t n_lags, const int64_t* lags, int64_t n_p,
@@ -665,20 +697,27 @@ int elfi_b200_toad_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld
  * sim_lotka_volterra: row i has parameters (r1, r2, r3, prey0, predator0, sigma) = P[i * ldP +
  *   0..5] (ldP >= 6) and starts from (floor(prey0), floor(predator0)); Gillespie's direct method
  *   runs it to time_end (finite, > 0).  X[i * 2 n_obs + 2 j + s] (B, n_obs, 2) is the count of
- *   species s (0 prey, 1 predators) at t_out[j] (device array of n_obs <= 1024 times, t_out[0] = 0,
- *   t_out[n_obs - 1] = time_end; np.linspace), interpolated linearly between the events around it,
- *   plus sigma times a standard normal for j >= 1, truncated toward zero as int32 (NaN or out of
- *   range: -2^31).  n_events[i] (int64) is the number of events row i ran.  Event k draws Philox
- *   block k, observation j block j, of (seed, offset + i): a pure function of the row, whatever
- *   the launch.  A row still short of time_end after max_events (1 .. 2^32 - 1) events gets NaN
- *   observations and n_events = max_events; a negative or NaN rate or sigma, initial counts
- *   outside [0, 2^31) or a negative or NaN total hazard (where the reference raises) give NaN
- *   observations.  The kernel is persistent: its lanes take new rows as theirs finish.
+ *   species s (0 prey, 1 predators) at t_out[j] (device array of n_obs <= ELFI_B200_LV_NOBS_MAX
+ *   times, t_out[0] = 0, t_out[n_obs - 1] = time_end; np.linspace), interpolated linearly between
+ *   the events around it, plus sigma times a standard normal for j >= 1, truncated toward zero as
+ *   int32 (NaN or out of range: -2^31).  n_events[i] (int64) is the number of events row i ran.
+ *   Event k draws Philox block k, observation j block j, of (seed, offset + i): a pure function of
+ *   the row, whatever the launch.  A row still short of time_end after max_events (1 ..
+ *   ELFI_B200_LV_MAX_EVENTS_LIMIT) events gets NaN observations and n_events = max_events; a
+ *   negative or NaN rate or sigma, initial counts outside [0, 2^31) or a negative or NaN total
+ *   hazard (where the reference raises) give NaN observations.  The kernel is persistent: its lanes
+ *   take new rows as theirs finish.
  * lv_summaries: S[i * ldS + 0..8] = prey_mean, pred_mean, prey_log_var, pred_log_var,
  *   prey_autocorr_1, pred_autocorr_1, prey_autocorr_2, pred_autocorr_2, crosscorr
  *   (lotka_volterra.py:206-277) of the row X[i * ld_row + j * ld_obs + s * ld_species]
- *   (n_obs, 2), 3 <= n_obs <= 128, ldS >= 9; bit for bit NumPy's except for log(var + 1), which
+ *   (n_obs, 2), ELFI_B200_LV_SUMM_NOBS_MIN <= n_obs <= ELFI_B200_LV_SUMM_NOBS_MAX,
+ *   ldS >= ELFI_B200_LV_NSUMM; bit for bit NumPy's except for log(var + 1), which
  *   uses the device's log. */
+#define ELFI_B200_LV_NOBS_MAX 1024       /* observation times staged in shared memory */
+#define ELFI_B200_LV_SUMM_NOBS_MIN 3     /* the lag-2 autocorrelation needs one product */
+#define ELFI_B200_LV_SUMM_NOBS_MAX 128   /* one leaf of NumPy's pairwise sum */
+#define ELFI_B200_LV_NSUMM 9
+#define ELFI_B200_LV_MAX_EVENTS_LIMIT 4294967295LL   /* 2^32 - 1: the event is one Philox word */
 int elfi_b200_sim_lotka_volterra_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
                                      const double* t_out, int64_t n_obs, double time_end,
                                      int64_t max_events, uint64_t seed, uint64_t offset,
@@ -691,18 +730,23 @@ int elfi_b200_lv_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_r
  * executable elfi/examples/cpp/bdm.cpp with --mode 1 (throughput mode, statistical parity); law,
  * stream layout, lane layout and arithmetic in elfi_b200/csrc/bdm.cu and bdm.cuh.
  * sim_bdm: row i has rates (alpha, delta, tau) = P[i * ldP + 0..2] (ldP >= 3) and population bound
- *   N (1 <= N <= 1024, B < 2^31).  X[i * ldX + j] (int16, ldX >= N) is the size of cluster j when
- *   the population first exceeds N (that birth undone) or dies out; S[i * ldS + 0..1] (ldS >= 2)
- *   are T1 = count(c > 0) / sum(c) (NaN for an extinct row) and T2 = 1 - sum_j (c_j / n_t2)^2 in
- *   NumPy's pairwise order; either of X and S may be NULL.  n_events[i] (int64) is the number of
- *   events row i ran.  Event k draws Philox block k of (seed, offset + i): a pure function of the
- *   row, whatever the launch.  A rate that is negative, NaN or infinite, or a total rate of 0 or
+ *   N (1 <= N <= ELFI_B200_BDM_N_MAX, B <= ELFI_B200_BDM_BATCH_MAX).  X[i * ldX + j] (int16, ldX >=
+ *   N) is the size of cluster j when the population first exceeds N (that birth undone) or dies
+ *   out; S[i * ldS + 0..1] (ldS >= 2) are T1 = count(c > 0) / sum(c) (NaN for an extinct row) and
+ *   T2 = 1 - sum_j (c_j / n_t2)^2 in NumPy's pairwise order; either of X and S may be NULL.
+ *   n_events[i] (int64) is the number of events row i ran.  Event k draws Philox block k of (seed,
+ *   offset + i): a pure function of the row, whatever the launch.  A rate that is negative, NaN or
+ *   infinite, or a total rate of 0 or
  *   +inf, gives counts of -1, NaN summaries and n_events = -1; a row still running after
- *   max_events (1 .. 2^32 - 1) events gives counts of -1, NaN summaries and n_events =
- *   max_events.  The kernel is persistent: its lanes take new rows as theirs finish.
+ *   max_events (1 .. ELFI_B200_BDM_MAX_EVENTS_LIMIT) events gives counts of -1, NaN summaries and
+ *   n_events = max_events.  The kernel is persistent: its lanes take new rows as theirs finish.
  * bdm_summaries: S[i * ldS + 0..1] = T1, T2 (with n) of the row X[i * ld_row + j * ld_col]
- *   (int16, 1 <= N <= 1024), bit for bit NumPy's and sim_bdm's; a row with a negative count gets
- *   NaN summaries. */
+ *   (int16, 1 <= N <= ELFI_B200_BDM_N_MAX), bit for bit NumPy's and sim_bdm's; a row with a
+ *   negative count gets NaN summaries. */
+#define ELFI_B200_BDM_N_MAX 1024   /* a count stays below N + 2 <= 2^16 (uint16 in shared memory) */
+#define ELFI_B200_BDM_NSUMM 2      /* T1, T2 */
+#define ELFI_B200_BDM_BATCH_MAX 2147483647   /* 2^31 - 1 */
+#define ELFI_B200_BDM_MAX_EVENTS_LIMIT 4294967295LL  /* 2^32 - 1: the event is one Philox word */
 int elfi_b200_sim_bdm_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B, int64_t N,
                           double n_t2, int64_t max_events, uint64_t seed, uint64_t offset,
                           int16_t* X, int64_t ldX, double* S, int64_t ldS, int64_t* n_events,
@@ -714,7 +758,8 @@ int elfi_b200_bdm_summaries_f64(elfi_b200_ctx* ctx, const int16_t* X, int64_t ld
 /* Day care model of elfi/examples/daycare.py (throughput mode, statistical parity); law, stream
  * layout, lane layout and arithmetic in elfi_b200/csrc/daycare.cu and daycare.cuh.
  * sim_daycare: row i has parameters (t1, t2, t3) = P[i * ldP + 0..2] (ldP >= 3); each of its n_dcc
- *   (<= 32) DCCs of n_ind (2 .. 64) children and n_strains (<= 40) strains, community
+ *   (<= ELFI_B200_DC_DCC_MAX) DCCs of n_ind (2 .. ELFI_B200_DC_IND_MAX) children and n_strains
+ *   (<= ELFI_B200_DC_STRAINS_MAX) strains, community
  *   frequencies freq (device, n_strains), runs Gillespie's direct method, and every DCC of the row
  *   takes as many transitions K[i] (int64) as the one that needs most to pass time_end (finite,
  *   > 0).  Transition k of DCC c draws Philox block k of (seed, offset + i) salted with c: a pure
@@ -723,14 +768,22 @@ int elfi_b200_bdm_summaries_f64(elfi_b200_ctx* ctx, const int16_t* X, int64_t ld
  *   (1 .. n_ind) children; X (or NULL) gets their states X[((i * n_dcc + c) * n_obs + o) *
  *   n_strains + s] as 0 / 1.  t1, t2 or t3 negative, NaN or infinite, time_end n_ind n_strains
  *   max(1, max(1, t3) (t1 + 1e-9 + t2 max(freq))) >= 2^32 - 1, or freq negative or not finite:
- *   NaN summaries, zero data, K = -1.  B < 2^31 (one CTA per row).
+ *   NaN summaries, zero data, K = -1.  B <= ELFI_B200_DC_BATCH_MAX.
  * daycare_summaries: S[i * ldS + j * n_dcc + c] as above from X[i * ld_b + c * ld_c + o * ld_i +
- *   s * ld_s] (uint8, nonzero = carrier; n_strains <= 64); bit for bit NumPy's except for the log
+ *   s * ld_s] (uint8, nonzero = carrier;
+ *   n_strains <= ELFI_B200_DC_SUMM_STRAINS_MAX); bit for bit NumPy's except for the log
  *   in Shannon, which uses the device's log.
  * daycare_distance: d[i] (daycare.py:278-312) of the n_ss summaries S[i * ldS + k * n_dcc + c]
- *   (n_ss * n_dcc <= 128) against the observed maxima obs_max (n_ss, 0 replaced by 1) and the
- *   sorted observed values divided by them y (n_ss, n_dcc), both device; bit for bit NumPy's,
- *   including its summation order for B == 1 and B > 1. */
+ *   (n_ss * n_dcc <= ELFI_B200_DC_DIST_TERMS_MAX) against the observed maxima obs_max (n_ss, 0
+ *   replaced by 1) and the sorted observed values divided by them y (n_ss, n_dcc), both device; bit
+ *   for bit NumPy's, including its summation order for B == 1 and B > 1. */
+#define ELFI_B200_DC_DCC_MAX 32             /* one lane per DCC */
+#define ELFI_B200_DC_IND_MAX 64             /* num_s * 64 stays within int64 for n_strains <= 40 */
+#define ELFI_B200_DC_STRAINS_MAX 40         /* lcm(1 .. 40) = 5.3e15 < 2^53 */
+#define ELFI_B200_DC_SUMM_STRAINS_MAX 64    /* one 64-bit strain mask per child */
+#define ELFI_B200_DC_NSUMM 4                /* Shannon, n_strains, prevalence, multi */
+#define ELFI_B200_DC_DIST_TERMS_MAX 128     /* n_ss * n_dcc of the distance: one pairwise leaf */
+#define ELFI_B200_DC_BATCH_MAX 2147483647   /* 2^31 - 1: one CTA per row */
 int elfi_b200_sim_daycare_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
                               int64_t n_dcc, int64_t n_ind, int64_t n_strains,
                               const double* freq, int64_t n_obs, double time_end, uint64_t seed,
@@ -746,7 +799,8 @@ int elfi_b200_daycare_distance_f64(elfi_b200_ctx* ctx, const double* S, int64_t 
 
 /* ARCH(1) model of elfi/examples/arch.py (throughput mode, statistical parity); stream layout,
  * thread layout and arithmetic in elfi_b200/csrc/arch.cu and arch.cuh.
- * Both take 2 <= n_obs (n) <= 128 and 1 <= n_lags <= min(8, n - 1); the summaries are
+ * Both take ELFI_B200_ARCH_NOBS_MIN <= n_obs (n) <= ELFI_B200_ARCH_NOBS_MAX and
+ * 1 <= n_lags <= min(ELFI_B200_ARCH_LAGS_MAX, n - 1); the summaries are
  * S[i * ldS + k], k < 2 + L + L(L-1)/2 (ldS at least that): MU, VAR (ddof = 1), AC_1 .. AC_L, then
  * PW_i_j = AC_i * AC_j in itertools.combinations order, bit for bit NumPy's.
  * sim_arch: row i has parameters (t1, t2) = P[i * ldP + 0..1] (ldP >= 2) and observations
@@ -754,6 +808,9 @@ int elfi_b200_daycare_distance_f64(elfi_b200_ctx* ctx, const double* S, int64_t 
  *   the normals z_{2m}, z_{2m+1}, z_0 = e_0, z_k = xi_k: a pure function of the row, whatever the
  *   launch.  Y and S may each be NULL; S is computed from the row without writing Y.
  * arch_summaries: the summaries of the row X[i * ld_b + j * ld_j], j < n, any strides. */
+#define ELFI_B200_ARCH_NOBS_MIN 2
+#define ELFI_B200_ARCH_NOBS_MAX 128   /* one leaf of NumPy's pairwise sum per reduction */
+#define ELFI_B200_ARCH_LAGS_MAX 8
 int elfi_b200_sim_arch_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
                            int64_t n_obs, int64_t n_lags, uint64_t seed, uint64_t offset,
                            double* Y, int64_t ldY, double* S, int64_t ldS, void* stream);
@@ -766,7 +823,8 @@ int elfi_b200_arch_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld
  * elfi_b200/csrc/ar1.cu and ar1.cuh.  Row i has parameter phi[i] and series
  * x_t = phi x_{t-1} + w_t (x_0 = 0), X[i * ldX + t - 1] for t = 1 .. n_obs (ldX >= n_obs; X may be
  * NULL).  Block m of (seed, offset + i) gives the innovations w_{2m+1}, w_{2m+2}: a pure function
- * of the row, whatever the launch.  0 <= B <= 2^31 - 1, 1 <= n_obs <= 2^24.
+ * of the row, whatever the launch.  0 <= B <= ELFI_B200_AR1_BATCH_MAX,
+ * 1 <= n_obs <= ELFI_B200_AR1_NOBS_MAX.
  * With obs (n_obs doubles) the row's distance d_out[i] = sqrt(sum_t (x_t - obs_t)^2), t ascending,
  * one rounding per operation: bit for bit elfi_b200_dist_euclid_thr_f64 of the written series
  * (K = 1, no weights), computed without writing X.  With a threshold (one double, thr_host on the
@@ -774,6 +832,8 @@ int elfi_b200_arch_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld
  * (B int32, may be NULL) gets their indices ascending and n_acc (one int64 on the device, may be
  * NULL) their number, the contract of the distance entry points above.  Without obs, d_out,
  * thresholds, acc_idx and n_acc must be NULL. */
+#define ELFI_B200_AR1_NOBS_MAX 16777216     /* 2^24 */
+#define ELFI_B200_AR1_BATCH_MAX 2147483647  /* 2^31 - 1: accepted rows are int32 indices */
 int elfi_b200_sim_ar1_f64(elfi_b200_ctx* ctx, const double* phi, int64_t B, int64_t n_obs,
                           uint64_t seed, uint64_t offset, double* X, int64_t ldX,
                           const double* obs, const double* thr_host, const double* thr_dev,
@@ -783,12 +843,17 @@ int elfi_b200_sim_ar1_f64(elfi_b200_ctx* ctx, const double* phi, int64_t B, int6
  * layout and arithmetic in elfi_b200/csrc/mg1.cu and mg1.cuh.  Rows where the reference's NumPy
  * raises (1/t3 with its sign bit set, t2 - t1 not finite) give NaN data and NaN quantiles.
  * sim_mg1: row i has parameters (t1, t2, t3) = P[i * ldP + 0..2] (ldP >= 3) and inter-departure
- *   times Y[i * ldY + j], j < n_obs (2 <= n_obs <= 512); S[i * ldS + k] = np.quantile(y_i, q[k])
- *   (method 'linear'; 1 <= nq <= 32, q_host on the host, each in [0, 1]) is computed in the same
- *   kernel.  Y or S may be NULL; row i is a pure function of (seed, offset + i).
+ *   times Y[i * ldY + j], j < n_obs (ELFI_B200_MG1_NOBS_MIN <= n_obs <= ELFI_B200_MG1_NOBS_MAX);
+ *   S[i * ldS + k] = np.quantile(y_i, q[k]) (method 'linear'; 1 <= nq <= ELFI_B200_MG1_NQ_MAX,
+ *   q_host on the host, each in [0, 1]) is computed in the same kernel.  Y or S may be NULL; row i
+ *   is a pure function of (seed, offset + i).
  * row_quantiles: S[b * ldS + k] = np.quantile(X[b, :], q[k]) of the row X[b * ld_b + j * ld_j],
- *   j < n (2 <= n <= 512), any strides; a row with a NaN has every quantile NaN.  Bit for bit
+ *   j < n (ELFI_B200_MG1_NOBS_MIN <= n <= ELFI_B200_MG1_NOBS_MAX), any strides; a row with a NaN
+ *   has every quantile NaN.  Bit for bit
  *   NumPy's, and the quantiles sim_mg1 fuses are the bits of row_quantiles of its data. */
+#define ELFI_B200_MG1_NOBS_MIN 2
+#define ELFI_B200_MG1_NOBS_MAX 512   /* one warp sorts a row in registers (32 lanes x 16 keys) */
+#define ELFI_B200_MG1_NQ_MAX 32      /* one quantile per lane */
 int elfi_b200_sim_mg1_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
                           int64_t n_obs, int64_t nq, const double* q_host, uint64_t seed,
                           uint64_t offset, double* Y, int64_t ldY, double* S, int64_t ldS,
@@ -817,16 +882,20 @@ int elfi_b200_sim_svm_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int6
  * streams); law, stream layout and warp layout in elfi_b200/csrc/scratch_assay.cuh and
  * scratch_assay.cu.
  * sim_scratch_assay: row i has parameters (pm, pp) = P[i * ldP + 0..1] (ldP >= 2) and starts from
- *   the lattice init[r * ncols + c] (device, nrows * ncols <= 4096 bytes, nonzero = a cell).  It
- *   runs num_iter (< 2^31) iterations of motility then proliferation and observes the lattice
- *   every obs_interval (>= 1) iterations: num_obs = num_iter / obs_interval frames after the
- *   initial one.  S[i * ldS + k] (ldS >= num_obs + 1) gets the mismatches between frames k and
- *   k + 1, k < num_obs, then S[i * ldS + num_obs] the cells of the last frame; X gets the frames
- *   X[((i * nrows + r) * ncols + c) * (num_obs + 1) + k] as 0 / 1.  S and X may each be NULL; S is
- *   computed without writing X.  Row i is a pure function of (seed, offset + i); B < 2^31.
+ *   the lattice init[r * ncols + c] (device, nrows * ncols <= ELFI_B200_SA_SITES_MAX bytes, nonzero
+ *   = a cell).  It runs num_iter (<= ELFI_B200_SA_ITER_MAX) iterations of motility then
+ *   proliferation and observes the lattice every obs_interval (>= 1) iterations: num_obs = num_iter
+ *   / obs_interval frames after the initial one.  S[i * ldS + k] (ldS >= num_obs + 1) gets the
+ *   mismatches between frames k and k + 1, k < num_obs, then S[i * ldS + num_obs] the cells of the
+ *   last frame; X gets the frames X[((i * nrows + r) * ncols + c) * (num_obs + 1) + k] as 0 / 1.  S
+ *   and X may each be NULL; S is computed without writing X.  Row i is a pure function of (seed,
+ *   offset + i); B <= ELFI_B200_SA_BATCH_MAX.
  * scratch_assay_summaries: the same summaries S[i * ldS + k], k < n_frames (ldS >= n_frames), of
  *   the frames X[i * ld_b + r * ld_r + c * ld_c + k * ld_k] (uint8, nonzero = a cell), any
  *   strides: n_frames - 1 mismatches, then the cells of the last frame. */
+#define ELFI_B200_SA_SITES_MAX 4096         /* lattice sites: list entries fit uint16 */
+#define ELFI_B200_SA_ITER_MAX 2147483647    /* 2^31 - 1: iteration counters of the Philox streams */
+#define ELFI_B200_SA_BATCH_MAX 2147483647   /* 2^31 - 1: one warp per row */
 int elfi_b200_sim_scratch_assay_f64(elfi_b200_ctx* ctx, const double* P, int64_t ldP, int64_t B,
                                     const uint8_t* init, int64_t nrows, int64_t ncols,
                                     int64_t num_iter, int64_t obs_interval, uint64_t seed,
@@ -857,10 +926,11 @@ int elfi_b200_scratch_assay_summaries_f64(elfi_b200_ctx* ctx, const uint8_t* X, 
  * Sigma_l is not finite or L_jj^2 <= 1e6 * DBL_EPSILON * max_i Sigma_l,ii.  SciPy instead tests the
  * eigenvalues against 1e6 eps lambda_max and gives up near cond(Sigma) ~ 4.5e9; near that boundary
  * the two tests can disagree (by a factor that depends on d), and one may return a finite value
- * where the other returns -inf.  Limits: 1 <= d <= 160, n >= 2, G <= 2^22, K <= 65535.  Results
- * are bit-identical across calls, and a group's value does not depend on G, K or the other
- * groups.  Asynchronous on `stream`; uses the context's scratch (about G d^2 doubles, more with
- * whitening or when few groups split their rows over several CTAs). */
+ * where the other returns -inf.  Limits: 1 <= d <= ELFI_B200_SYNLIK_D_MAX, n >= 2, G <= 2^22, K <=
+ * 65535.  Results are bit-identical across calls, and a group's value does not depend on G, K or
+ * the other groups.  Asynchronous on `stream`; uses the context's scratch (about G d^2 doubles,
+ * more with whitening or when few groups split their rows over several CTAs). */
+#define ELFI_B200_SYNLIK_D_MAX 160   /* Sigma, its factor and y in one CTA's shared memory */
 int elfi_b200_synlik_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_row, int64_t ld_group,
                          int64_t G, int64_t n, int64_t d, const double* y, const double* W,
                          int32_t estimator, const double* penalties_host, int64_t K,
@@ -903,9 +973,10 @@ int elfi_b200_synlik_obs_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_row
  *     log prior is not finite.
  * Random stream: Philox4x32-10 keyed by seed; u = u01(x, y) of counter (t, c, 0, 0x4253434c), and
  * z_2k, z_2k+1 the two Box-Muller normals of counter (t + 1, c, 1 + k, 0x4253434c), so that no
- * value depends on C or on the other chains.  Limits: 1 <= C <= 2^22, 1 <= p <= 16, b >= 1,
- * C b < 2^31, ld_rows >= C b, 0 <= t < n_samples < 2^32.  Asynchronous on `stream`, bit-identical
- * across calls. */
+ * value depends on C or on the other chains.  Limits: 1 <= C <= ELFI_B200_BSL_MAX_CHAINS,
+ * 1 <= p <= 16, b >= 1, C b < 2^31, ld_rows >= C b, 0 <= t < n_samples < 2^32.  Asynchronous on
+ * `stream`, bit-identical across calls. */
+#define ELFI_B200_BSL_MAX_CHAINS 4194304   /* 2^22 */
 int elfi_b200_bsl_mh_step_f64(elfi_b200_ctx* ctx, int64_t C, int64_t p, int64_t t,
                               int64_t n_samples, int64_t burn_in, int64_t b, uint64_t seed,
                               const double* spec_host, const double* chol_host,
@@ -948,9 +1019,12 @@ int elfi_b200_bsl_mh_step_keyed_f64(elfi_b200_ctx* ctx, int64_t C, int64_t p, in
  *   (coef device, q x pg row-major).  dense = 1 states that every row is in the group (n_g = N):
  *   pos = i, with no compaction; dense = 0 gives pos = the rank of i among the group's rows.
  *   ld_out >= N when dense.
- * Limits: q, p >= 1, q + p <= 256, 1 <= N < 2^31, 1 <= pg <= p, -1 <= sel < p.  Asynchronous on
- * `stream`; moments use about min(N / 256, 2048) * 64^2 doubles of the context's scratch, adjust
+ * Limits: q, p >= 1, q + p <= ELFI_B200_REGADJ_D_MAX, 1 <= N <= ELFI_B200_REGADJ_N_MAX,
+ * 1 <= pg <= p, -1 <= sel < p.  Asynchronous on `stream`; moments use about min(N / 256, 2048) *
+ * 64^2 doubles of the context's scratch, adjust
  * N / 2048 int64. */
+#define ELFI_B200_REGADJ_D_MAX 256   /* q + p: a group's mean and tile rows in shared memory */
+#define ELFI_B200_REGADJ_N_MAX 2147483647   /* 2^31 - 1: int32 row ranks in the compaction */
 int elfi_b200_regadj_mask_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t N,
                               int64_t q, const double* obs, const double* T, int64_t ldT, int64_t p,
                               uint8_t* flags, int64_t* counts, void* stream);
@@ -987,10 +1061,12 @@ int elfi_b200_regadj_adjust_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS
  *   with v = sum_j coef_j (x_j - mean_j) / scale_j + intercept_, p = 1 / (1 + exp(-v)), then
  *   p = max(p, class_min): the reference's log-likelihood ratio (p = 1 gives +inf).  A row with a
  *   non-finite value, or a fit with a negative status, gives NaN.
- * Limits: 1 <= d <= 160, 2 <= n < 2^31, C > 0.  One CTA per fit; reductions in a fixed order, no
- * atomics: repeated calls are bit-identical.  Asynchronous on `stream`; the fit uses 4 n doubles of
- * the context's scratch. */
-#define ELFI_B200_LOGREG_BLOCK(d) (8 + 3 * (d))
+ * Limits: 1 <= d <= ELFI_B200_LOGREG_D_MAX, 2 <= n < 2^31, C > 0.  One CTA per fit; reductions in a
+ * fixed order, no atomics: repeated calls are bit-identical.  Asynchronous on `stream`; the fit
+ * uses 4 n doubles of the context's scratch. */
+#define ELFI_B200_LOGREG_D_MAX 160   /* H and the row tiles in one CTA's shared memory */
+#define ELFI_B200_LOGREG_HEAD 8      /* header doubles of a fit block */
+#define ELFI_B200_LOGREG_BLOCK(d) (ELFI_B200_LOGREG_HEAD + 3 * (d))
 int elfi_b200_logreg_fit_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_row, int64_t n,
                              int64_t d, const double* y, int32_t penalty, double C,
                              int64_t max_iter, double* fit, void* stream);
@@ -1032,11 +1108,14 @@ int elfi_b200_rowsort_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, int6
  * accumulated left to right over the concatenated columns with one rounding per multiply and add,
  * the arithmetic of elfi_b200_dist_metric_thr_f64, so every value is bit-identical to SciPy's cdist
  * on the concatenation, NaN and +-inf included (a NaN term makes the sums NaN; 'chebyshev' skips
- * it, as SciPy does).  Limits: 1 <= W <= 512, 1 <= C < 2^24, 0 <= B < 2^31.  One CTA stages 32
+ * it, as SciPy does).  Limits: 1 <= W <= ELFI_B200_SUBSET_MAX_WIDTH,
+ * 1 <= C <= ELFI_B200_SUBSET_MAX_COMBINATIONS, 0 <= B < 2^31.  One CTA stages 32
  * rows in shared memory (32 (W + 1) doubles) and its warps take the combinations in turn, so each
  * row is read from HBM once for all C.  No scratch, no atomics: repeated calls give the same bits.
  * Asynchronous on `stream`. */
 #define ELFI_B200_METRIC_EUCLIDEAN 0
+#define ELFI_B200_SUBSET_MAX_WIDTH 512
+#define ELFI_B200_SUBSET_MAX_COMBINATIONS 16777215   /* 2^24 - 1 */
 
 int elfi_b200_subset_distance_f64(elfi_b200_ctx* ctx, int32_t metric, const double* S, int64_t ldS,
                                   int64_t B, int64_t W, const double* obs, const int32_t* ranges,
@@ -1069,10 +1148,15 @@ int elfi_b200_dist_seg_f64(elfi_b200_ctx* ctx, int32_t metric, double pexp, cons
  *           i = t, t + 256, ... in turn, then a fixed pairwise tree), so identical sets give
  *           identical bits; a zero R gives -inf, an infinite one +inf.
  * The host forms the entropy log(pi^(q/2) / Gamma(q/2 + 1)) - digamma(k) + log(n) + q / n logsum.
- * Limits: 1 <= q <= 16, 1 <= k <= 32, 1 <= n <= 2^20, 1 <= C < 2^16.  Brute force: a CTA of 128
+ * Limits: 1 <= q <= ELFI_B200_KNN_MAX_Q, 1 <= k <= ELFI_B200_KNN_MAX_K, 
+ * 1 <= n <= ELFI_B200_KNN_MAX_N, 1 <= C <= ELFI_B200_KNN_MAX_SETS.  Brute force: a CTA of 128
  * query points streams the set through shared memory in tiles of 256 points, and each thread keeps
  * its k smallest squared distances in registers (a sorted insertion).  Two launches, no scratch,
  * no atomics.  Asynchronous on `stream`. */
+#define ELFI_B200_KNN_MAX_Q 16
+#define ELFI_B200_KNN_MAX_K 32
+#define ELFI_B200_KNN_MAX_N 1048576    /* 2^20 */
+#define ELFI_B200_KNN_MAX_SETS 65535   /* 2^16 - 1 */
 int elfi_b200_knn_entropy_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, int64_t C,
                               int64_t n, int64_t q, int64_t k, double* R, double* logsum,
                               void* stream);
@@ -1085,20 +1169,22 @@ int elfi_b200_knn_entropy_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, 
  *           taken in a fixed order (256 threads over the n q entries, then a fixed tree) and the
  *           roots are added in order of j, so repeated calls give the same bits; NumPy's norm sums
  *           in another order, so the two agree to rounding.  NaN and inf propagate.
- * Limits: 1 <= q <= 16, 1 <= n q < 2^31, 1 <= m < 2^31, 1 <= C < 2^31.  One CTA per set, one
- * launch, no scratch, no atomics.  Asynchronous on `stream`. */
+ * Limits: 1 <= q <= ELFI_B200_KNN_MAX_Q, 1 <= n q < 2^31, 1 <= m < 2^31, 1 <= C < 2^31.  One CTA
+ * per set, one launch, no scratch, no atomics.  Asynchronous on `stream`. */
 int elfi_b200_mrsse_f64(elfi_b200_ctx* ctx, const double* T, int64_t ldT, int64_t C, int64_t n,
                         int64_t q, const double* P, int64_t ldP, int64_t m, double* out,
                         void* stream);
 
 /* ---- robust optimisation Monte Carlo (ROMC, elfi/methods/inference/romc.py) ----------------
- * P optimisation problems with 1 <= p <= 16 parameters advance in lock-step: every call consumes
- * the objective value of the point each problem proposed last call and writes the next point.
+ * P optimisation problems with 1 <= p <= ELFI_B200_ROMC_MAX_P parameters advance in lock-step:
+ * every call consumes the objective value of the point each problem proposed last call and writes
+ * the next point.
  * The host evaluates all P points of a call as one batch, so the stream row of problem i stays i.
  * Products, sums and quotients that must match NumPy use round-to-nearest intrinsics (no FMA).
  * One thread per problem (or per point), no scratch, no atomics.  Asynchronous on `stream`. */
 #define ELFI_B200_ROMC_MAX_P 16
 #define ELFI_B200_ROMC_NM_INTS 8   /* ints of Nelder-Mead state per problem */
+#define ELFI_B200_ROMC_NM_DONE 6   /* istate[i, 0] of a finished problem */
 /* doubles of Nelder-Mead state per problem: the simplex (p + 1, p), fsim (p + 1), xbar, the
  * reflected point and the trial point (p each), f at the reflection and f_min */
 #define ELFI_B200_ROMC_NM_DOUBLES(p) (((p) + 1) * ((p) + 1) + 3 * (p) + 2)
@@ -1122,9 +1208,10 @@ int elfi_b200_romc_nm_init_f64(elfi_b200_ctx* ctx, int64_t P, int64_t p, const d
  * by a stable sort, NaN last: np.argsort's order whenever fsim has no ties, and for p <= 2; with
  * ties at p >= 3 NumPy's order depends on the CPU's SIMD sort (DESIGN.md section 7, "ROMC").
  * A finished problem keeps x_min in its theta row and ignores its value from then on:
- *   istate[i, 0] = 6 (done), istate[i, 1] = nit, istate[i, 2] = nfev, istate[i, 4] = scipy's
- *   warnflag (0 success, 1 maxfev, 2 maxiter); the first p doubles of state row i are x_min and
- *   double ELFI_B200_ROMC_NM_DOUBLES(p) - 1 is f_min = np.min(fsim) (NaN when any vertex is NaN).
+ *   istate[i, 0] = ELFI_B200_ROMC_NM_DONE, istate[i, 1] = nit, istate[i, 2] = nfev, istate[i, 4] =
+ *   scipy's warnflag (0 success, 1 maxfev, 2 maxiter); the first p doubles of state row i are x_min
+ *   and double ELFI_B200_ROMC_NM_DOUBLES(p) - 1 is f_min = np.min(fsim) (NaN when any vertex is
+ *   NaN).
  * Limits: 0 <= P < 2^31, 1 <= maxiter, maxfev < 2^30. */
 int elfi_b200_romc_nm_step_f64(elfi_b200_ctx* ctx, int64_t P, int64_t p, double* state,
                                int32_t* istate, const double* fvals, double* theta,

@@ -4,8 +4,9 @@ The product has no CPU path: elfi_b200 raises without a CUDA device.  To test th
 (operator wrappers in ops.py, the ElfiModel graph, Rejection / SMC state machines, the rank
 sharding) on a machine without a GPU, the `cpu_double` fixture of tests/conftest.py swaps
 
-  * elfi_b200._lib.call        -> `call` below: every entry point restated on host pointers with
-                                  NumPy + the oracle (same argument lists as the header), and
+  * elfi_b200._lib.call        -> the router `install` sets: every entry point restated on host
+                                  pointers with NumPy + the oracle (same argument lists as the
+                                  header), and
   * the allocation helpers of elfi_b200.device -> CPU torch tensors.
 
 Nothing outside tests/ imports this module.  Entry points that the CPU tests do not need raise
@@ -620,19 +621,6 @@ _TABLE = {'elfi_b200_' + f.__name__: f for f in (
     gm_rvs_f64, gm_cdf_f64, gm_rvs_cdf_f64, prior_gauss_f64, logprior_gauss_f64, sim_gauss_f64, sim_gnk_f64, logprior_box_f64)}
 
 
-def call(name, *args):
-    """Stand-in for elfi_b200._lib.call: same names, same argument lists, host pointers."""
-    fn = _TABLE.get(name)
-    if fn is None:
-        raise _lib.ElfiB200Error('cpu double: {} is not emulated (device-only entry point)'.format(name))
-    if len(args) != len(_lib.SIGNATURES[name]):
-        raise TypeError('{} takes {} arguments, got {}'.format(name, len(_lib.SIGNATURES[name]),
-                                                               len(args)))
-    CALLS.append(name)
-    fn(*args)
-    return 0
-
-
 # ------------------------------------------------------------------------------ device.py side
 class DeviceTensor(torch.Tensor):
     """A CPU tensor that behaves like a CUDA tensor where the two differ for host code: it cannot
@@ -689,9 +677,26 @@ def _flatten(items):
     return out
 
 
-def install(monkeypatch):
+def install(monkeypatch, *tables):
     """Patch elfi_b200._lib.call and the allocation helpers of elfi_b200.device (CPU tensors that
-    are as strict as CUDA tensors, see DeviceTensor)."""
+    are as strict as CUDA tensors, see DeviceTensor).  Each of `tables` (entry point name ->
+    restatement, the TABLE of a tests/*_double.py module) takes precedence over the ones before
+    it and over this module's own; the tables are read at call time."""
+    routes = tables[::-1] + (_TABLE,)
+
+    def call(name, *args):
+        """Stand-in for elfi_b200._lib.call: same names, same argument lists, host pointers."""
+        fn = next((t[name] for t in routes if name in t), None)
+        if fn is None:
+            raise _lib.ElfiB200Error('cpu double: {} is not emulated (device-only entry point)'
+                                     .format(name))
+        if len(args) != len(_lib.SIGNATURES[name]):
+            raise TypeError('{} takes {} arguments, got {}'.format(name, len(_lib.SIGNATURES[name]),
+                                                                   len(args)))
+        CALLS.append(name)
+        fn(*args)
+        return 0
+
     from elfi_b200 import device as dev
     from elfi_b200 import samplers
 

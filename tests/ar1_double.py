@@ -1,6 +1,6 @@
 """CPU test double of the AR(1) entry point -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py (installed first, by the `cpu_double` fixture) with a restatement of
+Extends tests/abi_double.py (through `abi_double.install`) with a restatement of
 elfi_b200_sim_ar1_f64 on host pointers: the series is tests/ar1_replay.py (the kernel's Philox
 streams and recursion, so the same rows as the device up to the last bits of the normals), the
 distance and the accepted rows are the oracle's cdist and acceptance of exactly that series, as on
@@ -11,7 +11,7 @@ import numpy as np
 import abi_double as d
 import ar1_replay
 import elfi_oracle as o
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 
 def sim_ar1_f64(ctx, phi, B, n_obs, seed, offset, X, ldX, obs, thr_host, thr_dev, d_out, acc_idx,
@@ -41,21 +41,4 @@ def sim_ar1_f64(ctx, phi, B, n_obs, seed, offset, X, ldX, obs, thr_host, thr_dev
             d._vec(n_acc, 1, np.int64)[0] = len(idx)
 
 
-_TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_ar1_f64,)}
-
-
-def install(monkeypatch):
-    """Route the AR(1) entry point here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_ar1_f64,)}

@@ -1,6 +1,6 @@
 """CPU test double of the ARCH(1) entry points -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py (installed first, by the `cpu_double` fixture) with restatements of
+Extends tests/abi_double.py (through `abi_double.install`) with restatements of
 elfi_b200_sim_arch_f64 and elfi_b200_arch_summaries_f64 on host pointers.  The summaries are the
 reference's NumPy code (elfi_b200.examples.arch on host arrays); the simulator runs the reference's
 recurrence on normals from a NumPy RandomState instead of the device's Philox streams (same
@@ -12,7 +12,7 @@ from itertools import combinations
 import numpy as np
 
 import abi_double as d
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 
 def summaries(x, n_lags):
@@ -63,21 +63,4 @@ def arch_summaries_f64(ctx, X, ld_b, ld_j, B, n, n_lags, S, ldS, stream):
     d._mat(S, B, ops.arch_nsumm(n_lags), ldS)[:] = summaries(x, n_lags)
 
 
-_TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_arch_f64, arch_summaries_f64)}
-
-
-def install(monkeypatch):
-    """Route the ARCH entry points here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_arch_f64, arch_summaries_f64)}

@@ -1,6 +1,6 @@
 """CPU test double of the birth-death-mutation entry points -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py (installed first, by the `cpu_double` fixture) with restatements of
+Extends tests/abi_double.py (through `abi_double.install`) with restatements of
 elfi_b200_sim_bdm_f64 and elfi_b200_bdm_summaries_f64 on host pointers: the simulator is
 tests/bdm_replay.py (the kernel's Philox streams, so the same rows as the device), the summaries
 are the reference's NumPy T1 and T2 (elfi_b200.examples.bdm on host arrays), NaN for a row with a
@@ -10,7 +10,7 @@ import numpy as np
 
 import abi_double as d
 import bdm_replay
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 
 def summaries(x, n):
@@ -47,21 +47,4 @@ def bdm_summaries_f64(ctx, X, ld_row, ld_col, B, N, n, S, ldS, stream):
     d._mat(S, B, ops.BDM_NSUMM, ldS)[:] = summaries(x, n)
 
 
-_TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_bdm_f64, bdm_summaries_f64)}
-
-
-def install(monkeypatch):
-    """Route the BDM entry points here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_bdm_f64, bdm_summaries_f64)}

@@ -1,7 +1,7 @@
 """NumPy restatements of the lock-step BSL chains -- TEST INFRASTRUCTURE ONLY.
 
 * `mh_step` restates elfi_b200_bsl_mh_step_f64 (include/elfi_b200.h) with oracle/streams.py's
-  Philox4x32-10, u01 and Box-Muller, in the kernel's order of operations; `install` routes the entry
+  Philox4x32-10, u01 and Box-Muller, in the kernel's order of operations; `TABLE` routes the entry
   point here on top of tests/abi_double.py, so throughput mode's host logic runs without a GPU.
 * `parity_chains` restates parity mode as C reference-style Metropolis-Hastings loops (each with
   its own RandomState) that share one batch stream per iteration: batch k is simulated by the
@@ -14,7 +14,6 @@ import abi_double as d
 import bsl_double
 import conditional_prior_replay as cpr
 import streams
-from elfi_b200 import _lib
 from elfi_b200 import model as em
 from elfi_b200.bsl import BSL
 from elfi_b200.samplers import ModelPrior
@@ -134,24 +133,7 @@ def bsl_mh_step_f64(ctx, C, p, t, n_samples, burn_in, b, seed, spec_host, chol_h
         out[:] = np.repeat(r, b, axis=0).T
 
 
-_TABLE = {'elfi_b200_bsl_mh_step_f64': bsl_mh_step_f64}
-
-
-def install(monkeypatch):
-    """Route elfi_b200_bsl_mh_step_f64 here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_bsl_mh_step_f64': bsl_mh_step_f64}
 
 
 # ------------------------------------------------------------------------------ parity mode

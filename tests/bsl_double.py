@@ -4,15 +4,14 @@ its CPU test double -- TEST INFRASTRUCTURE ONLY.
 `synlik` states the device's definition with NumPy and SciPy: np.cov moments, whitening as
 W Sigma W^T and W (y - mu), Warton shrinkage (1 - l) Sigma + l diag(Sigma_jj + 1e-5), one Cholesky
 factor, and -inf for a group with a non-finite input or a pivot L_jj^2 <= 1e6 eps max_i Sigma_ii.
-`install` routes the entry point here on top of tests/abi_double.py (installed first, by the
-`cpu_double` fixture), so the unmodified BSL host code runs without a GPU.
+`TABLE` routes the entry point here on top of tests/abi_double.py (through
+`abi_double.install`), so the unmodified BSL host code runs without a GPU.
 """
 import numpy as np
 import scipy.linalg
 from scipy.special import gammaln
 
 import abi_double as d
-from elfi_b200 import _lib
 
 PIVOT_CUT = 1e6 * np.finfo(np.float64).eps
 D_MAX = 160
@@ -92,21 +91,4 @@ def synlik_f64(ctx, S, ld_row, ld_group, G, n, dim, y, W, estimator, penalties_h
     d._vec(loglik, G * max(K, 1))[:] = ll.reshape(-1)
 
 
-_TABLE = {'elfi_b200_synlik_f64': synlik_f64}
-
-
-def install(monkeypatch):
-    """Route elfi_b200_synlik_f64 here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_synlik_f64': synlik_f64}

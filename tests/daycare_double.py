@@ -1,6 +1,6 @@
 """CPU test double of the day care entry points -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py (installed first, by the `cpu_double` fixture) with restatements of
+Extends tests/abi_double.py (through `abi_double.install`) with restatements of
 elfi_b200_sim_daycare_f64, elfi_b200_daycare_summaries_f64 and elfi_b200_daycare_distance_f64 on
 host pointers.  The summaries and the distance are the reference's NumPy code
 (elfi_b200.examples.daycare on host arrays); the simulator is the reference's daycare() run one row
@@ -11,7 +11,7 @@ NaN summaries, zero data and K = -1 for the rows the device refuses (daycare_rep
 import numpy as np
 
 import abi_double as d
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 
 def _summaries(x):
@@ -89,22 +89,5 @@ def daycare_distance_f64(ctx, S, ldS, B, n_ss, n_dcc, obs_max, y, dist, stream):
         d._vec(dist, B)[:] = np.sum(np.abs(x - yy), axis=(0, 2)) / (n_ss * n_dcc)
 
 
-_TABLE = {'elfi_b200_' + f.__name__: f
-          for f in (sim_daycare_f64, daycare_summaries_f64, daycare_distance_f64)}
-
-
-def install(monkeypatch):
-    """Route the day care entry points here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_' + f.__name__: f
+         for f in (sim_daycare_f64, daycare_summaries_f64, daycare_distance_f64)}

@@ -5,15 +5,14 @@ double -- TEST INFRASTRUCTURE ONLY.
 `subset_distance` is SciPy's cdist on each combination's concatenated columns, `select` the first n
 rows of a stable argsort by distance (NaN last: the order Rejection's batch-by-batch merge keeps),
 `knn_radii` cKDTree's k-th distances and `mrsse` the reference's mean root sum of squared errors.
-`install` routes the three entry points here on top of tests/abi_double.py (installed first, by the
-`cpu_double` fixture), so the unmodified TwoStageSelection host code runs without a GPU.
+`TABLE` routes the three entry points here on top of tests/abi_double.py (through
+`abi_double.install`), so the unmodified TwoStageSelection host code runs without a GPU.
 """
 import numpy as np
 from scipy.spatial import cKDTree
 from scipy.spatial.distance import cdist
 
 import abi_double as d
-from elfi_b200 import _lib
 
 METRICS = ('euclidean', 'sqeuclidean', 'cityblock', 'chebyshev')
 
@@ -81,21 +80,4 @@ def mrsse_f64(ctx, T, ldT, C, n, q, P, ldP, m, out, stream):
     d._vec(out, C)[:] = [mrsse(pts[c * n:(c + 1) * n], closest) for c in range(C)]
 
 
-_TABLE = {'elfi_b200_' + f.__name__: f for f in (subset_distance_f64, knn_entropy_f64, mrsse_f64)}
-
-
-def install(monkeypatch):
-    """Route the three entry points here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_' + f.__name__: f for f in (subset_distance_f64, knn_entropy_f64, mrsse_f64)}

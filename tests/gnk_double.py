@@ -1,6 +1,6 @@
 """CPU test double of the g-and-k summary entry points -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py (installed first, by the `cpu_double` fixture) with restatements of
+Extends tests/abi_double.py (through `abi_double.install`) with restatements of
 elfi_b200_gnk_summaries_f64, elfi_b200_sim_gnk_summaries_f64, elfi_b200_sim_bignk_f64 and
 elfi_b200_euclidean_multiss_f64 on host pointers.  The summaries are the reference's NumPy code
 (elfi_b200.examples.gnk on host arrays); the simulators draw from a NumPy RandomState instead of
@@ -12,7 +12,7 @@ import ctypes
 import numpy as np
 
 import abi_double as d
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 KINDS = {v: k for k, v in ops.GNK_KINDS.items()}
 
@@ -97,22 +97,5 @@ def euclidean_multiss_f64(ctx, S, ldS, B, K, obs, out, stream):
                                                   observed=[d._vec(obs, K)[None, :, None]])
 
 
-_TABLE = {'elfi_b200_' + f.__name__: f for f in (
+TABLE = {'elfi_b200_' + f.__name__: f for f in (
     gnk_summaries_f64, sim_gnk_summaries_f64, sim_bignk_f64, euclidean_multiss_f64)}
-
-
-def install(monkeypatch):
-    """Route the g-and-k summary entry points here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)

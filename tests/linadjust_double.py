@@ -6,14 +6,13 @@ INFRASTRUCTURE ONLY.
 without a non-finite value on rows with finite summaries share one group, any other parameter has
 its own), the count, means and centred moments of [S - o | theta_g] over a group's rows, the
 device's solve rule (eigh of the q x q block, eigenvalues above tol^2 lambda_max, minimum-norm
-solution) and the ordered adjusted columns.  `install` routes the three entry points here on top
-of tests/abi_double.py (installed first, by the `cpu_double` fixture), so the unmodified host code
+solution) and the ordered adjusted columns.  `TABLE` routes the three entry points here on top
+of tests/abi_double.py (through `abi_double.install`), so the unmodified host code
 runs without a GPU.
 """
 import numpy as np
 
 import abi_double as d
-from elfi_b200 import _lib
 
 D_MAX = 256
 
@@ -137,24 +136,6 @@ def regadj_adjust_f64(ctx, S, ldS, N, q, obs, T, ldT, p, flags, cols_host, pg, s
     res[:] = adj.T
 
 
-_TABLE = {'elfi_b200_regadj_mask_f64': regadj_mask_f64,
-          'elfi_b200_regadj_moments_f64': regadj_moments_f64,
-          'elfi_b200_regadj_adjust_f64': regadj_adjust_f64}
-
-
-def install(monkeypatch):
-    """Route the regression-adjustment entry points here, everything else to the installed
-    _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_regadj_mask_f64': regadj_mask_f64,
+         'elfi_b200_regadj_moments_f64': regadj_moments_f64,
+         'elfi_b200_regadj_adjust_f64': regadj_adjust_f64}

@@ -6,13 +6,12 @@ INFRASTRUCTURE ONLY.
 a constant column by _is_constant_feature).  `fit` solves liblinear's primal with a penalised
 intercept to the header's stopping rule: an exact Newton solve for L2, and for L1 proximal Newton
 with coordinate descent on the quadratic model.  `objective` and `subgradient_norm` state F and the
-optimality measure.  `install` routes both entry points here on top of tests/abi_double.py, so the
+optimality measure.  `TABLE` routes both entry points here on top of tests/abi_double.py, so the
 unmodified classifier and BOLFIRE host code run without a GPU.
 """
 import numpy as np
 
 import abi_double as d
-from elfi_b200 import _lib
 
 EPS = np.finfo(np.float64).eps
 TOL = 1e-10
@@ -173,23 +172,5 @@ def logreg_predict_f64(ctx, block, dim, Xq, ld_row, m, class_min, out, stream):
     d._vec(out, m)[:] = v
 
 
-_TABLE = {'elfi_b200_logreg_fit_f64': logreg_fit_f64,
-          'elfi_b200_logreg_predict_f64': logreg_predict_f64}
-
-
-def install(monkeypatch):
-    """Route the two logistic-regression entry points here, everything else to the installed
-    _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_logreg_fit_f64': logreg_fit_f64,
+         'elfi_b200_logreg_predict_f64': logreg_predict_f64}

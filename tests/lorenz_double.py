@@ -1,6 +1,6 @@
 """CPU test double of the Lorenz entry points -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py (installed first, by the `cpu_double` fixture) with restatements of
+Extends tests/abi_double.py (through `abi_double.install`) with restatements of
 elfi_b200_sim_lorenz_f64 and elfi_b200_lorenz_summaries_f64 on host pointers.  The summaries are the
 reference's NumPy code (elfi_b200.examples.lorenz on host arrays); the simulator is the reference's
 recurrence on normals from a NumPy RandomState instead of the device's Philox streams (same
@@ -10,7 +10,7 @@ summaries are those of exactly the data the unfused form writes, as on the devic
 import numpy as np
 
 import abi_double as d
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 
 def lorenz_data(P, init, T, f, phi, s_phi, dt, rs):
@@ -64,21 +64,4 @@ def lorenz_summaries_f64(ctx, X, ld_row, ld_t, ld_k, B, n_timestep, n_obs, S, ld
     d._mat(S, B, 6, ldS)[:] = _summaries(np.ascontiguousarray(x))
 
 
-_TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_lorenz_f64, lorenz_summaries_f64)}
-
-
-def install(monkeypatch):
-    """Route the Lorenz entry points here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_lorenz_f64, lorenz_summaries_f64)}

@@ -1,6 +1,6 @@
 """CPU test double of the Lotka-Volterra entry points -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py (installed first, by the `cpu_double` fixture) with restatements of
+Extends tests/abi_double.py (through `abi_double.install`) with restatements of
 elfi_b200_sim_lotka_volterra_f64 and elfi_b200_lv_summaries_f64 on host pointers.  The summaries
 are the reference's NumPy code (elfi_b200.examples.lotka_volterra on host arrays); the simulator is
 the reference's lotka_volterra() on a NumPy RandomState instead of the device's Philox streams (same
@@ -10,7 +10,7 @@ parameters, and rows that need more than max_events events (n_events = max_event
 import numpy as np
 
 import abi_double as d
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 
 def lv_data(P, n_obs, time_end, max_events, rs):
@@ -63,21 +63,4 @@ def lv_summaries_f64(ctx, X, ld_row, ld_obs, ld_species, B, n_obs, S, ldS, strea
     d._mat(S, B, ops.LV_NSUMM, ldS)[:] = np.column_stack(cols)
 
 
-_TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_lotka_volterra_f64, lv_summaries_f64)}
-
-
-def install(monkeypatch):
-    """Route the Lotka-Volterra entry points here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_lotka_volterra_f64, lv_summaries_f64)}

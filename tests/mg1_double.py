@@ -1,11 +1,11 @@
 """CPU test double of the M/G/1 and conditional-prior entry points -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py and tests/priors_double.py (installed first) with restatements, on host
-pointers, of elfi_b200_sim_mg1_f64 and elfi_b200_row_quantiles_f64 (the reference's recurrence and
-np.quantile; uniforms from a NumPy RandomState instead of the device's Philox streams, same
-distribution, deterministic in (seed, offset)) and of elfi_b200_prior_rvs_cond_f64,
-elfi_b200_prior_logpdf_cond_f64 and the mixture proposals with support 4 (SciPy draws and densities
-with per-row loc / scale).
+Extends tests/abi_double.py and tests/priors_double.py (TABLE goes after theirs) with
+restatements, on host pointers, of elfi_b200_sim_mg1_f64 and elfi_b200_row_quantiles_f64 (the
+reference's recurrence and np.quantile; uniforms from a NumPy RandomState instead of the device's
+Philox streams, same distribution, deterministic in (seed, offset)) and of
+elfi_b200_prior_rvs_cond_f64, elfi_b200_prior_logpdf_cond_f64 and the mixture proposals with
+support 4 (SciPy draws and densities with per-row loc / scale).
 """
 import numpy as np
 import scipy.stats as ss
@@ -14,7 +14,7 @@ import abi_double as d
 import conditional_prior_replay as cr
 import prior_replay as pr
 import priors_double
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 
 def mg1_data(P, n, rs):
@@ -120,23 +120,5 @@ def gm_rvs_cdf_f64(ctx, means, ldm, cumw, N, p, Lchol_host, B, seed, offset, sup
             break
 
 
-_TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_mg1_f64, row_quantiles_f64, prior_rvs_cond_f64,
-                                                  prior_logpdf_cond_f64, gm_rvs_cdf_f64)}
-
-
-def install(monkeypatch):
-    """Route the M/G/1 and conditional-prior entry points here (support 4 of the proposals
-    included), everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_mg1_f64, row_quantiles_f64, prior_rvs_cond_f64,
+                                                 prior_logpdf_cond_f64, gm_rvs_cdf_f64)}

@@ -1,6 +1,6 @@
 """CPU test double of the stock-prior entry points -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py (installed first, by the `cpu_double` fixture) with restatements of
+Extends tests/abi_double.py (through `abi_double.install`) with restatements of
 elfi_b200_prior_rvs_f64, elfi_b200_prior_logpdf_f64 and the mixture proposals with support 3
 (the prior table) on host pointers: scipy.stats draws and densities instead of the device's
 Philox streams, so only statistical assertions apply.  Every other call goes to abi_double
@@ -11,7 +11,7 @@ import scipy.stats as ss
 
 import abi_double as d
 import prior_replay as pr
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 
 def _table(spec_host, p):
@@ -60,23 +60,5 @@ def gm_rvs_cdf_f64(ctx, means, ldm, cumw, N, p, Lchol_host, B, seed, offset, sup
             break
 
 
-_TABLE = {'elfi_b200_prior_rvs_f64': prior_rvs_f64, 'elfi_b200_prior_logpdf_f64': prior_logpdf_f64,
-          'elfi_b200_gm_rvs_cdf_f64': gm_rvs_cdf_f64}
-
-
-def install(monkeypatch):
-    """Route the stock-prior entry points here, everything else to abi_double.call (which
-    `cpu_double` has installed as elfi_b200._lib.call)."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_prior_rvs_f64': prior_rvs_f64, 'elfi_b200_prior_logpdf_f64': prior_logpdf_f64,
+         'elfi_b200_gm_rvs_cdf_f64': gm_rvs_cdf_f64}

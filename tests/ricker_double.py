@@ -1,6 +1,6 @@
 """CPU test double of the Ricker entry points -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py (installed first, by the `cpu_double` fixture) with restatements of
+Extends tests/abi_double.py (through `abi_double.install`) with restatements of
 elfi_b200_poisson_f64, elfi_b200_sim_ricker_f64, elfi_b200_count_zeros_f64 and
 elfi_b200_chi_squared_f64 on host pointers.  The summaries and chi_squared are the reference's
 NumPy code (elfi_b200.examples.ricker on host arrays); the simulators draw from a NumPy
@@ -11,7 +11,7 @@ those of exactly the data the unfused form writes, as on the device.
 import numpy as np
 
 import abi_double as d
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 
 def _poisson(lam, rs):
@@ -85,22 +85,5 @@ def chi_squared_f64(ctx, S, ldS, B, K, obs, out, stream):
             d._vec(out, B)[:] = ricker.chi_squared(*sim.T, observed=tuple(o[:, None]))
 
 
-_TABLE = {'elfi_b200_' + f.__name__: f for f in (
+TABLE = {'elfi_b200_' + f.__name__: f for f in (
     poisson_f64, sim_ricker_f64, count_zeros_f64, chi_squared_f64)}
-
-
-def install(monkeypatch):
-    """Route the Ricker entry points here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)

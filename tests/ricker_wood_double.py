@@ -1,12 +1,12 @@
 """CPU test double of elfi_b200_ricker_wood_f64 -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py (installed first, by the `cpu_double` fixture) with a restatement of
+Extends tests/abi_double.py (through `abi_double.install`) with a restatement of
 Wood's 13 Ricker statistics on host pointers: the NumPy definition of
 elfi_b200.examples.ricker.wood_statistics on the rows of Y and the design P the call passes, with
 the kernel's argument checks.
 """
 import abi_double as d
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 
 def ricker_wood_f64(ctx, Y, ldY, B, n, P, out, ld_out, stream):
@@ -20,21 +20,4 @@ def ricker_wood_f64(ctx, Y, ldY, B, n, P, out, ld_out, stream):
         d._mat(Y, B, n, ldY).copy(), d._mat(P, 3, n - 1).copy())
 
 
-_TABLE = {'elfi_b200_' + f.__name__: f for f in (ricker_wood_f64,)}
-
-
-def install(monkeypatch):
-    """Route elfi_b200_ricker_wood_f64 here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_' + f.__name__: f for f in (ricker_wood_f64,)}

@@ -4,15 +4,14 @@ test double -- TEST INFRASTRUCTURE ONLY.
 The functions state each kernel's definition on host arrays: `nm_init` / `nm_step` the lock-step
 Nelder-Mead state machine (scipy's _minimize_neldermead, one point per call, stable vertex order
 with NaN last), `ls_init` / `ls_step` the line search, `box_sample` the Philox box draws,
-`weights` and `posterior_unnorm`.  `install` routes the entry points here on top of
-tests/abi_double.py (installed first, by the `cpu_double` fixture), so the unmodified ROMC host code
+`weights` and `posterior_unnorm`.  `TABLE` routes the entry points here on top of
+tests/abi_double.py (through `abi_double.install`), so the unmodified ROMC host code
 runs without a GPU.
 """
 import numpy as np
 
 import abi_double as d
 import streams
-from elfi_b200 import _lib
 
 INIT, REFLECT, EXPAND, CONTRACT_OUT, CONTRACT_IN, SHRINK, DONE = range(7)
 NM_INTS = 8
@@ -344,26 +343,9 @@ def posterior_unnorm_f64(ctx, M, R, p, theta, ld_theta, center, rot_inv, limits,
     d._vec(out, M)[:] = res
 
 
-_TABLE = {'elfi_b200_romc_nm_init_f64': nm_init_f64,
-          'elfi_b200_romc_nm_step_f64': nm_step_f64,
-          'elfi_b200_romc_line_search_f64': line_search_f64,
-          'elfi_b200_romc_box_sample_f64': box_sample_f64,
-          'elfi_b200_romc_weights_f64': weights_f64,
-          'elfi_b200_romc_posterior_unnorm_f64': posterior_unnorm_f64}
-
-
-def install(monkeypatch):
-    """Route the ROMC entry points here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_romc_nm_init_f64': nm_init_f64,
+         'elfi_b200_romc_nm_step_f64': nm_step_f64,
+         'elfi_b200_romc_line_search_f64': line_search_f64,
+         'elfi_b200_romc_box_sample_f64': box_sample_f64,
+         'elfi_b200_romc_weights_f64': weights_f64,
+         'elfi_b200_romc_posterior_unnorm_f64': posterior_unnorm_f64}

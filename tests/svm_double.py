@@ -1,17 +1,18 @@
 """CPU test double of the stochastic volatility entry point -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py and tests/priors_double.py (installed first) with a restatement, on
-host pointers, of elfi_b200_sim_svm_f64: the reference's arithmetic (SciPy's levy_stable formula in
-S0 and the AR(1) log-volatility) on uniforms and normals from a NumPy RandomState instead of the
-device's Philox streams (same distribution, deterministic in (seed, offset)), and the kurt / skew of
-np.quantile.  elfi_b200_row_quantiles_f64 comes from tests/mg1_double.py.
+Extends tests/abi_double.py and tests/priors_double.py (TABLE goes after theirs) with a
+restatement, on host pointers, of elfi_b200_sim_svm_f64: the reference's arithmetic (SciPy's
+levy_stable formula in S0 and the AR(1) log-volatility) on uniforms and normals from a NumPy
+RandomState instead of the device's Philox streams (same distribution, deterministic in
+(seed, offset)), and the kurt / skew of np.quantile.  elfi_b200_row_quantiles_f64 comes from
+tests/mg1_double.py.
 """
 import numpy as np
 
 import abi_double as d
 import mg1_double
 import svm_replay
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 
 def svm_data(P, n, rs):
@@ -46,23 +47,5 @@ def sim_svm_f64(ctx, P, ldP, B, n_obs, seed, offset, Y, ldY, S, ldS, stream):
         d._mat(S, B, 2, ldS)[:] = summaries(y)
 
 
-_TABLE = {'elfi_b200_sim_svm_f64': sim_svm_f64,
-          'elfi_b200_row_quantiles_f64': mg1_double.row_quantiles_f64}
-
-
-def install(monkeypatch):
-    """Route the stochastic volatility entry point and row_quantiles here, everything else to the
-    installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_sim_svm_f64': sim_svm_f64,
+         'elfi_b200_row_quantiles_f64': mg1_double.row_quantiles_f64}

@@ -30,10 +30,42 @@ def test_library_exports_every_header_symbol():
 
 
 def test_binding_covers_header():
+    """Every prototype parses into known ctypes, one per declared parameter; each type class maps
+    as the header declares it."""
     from elfi_b200 import _lib
     assert sorted(_lib.SIGNATURES) == header_functions()
+    text = re.sub(r'/\*.*?\*/', '', open(_lib.HEADER_PATH).read(), flags=re.S)
+    known = {ctypes.c_void_p, ctypes.c_char_p, ctypes.c_int, ctypes.c_int64, ctypes.c_uint64,
+             ctypes.c_double}
+    for name, argtypes in _lib.SIGNATURES.items():
+        params = re.search(name + r'\s*\(([^)]*)\)', text).group(1).strip()
+        assert len(argtypes) == (0 if params == 'void' else params.count(',') + 1), name
+        assert set(argtypes) | {_lib._RESTYPES[name]} <= known, name
+    assert _lib._RESTYPES['elfi_b200_last_error'] is ctypes.c_char_p
+    assert _lib._RESTYPES['elfi_b200_gp_padded_size'] is ctypes.c_int64
+    assert _lib.SIGNATURES['elfi_b200_gp_padded_size'] == [ctypes.c_int64]
+    assert _lib._RESTYPES['elfi_b200_dist_euclid_thr_f64'] is ctypes.c_int
+    # (ctx, P, ldP, n_params, B, n_obs, double stock_init, uint64_t seed, uint64_t offset, Y, ...)
+    ricker = _lib.SIGNATURES['elfi_b200_sim_ricker_f64']
+    assert ricker[:9] == [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int64] * 4 + [
+        ctypes.c_double, ctypes.c_uint64, ctypes.c_uint64]
+    # (ctx, int32_t metric, double pexp, const double* S, int64_t ldS, ...)
+    assert _lib.SIGNATURES['elfi_b200_dist_metric_thr_f64'][:5] == [
+        ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_void_p, ctypes.c_int64]
     lib = _lib.load()
-    assert lib.elfi_b200_version() == 100
+    assert lib.elfi_b200_version() == _lib.CONSTANTS['VERSION'] == 100
+
+
+def test_constants_cover_header_macros():
+    """Every object-like ELFI_B200_ macro but the include guard is in CONSTANTS, int or float as
+    its literal is written."""
+    from elfi_b200 import _lib
+    text = re.sub(r'/\*.*?\*/', '', open(_lib.HEADER_PATH).read(), flags=re.S)
+    names = re.findall(r'^\s*#\s*define\s+ELFI_B200_(\w+)(?!\w|\()', text, re.M)
+    assert sorted(_lib.CONSTANTS) == sorted(n for n in names if n != 'H')
+    assert _lib.CONSTANTS['ERR_ARG'] == -1 and _lib.CONSTANTS['TOAD_CELLS_MAX'] == 2 ** 31
+    assert isinstance(_lib.CONSTANTS['POISSON_LAM_MAX'], float)
+    assert all(type(v) is int for k, v in _lib.CONSTANTS.items() if k != 'POISSON_LAM_MAX')
 
 
 def test_fails_loudly_without_gpu():

@@ -139,10 +139,10 @@ def test_step_and_distance_equal_numpy_and_scipy(harness):
 # ---------------------------------------------------------------------------- Python layer
 @pytest.fixture
 def ar1_double(cpu_double, monkeypatch):
+    import abi_double
     import ar1_double
     import priors_double
-    priors_double.install(monkeypatch)
-    ar1_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE, ar1_double.TABLE)
     return cpu_double
 
 

@@ -203,10 +203,10 @@ def test_summaries_equal_golden_crafted_rows(harness):
 # ---------------------------------------------------------------------------- Python layer
 @pytest.fixture
 def arch_double(cpu_double, monkeypatch):
+    import abi_double
     import arch_double
     import priors_double
-    priors_double.install(monkeypatch)
-    arch_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE, arch_double.TABLE)
     return cpu_double
 
 

@@ -261,10 +261,10 @@ def test_external_operation_completed_process_and_check(tmp_path):
 # ---------------------------------------------------------------------------- Python layer
 @pytest.fixture
 def bdm_double(cpu_double, monkeypatch):
+    import abi_double
     import bdm_double
     import priors_double
-    priors_double.install(monkeypatch)
-    bdm_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE, bdm_double.TABLE)
     return cpu_double
 
 

@@ -3,6 +3,7 @@ reference's marginal data and prior-drawn rounds (tests/golden/gen_golden_bolfir
 round's value is the optimum of its classifier."""
 import numpy as np
 
+import abi_double
 import logreg_double
 from elfi_b200.bolfire import BOLFIRE
 from elfi_b200.examples import arch
@@ -19,7 +20,7 @@ def run(g):
 
 
 def test_rounds_match_reference(cpu_double, monkeypatch, golden):
-    logreg_double.install(monkeypatch)
+    abi_double.install(monkeypatch, logreg_double.TABLE)
     g = golden('bolfire_rounds')
     bolfire, post = run(g)
     np.testing.assert_array_equal(bolfire.observed, g['observed'])
@@ -43,7 +44,7 @@ def test_rounds_match_reference(cpu_double, monkeypatch, golden):
 
 def test_host_classifier(cpu_double, monkeypatch, golden):
     """A user Classifier gets NumPy (X, y) of the round's simulations then the marginal data."""
-    logreg_double.install(monkeypatch)
+    abi_double.install(monkeypatch, logreg_double.TABLE)
     g = golden('bolfire_rounds')
     seen = []
 

@@ -4,6 +4,7 @@ mode's host logic runs end to end with the NumPy restatement of elfi_b200_bsl_mh
 import numpy as np
 import pytest
 
+import abi_double
 import bsl_chains_double
 import bsl_double
 import priors_double
@@ -25,13 +26,13 @@ def _record_groups(monkeypatch):
     def synlik_f64(*args):
         groups.append(args[4])
         return bsl_double.synlik_f64(*args)
-    monkeypatch.setitem(bsl_double._TABLE, 'elfi_b200_synlik_f64', synlik_f64)
+    monkeypatch.setitem(bsl_double.TABLE, 'elfi_b200_synlik_f64', synlik_f64)
     return groups
 
 
 def test_parity_chains_match_restatement(cpu_double, monkeypatch):
     groups = _record_groups(monkeypatch)
-    bsl_double.install(monkeypatch)
+    abi_double.install(monkeypatch, bsl_double.TABLE)
     n, n_round, b, seed = 40, 100, 50, 17
     sampler = bsl.BSL(_model(), n_round, ['MA2'], batch_size=b, seed=seed)
     res = sampler.sample(n, SIGMA_WIDE, params0=PARAMS0, burn_in=5, logit_transform_bound=BOUNDS,
@@ -58,7 +59,7 @@ def test_parity_chains_match_restatement(cpu_double, monkeypatch):
 
 
 def test_parity_chains_without_bounds_and_prior_start(cpu_double, monkeypatch):
-    bsl_double.install(monkeypatch)
+    abi_double.install(monkeypatch, bsl_double.TABLE)
     sigma = np.array([[.02, .01], [.01, .02]])
     sampler = bsl.BSL(_model(), 100, ['MA2'], seed=3)
     res = sampler.sample(12, sigma, n_chains=4)
@@ -74,7 +75,7 @@ def test_parity_chains_without_bounds_and_prior_start(cpu_double, monkeypatch):
 
 def test_one_chain_is_the_single_chain_sampler(cpu_double, monkeypatch):
     """n_chains=1 is the same code path: the restatement with C = 1 is the reference's chain."""
-    bsl_double.install(monkeypatch)
+    abi_double.install(monkeypatch, bsl_double.TABLE)
     sampler = bsl.BSL(_model(), 100, ['MA2'], batch_size=50, seed=9)
     res = sampler.sample(15, SIGMA_WIDE, params0=[.6, .2], logit_transform_bound=BOUNDS)
     chains, lp, acc, n_batches = bsl_chains_double.parity_chains(
@@ -87,7 +88,7 @@ def test_one_chain_is_the_single_chain_sampler(cpu_double, monkeypatch):
 
 
 def test_argument_errors(cpu_double, monkeypatch):
-    bsl_double.install(monkeypatch)
+    abi_double.install(monkeypatch, bsl_double.TABLE)
     sigma = np.array([[.02, .01], [.01, .02]])
     with pytest.raises(ValueError, match=r'params0 must be \(2,\) or \(3, 2\)'):
         bsl.BSL(_model(), 100, ['MA2'], seed=1).sample(5, sigma, params0=np.zeros((2, 2)),
@@ -103,9 +104,7 @@ def test_argument_errors(cpu_double, monkeypatch):
 
 
 def test_throughput_mode_host_logic(cpu_double, monkeypatch):
-    bsl_double.install(monkeypatch)
-    priors_double.install(monkeypatch)
-    bsl_chains_double.install(monkeypatch)
+    abi_double.install(monkeypatch, bsl_double.TABLE, priors_double.TABLE, bsl_chains_double.TABLE)
     m, dp = ma2.get_uniform_device_model(n_obs=20, seed_obs=4)
     sigma = np.diag([.05, .05])
 

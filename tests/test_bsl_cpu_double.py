@@ -3,6 +3,7 @@ chains, penalty selection and whitening matrix (tests/golden/gen_golden_bsl.py).
 import numpy as np
 import pytest
 
+import abi_double
 import bsl_double
 from elfi_b200 import bsl
 from elfi_b200.examples import ma2
@@ -42,7 +43,7 @@ def check_chain(name, g, sampler, res):
 
 @pytest.mark.parametrize('name', ['standard', 'unbiased', 'bounded', 'whitened'])
 def test_chain_matches_reference(cpu_double, monkeypatch, golden, name):
-    bsl_double.install(monkeypatch)
+    abi_double.install(monkeypatch, bsl_double.TABLE)
     g = golden('bsl_chains')
     sampler, res = run_chain(name, g)
     check_chain(name, g, sampler, res)
@@ -52,7 +53,7 @@ def test_chain_matches_reference(cpu_double, monkeypatch, golden, name):
 
 
 def test_whitening_matrix_and_penalty(cpu_double, monkeypatch, golden):
-    bsl_double.install(monkeypatch)
+    abi_double.install(monkeypatch, bsl_double.TABLE)
     g = golden('bsl_chains')
     W = bsl.estimate_whitening_matrix(_model(), 5000, np.array([.6, .2]), ['MA2'], seed=1)
     np.testing.assert_array_equal(W, g['W'])
@@ -65,7 +66,7 @@ def test_whitening_matrix_and_penalty(cpu_double, monkeypatch, golden):
 
 
 def test_params0_outside_support_and_host_callable(cpu_double, monkeypatch):
-    bsl_double.install(monkeypatch)
+    abi_double.install(monkeypatch, bsl_double.TABLE)
     with pytest.raises(ValueError, match='outside prior support'):
         bsl.BSL(_model(), 100, ['MA2'], seed=1).sample(5, SIGMA, params0=[0.5, -0.9])
     seen = []

@@ -3,6 +3,7 @@ against the reference's pdf_methods, the logit transform of the proposals, and a
 import numpy as np
 import pytest
 
+import abi_double
 import bsl_double
 from elfi_b200 import bsl, ops
 from elfi_b200.examples import ma2
@@ -85,7 +86,7 @@ def test_bsl_argument_errors():
 
 
 def test_synlik_argument_errors(cpu_double, monkeypatch):
-    bsl_double.install(monkeypatch)
+    abi_double.install(monkeypatch, bsl_double.TABLE)
     rs = np.random.RandomState(2)
     S, y = rs.randn(20, 3), np.zeros(3)
     with pytest.raises(ValueError, match=r'\[0, 1\]'):

@@ -244,10 +244,10 @@ def test_conditional_device_model_prior_refusals():
 # ---------------------------------------------------------------------------- ops validation
 @pytest.fixture
 def cond_double(cpu_double, monkeypatch):
+    import abi_double
     import mg1_double
     import priors_double
-    priors_double.install(monkeypatch)
-    mg1_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE, mg1_double.TABLE)
     return cpu_double
 
 

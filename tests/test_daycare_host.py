@@ -284,10 +284,10 @@ def test_replay_matches_header(harness):
 # ---------------------------------------------------------------------------- Python layer
 @pytest.fixture
 def dc_double(cpu_double, monkeypatch):
+    import abi_double
     import daycare_double
     import priors_double
-    priors_double.install(monkeypatch)
-    daycare_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE, daycare_double.TABLE)
     return cpu_double
 
 

@@ -6,6 +6,7 @@ from functools import partial
 import numpy as np
 import pytest
 
+import abi_double
 import diagnostics_double
 from conftest import load_golden
 from elfi_b200 import TwoStageSelection, diagnostics
@@ -66,7 +67,7 @@ def close(a, b, tol=1e-10):
 
 @pytest.fixture
 def double(cpu_double, monkeypatch):
-    diagnostics_double.install(monkeypatch)
+    abi_double.install(monkeypatch, diagnostics_double.TABLE)
     return cpu_double
 
 

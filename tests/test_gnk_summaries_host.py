@@ -133,10 +133,10 @@ def test_bignk_rejection_matches_reference_golden(cpu_double):
 
 @pytest.fixture
 def gnk_double(cpu_double, monkeypatch):
+    import abi_double
     import gnk_double
     import priors_double
-    priors_double.install(monkeypatch)
-    gnk_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE, gnk_double.TABLE)
     return cpu_double
 
 

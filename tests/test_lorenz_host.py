@@ -186,10 +186,10 @@ def test_header_summaries_nan_inf_constant(harness):
 # ---------------------------------------------------------------------------- Python layer
 @pytest.fixture
 def lorenz_double(cpu_double, monkeypatch):
+    import abi_double
     import lorenz_double
     import priors_double
-    priors_double.install(monkeypatch)
-    lorenz_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE, lorenz_double.TABLE)
     return cpu_double
 
 

@@ -243,10 +243,10 @@ def test_header_summaries_match_numpy_every_n(harness):
 # ---------------------------------------------------------------------------- Python layer
 @pytest.fixture
 def lv_double(cpu_double, monkeypatch):
+    import abi_double
     import lv_double
     import priors_double
-    priors_double.install(monkeypatch)
-    lv_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE, lv_double.TABLE)
     return cpu_double
 
 

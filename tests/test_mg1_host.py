@@ -201,10 +201,10 @@ def test_quantile_picks_equal_numpy_for_every_n(harness):
 # ---------------------------------------------------------------------------- Python layer
 @pytest.fixture
 def mg1_double(cpu_double, monkeypatch):
+    import abi_double
     import mg1_double
     import priors_double
-    priors_double.install(monkeypatch)
-    mg1_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE, mg1_double.TABLE)
     return cpu_double
 
 

@@ -5,6 +5,7 @@ import warnings
 import numpy as np
 import pytest
 
+import abi_double
 import linadjust_double
 from post_processing_cases import case, check_case, close, statistics
 from elfi_b200 import adjust_posterior, results
@@ -18,7 +19,7 @@ def _cases():
 
 @pytest.mark.parametrize('name', _cases())
 def test_goldens(cpu_double, monkeypatch, golden, name):
-    linadjust_double.install(monkeypatch)
+    abi_double.install(monkeypatch, linadjust_double.TABLE)
     g = golden('post_processing')
     sample, model, snames, pnames = case(g, name)
     adj = LinearAdjustment()
@@ -39,7 +40,7 @@ def test_goldens(cpu_double, monkeypatch, golden, name):
 
 
 def test_functional_goldens(cpu_double, monkeypatch, golden):
-    linadjust_double.install(monkeypatch)
+    abi_double.install(monkeypatch, linadjust_double.TABLE)
     from elfi_b200.examples import ma2
     g = golden('post_processing')
     m = ma2.get_model(true_params=[0.6, 0.2], seed_obs=20170511)
@@ -53,7 +54,7 @@ def test_functional_goldens(cpu_double, monkeypatch, golden):
 
 
 def test_all_dropped_raises(cpu_double, monkeypatch, golden):
-    linadjust_double.install(monkeypatch)
+    abi_double.install(monkeypatch, linadjust_double.TABLE)
     sample, model, snames, pnames = case(golden('post_processing'), 'q2p3')
     sample.outputs['t1'] = np.full_like(sample.outputs['t1'], np.nan)
     with pytest.raises(ValueError, match='n_samples = 0'):

@@ -281,8 +281,9 @@ def _vector_model():
 # ------------------------------------------------------------------------------ samplers (double)
 @pytest.fixture
 def prior_double(cpu_double, monkeypatch):
+    import abi_double
     import priors_double
-    priors_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE)
     return cpu_double
 
 

@@ -179,10 +179,10 @@ def test_rejection_matches_reference_golden(cpu_double, variant):
 # ---------------------------------------------------------------------------- Python layer
 @pytest.fixture
 def ricker_double(cpu_double, monkeypatch):
+    import abi_double
     import priors_double
     import ricker_double
-    priors_double.install(monkeypatch)
-    ricker_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE, ricker_double.TABLE)
     return cpu_double
 
 

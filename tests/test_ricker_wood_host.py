@@ -115,13 +115,16 @@ def test_get_model_wood_node_and_argument_errors():
 # ---------------------------------------------------------------------------- Python layer
 @pytest.fixture
 def wood_double(cpu_double, monkeypatch):
+    import abi_double
+    abi_double.install(monkeypatch, *_wood_tables())
+    return cpu_double
+
+
+def _wood_tables():
     import priors_double
     import ricker_double
     import ricker_wood_double
-    priors_double.install(monkeypatch)
-    ricker_double.install(monkeypatch)
-    ricker_wood_double.install(monkeypatch)
-    return cpu_double
+    return priors_double.TABLE, ricker_double.TABLE, ricker_wood_double.TABLE
 
 
 def test_device_model_arguments(wood_double):
@@ -166,10 +169,11 @@ def test_dispatch_host_device_and_lazy_agree(wood_double):
 
 
 def test_bsl_on_the_host_model(wood_double, monkeypatch):
+    import abi_double
     import bsl_double
     from elfi_b200 import bsl
     from elfi_b200.examples import ricker
-    bsl_double.install(monkeypatch)
+    abi_double.install(monkeypatch, *_wood_tables(), bsl_double.TABLE)
     m = ricker.get_model(seed_obs=4, summary='wood')
     # the statistics' variances span ~16 orders of magnitude, beyond the likelihood's pivot cut
     # (relative to the largest variance): without a common scale every round gives -inf

@@ -6,6 +6,7 @@ import pytest
 
 import elfi_b200
 import romc_cases
+import abi_double
 import romc_double
 from elfi_b200 import device as dev, ops, romc
 from elfi_b200.examples import ma2
@@ -27,7 +28,7 @@ def _case(name):
 
 @pytest.mark.parametrize('name', ['oned', 'ma2'])
 def test_host_path_matches_reference(cpu_double, monkeypatch, golden, name):
-    romc_double.install(monkeypatch)
+    abi_double.install(monkeypatch, romc_double.TABLE)
     g = {k[len(name) + 1:]: v for k, v in golden('romc').items() if k.startswith(name + '_')}
     r, n1, seed = _case(name)
     assert not r.on_device
@@ -66,7 +67,7 @@ def test_host_path_matches_reference(cpu_double, monkeypatch, golden, name):
 
 def test_reference_functional_example(cpu_double, monkeypatch):
     """The reference's test_romc1 assertions on its one-parameter example."""
-    romc_double.install(monkeypatch)
+    abi_double.install(monkeypatch, romc_double.TABLE)
     m, dname = romc_cases.one_d_model(elfi_b200)
     r = romc.ROMC(m[dname], [(-2.5, 2.5)])
     r.solve_problems(n1=100, seed=21)
@@ -86,7 +87,7 @@ def test_reference_functional_example(cpu_double, monkeypatch):
 
 
 def test_argument_errors(cpu_double, monkeypatch):
-    romc_double.install(monkeypatch)
+    abi_double.install(monkeypatch, romc_double.TABLE)
     m, dname = romc_cases.one_d_model(elfi_b200)
     with pytest.raises(NotImplementedError):
         romc.ROMC(m[dname], custom_optim_class=object)
@@ -125,7 +126,7 @@ def test_local_fit_matches_reference_linear_regression(golden, case):
 def test_unnorm_posterior_without_local_models(cpu_double, monkeypatch):
     """Without local models a region counts where its own objective is <= eps (no containment),
     as RomcPosterior._sum_over_indicators; only the regions' columns of each batch are kept."""
-    romc_double.install(monkeypatch)
+    abi_double.install(monkeypatch, romc_double.TABLE)
     m, dname = romc_cases.one_d_model(elfi_b200)
     r = romc.ROMC(m[dname], [(-2.5, 2.5)])
     r.solve_problems(n1=20, seed=4)

@@ -18,8 +18,9 @@ def doubles(cpu_double, monkeypatch):
     """The segmented distances of testbench_double.py on top of the C ABI double, and the moments
     bound at the depth of the order the double restates: colmoments_f64's, for every route (the
     fused kernel's own order is checked on the device)."""
+    import abi_double
     import testbench_double
-    testbench_double.install(monkeypatch)
+    abi_double.install(monkeypatch, testbench_double.TABLE)
     monkeypatch.setattr(cases, 'moments_depth', lambda case, B, sm=None, optin=None:
                         cases.colmoments_depth(case.D, B, cpu_double.SM_COUNT))
 

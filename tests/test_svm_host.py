@@ -274,10 +274,10 @@ def test_summaries_equal_numpy_for_every_n(harness):
 # ---------------------------------------------------------------------------- Python layer
 @pytest.fixture
 def svm_double(cpu_double, monkeypatch):
+    import abi_double
     import priors_double
     import svm_double
-    priors_double.install(monkeypatch)
-    svm_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE, svm_double.TABLE)
     return cpu_double
 
 

@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 import torch
 
+import abi_double
 import bsl_chains_double
 import bsl_double
 import priors_double
@@ -23,10 +24,8 @@ SK = dict(n_samples=50, sigma_proposals=SIGMA, params0=np.array([.6, .2]))
 
 @pytest.fixture
 def double(cpu_double, monkeypatch):
-    bsl_double.install(monkeypatch)
-    bsl_chains_double.install(monkeypatch)
-    priors_double.install(monkeypatch)
-    testbench_bsl_double.install(monkeypatch)
+    abi_double.install(monkeypatch, bsl_double.TABLE, bsl_chains_double.TABLE,
+                                    priors_double.TABLE, testbench_bsl_double.TABLE)
     return cpu_double
 
 
@@ -112,7 +111,7 @@ def test_synlik_obs_double_shared_row_and_routing(double, monkeypatch):
     def record(*args):
         strides.append(args[8])
         return testbench_bsl_double.synlik_obs_f64(*args)
-    monkeypatch.setitem(testbench_bsl_double._TABLE, OBS_ENTRY, record)
+    monkeypatch.setitem(testbench_bsl_double.TABLE, OBS_ENTRY, record)
     shared = ops.synlik(S, dev.to_device(y)[None].expand(G, d)).cpu().numpy()
     assert strides == [0]                        # an expanded row is passed as ld_y = 0
     np.testing.assert_array_equal(shared, bsl_double.synlik(S, y))

@@ -11,6 +11,7 @@ from elfi_b200 import device as dev
 from elfi_b200 import ops
 from elfi_b200.examples import ma2 as exma2
 
+import abi_double
 import testbench_double
 
 SEG = ('elfi_b200_dist_seg_f64', 'elfi_b200_topn_merge_seg_f64')
@@ -27,7 +28,7 @@ METHODS = [
 
 @pytest.fixture
 def tb_double(cpu_double, monkeypatch):
-    testbench_double.install(monkeypatch)
+    abi_double.install(monkeypatch, testbench_double.TABLE)
     return cpu_double
 
 

@@ -188,10 +188,10 @@ def test_header_step_matches_scipy_formula(harness):
 # ---------------------------------------------------------------------------- Python layer
 @pytest.fixture
 def toad_double(cpu_double, monkeypatch):
+    import abi_double
     import priors_double
     import toad_double
-    priors_double.install(monkeypatch)
-    toad_double.install(monkeypatch)
+    abi_double.install(monkeypatch, priors_double.TABLE, toad_double.TABLE)
     return cpu_double
 
 

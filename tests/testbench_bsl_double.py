@@ -6,15 +6,14 @@ Both are stated as the existing doubles applied group by group or chain by chain
 * `bsl_mh_step_keyed_f64` runs tests/bsl_chains_double.py's mh_step for each chain slot c with
   the seed keys[c], on lanes[c] + 1 chains of which the one at index lanes[c] is slot c (the
   unkeyed step draws chain l's numbers on lane l).
-`install` routes both here on top of tests/abi_double.py (installed first, by the `cpu_double`
-fixture); tests/bsl_double.py and tests/bsl_chains_double.py route the unkeyed entry points.
+`TABLE` routes both here on top of tests/abi_double.py (through `abi_double.install`);
+tests/bsl_double.py and tests/bsl_chains_double.py route the unkeyed entry points.
 """
 import numpy as np
 
 import abi_double as d
 import bsl_chains_double
 import bsl_double
-from elfi_b200 import _lib
 
 
 def synlik_obs_f64(ctx, S, ld_row, ld_group, G, n, dim, Y, ld_y, W, estimator, penalties_host, K,
@@ -65,22 +64,5 @@ def bsl_mh_step_keyed_f64(ctx, C, p, t, n_samples, burn_in, b, keys, lanes, spec
             out[:, c * b:(c + 1) * b] = r[at][:, None]
 
 
-_TABLE = {'elfi_b200_synlik_obs_f64': synlik_obs_f64,
-          'elfi_b200_bsl_mh_step_keyed_f64': bsl_mh_step_keyed_f64}
-
-
-def install(monkeypatch):
-    """Route the two entry points here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_synlik_obs_f64': synlik_obs_f64,
+         'elfi_b200_bsl_mh_step_keyed_f64': bsl_mh_step_keyed_f64}

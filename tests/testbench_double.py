@@ -4,15 +4,14 @@ INFRASTRUCTURE ONLY.
 
 `dist_seg` measures segment r of S against observed row r with the oracle's cdist restatements;
 `topn_merge_seg` ranks each segment's [A_r; B_r] with a stable argsort (NaN last) and keeps the
-n_keep smallest rows of every output.  `install` routes both entry points here on top of
-tests/abi_double.py (installed first, by the `cpu_double` fixture), so the lock-step Testbench runs
+n_keep smallest rows of every output.  `TABLE` routes both entry points here on top of
+tests/abi_double.py (through `abi_double.install`), so the lock-step Testbench runs
 without a GPU.
 """
 import numpy as np
 
 import abi_double as d
 import elfi_oracle as o
-from elfi_b200 import _lib
 
 METRIC_NAMES = {0: 'euclidean', 1: 'sqeuclidean', 2: 'cityblock', 3: 'chebyshev', 4: 'minkowski'}
 
@@ -94,22 +93,5 @@ def topn_merge_seg_f64(ctx, R, keysA, ld_keysA, seg_keysA, nA, keysB, ld_keysB, 
         _seg(int(pd[k]), R, n_keep, w, int(ld[k]), int(sd[k]))[:] = top
 
 
-_TABLE = {'elfi_b200_dist_seg_f64': dist_seg_f64,
-          'elfi_b200_topn_merge_seg_f64': topn_merge_seg_f64}
-
-
-def install(monkeypatch):
-    """Route the segmented entry points here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_dist_seg_f64': dist_seg_f64,
+         'elfi_b200_topn_merge_seg_f64': topn_merge_seg_f64}

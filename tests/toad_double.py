@@ -1,6 +1,6 @@
 """CPU test double of the toad entry points -- TEST INFRASTRUCTURE ONLY.
 
-Extends tests/abi_double.py (installed first, by the `cpu_double` fixture) with restatements of
+Extends tests/abi_double.py (through `abi_double.install`) with restatements of
 elfi_b200_sim_toad_f64 and elfi_b200_toad_summaries_f64 on host pointers.  The summaries are the
 reference's NumPy code (elfi_b200.examples.toad on host arrays); the simulator is the reference's
 toad() on a NumPy RandomState instead of the device's Philox streams (same distribution,
@@ -10,7 +10,7 @@ are those of exactly the data the unfused form writes, as on the device.
 import numpy as np
 
 import abi_double as d
-from elfi_b200 import _lib, ops
+from elfi_b200 import ops
 
 
 def toad_data(P, n_toads, n_days, rs):
@@ -66,21 +66,4 @@ def toad_summaries_f64(ctx, X, ld_day, ld_toad, ld_row, n_days, n_toads, B, lag,
     d._mat(S, B, n_p + 1, ldS)[:] = _summaries(np.array(x), lag, d._vec(p, n_p).copy(), thd)
 
 
-_TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_toad_f64, toad_summaries_f64)}
-
-
-def install(monkeypatch):
-    """Route the toad entry points here, everything else to the installed _lib.call."""
-    base = _lib.call
-
-    def call(name, *args):
-        fn = _TABLE.get(name)
-        if fn is None:
-            return base(name, *args)
-        if len(args) != len(_lib.SIGNATURES[name]):
-            raise TypeError('{} takes {} arguments, got {}'.format(
-                name, len(_lib.SIGNATURES[name]), len(args)))
-        d.CALLS.append(name)
-        fn(*args)
-        return 0
-    monkeypatch.setattr(_lib, 'call', call)
+TABLE = {'elfi_b200_' + f.__name__: f for f in (sim_toad_f64, toad_summaries_f64)}
