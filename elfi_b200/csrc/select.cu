@@ -900,8 +900,10 @@ int elfi_b200_accept_append_f64(elfi_b200_ctx* ctx, const int32_t* acc_idx, cons
                                 int64_t ld_dst, int64_t capacity, int64_t* count, int64_t* dropped,
                                 void* stream_) {
     using namespace elfi;
-    ELFI_REQUIRE(ctx && n_acc && src_host && ld_src_host && width_host && dst && count,
-                 "accept_append: NULL argument");
+    // a buffer of capacity 0 has no storage (an empty allocation is a NULL pointer): every row
+    // is dropped and counted, nothing is written
+    ELFI_REQUIRE(ctx && n_acc && src_host && ld_src_host && width_host && (dst || capacity == 0) &&
+                 count, "accept_append: NULL argument");
     ELFI_REQUIRE(n_src >= 1 && n_src <= APPEND_MAX_SRC, "accept_append: 1..%d sources", APPEND_MAX_SRC);
     ELFI_REQUIRE(max_rows >= 0 && capacity >= 0, "accept_append: bad shape");
     AppendSources src;

@@ -498,14 +498,25 @@ class CandidateBuffer:
     def reset(self):
         self._counters.zero_()
 
+    @staticmethod
+    def _rows(sources):
+        """The sources as (B, width) views; the append reads width adjacent doubles per row, so a
+        view whose columns are not adjacent would be read in the wrong places and is refused."""
+        srcs = [_as_2d(t) for t in sources]
+        for t in srcs:
+            if t.shape[1] > 1 and t.stride(1) != 1:
+                raise ValueError('sources must have unit column stride, got strides {}'.format(
+                    tuple(t.stride())))
+        return srcs
+
     def _descriptors(self, sources):
         """ctypes descriptor arrays of a source list, cached while the same buffers come back
         (a sampler appends from the same output tensors batch after batch)."""
-        key = tuple((t.data_ptr(), tuple(t.shape), t.stride(0)) for t in sources)
+        key = tuple((t.data_ptr(), tuple(t.shape), tuple(t.stride())) for t in sources)
         cached = getattr(self, '_desc', None)
         if cached is not None and cached[0] == key:
             return cached[1]
-        srcs = [_as_2d(t) for t in sources]
+        srcs = self._rows(sources)
         if [t.shape[1] for t in srcs] != self.widths:
             raise ValueError('source widths do not match the buffer layout')
         n = len(srcs)
@@ -530,17 +541,26 @@ class CandidateBuffer:
         + append of the accepted rows [d | extras] to this buffer -- as a single library call
         (elfi_b200_rejection_batch_f64) with every argument marshalled once: microseconds of host
         time per batch, so that a busy host cannot starve a sub-millisecond kernel.  All tensors are device
-        tensors the caller keeps alive; `thresholds` is a host sequence or a device tensor."""
+        tensors the caller keeps alive; `thresholds` is a host sequence or a device tensor of K
+        float64 values (read at every call, so it may be updated in place between calls)."""
         S = _matrix(S)
         B, D = S.shape
         W = None if w is None else dev.to_device(w).reshape(-1, D)
         K = 1 if W is None else W.shape[0]
-        extras = [_as_2d(t) for t in extras]
+        extras = self._rows(extras)
         if [K] + [t.shape[1] for t in extras] != self.widths:
             raise ValueError('d / extra widths do not match the buffer layout')
+        if thresholds is None:
+            raise ValueError('bind_batch needs thresholds (a host sequence or a device tensor)')
         thr_dev = thresholds if dev.is_device_array(thresholds) else None
+        if thr_dev is not None and not (thr_dev.dtype == torch.float64 and thr_dev.is_contiguous()):
+            raise ValueError('device thresholds must be a contiguous float64 tensor (a converted '
+                             'copy would not see updates made in place)')
         thr_host = None if thr_dev is not None else np.ascontiguousarray(
             np.atleast_1d(thresholds), dtype=np.float64)
+        n_thr = thr_dev.numel() if thr_dev is not None else thr_host.size
+        if n_thr != K:
+            raise ValueError('need one threshold per distance column ({} != {})'.format(n_thr, K))
         n = len(extras)
         ptrs = (ctypes.c_void_p * max(n, 1))(*[t.data_ptr() for t in extras])
         lds = (ctypes.c_int64 * max(n, 1))(*[_ld(t) for t in extras])
@@ -557,8 +577,14 @@ class CandidateBuffer:
             _lib.call('elfi_b200_rejection_batch_f64', *args, dev.stream_ptr())
         return run
 
-    def best(self, n, key_col=0):
-        """(rows sorted by column key_col, first n; count, dropped) -- one D2H of the counters."""
+    def best(self, n, key_col=None):
+        """(rows sorted by column key_col, first n; count, dropped) -- one D2H of the counters.
+
+        The default key is the last column of the first source, the distance block: the
+        reference ranks nested distances by their last column (samplers.py:231-233).  Ties keep
+        the order in which the rows were appended."""
+        if key_col is None:
+            key_col = self.widths[0] - 1
         count, dropped = (int(v) for v in self._counters.cpu().tolist())
         keys = self.rows[:count, key_col].contiguous()
         perm = argsort(keys)

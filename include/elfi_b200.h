@@ -192,8 +192,9 @@ int elfi_b200_summary_meanvar_f64(elfi_b200_ctx* ctx, const double* X, int64_t l
  * == NULL: rows 0 .. *n_acc) of n_src <= 8 source arrays (src_host[k] = device pointer of a
  * (B, width_host[k]) array with leading dimension ld_src_host[k]; the three descriptor arrays
  * themselves are HOST arrays) are written side by side behind row *count of the packed candidate
- * buffer dst (capacity rows); *count += rows appended; rows that do not fit are dropped and
- * counted in *dropped (may be NULL).  n_acc, count, dropped are DEVICE int64.  max_rows bounds
+ * buffer dst (capacity rows; NULL when capacity is 0); *count += rows appended; rows that do not
+ * fit are dropped and counted in *dropped (may be NULL).  n_acc, count, dropped are DEVICE int64.
+ * ld_dst >= the total width; columns beyond it are left untouched.  max_rows bounds
  * *n_acc (sizes the launch).  The best n rows are taken once, when the population is extracted
  * (sort_pairs on the distance column + gather_rows) -- the same rows the reference's per-batch
  * argsort over n + batch_size rows leaves in its buffer (samplers.py:232-237).

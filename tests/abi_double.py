@@ -98,11 +98,19 @@ def dist_euclid_mom_f64(ctx, S, ldS, B, D, obs, W, K, thr_host, thr_dev, d_out, 
 
 def accept_append_f64(ctx, acc_idx, n_acc, max_rows, n_src, src_host, ld_src_host, width_host, dst,
                       ld_dst, capacity, count, dropped, stream):
-    n = int(_vec(n_acc, 1, np.int64)[0])
-    cnt = _vec(count, 1, np.int64)
+    _require(all(_addr(p) for p in (n_acc, src_host, ld_src_host, width_host, count)) and
+             (_addr(dst) or capacity == 0), 'accept_append: NULL argument')
+    _require(1 <= n_src <= 8, 'accept_append: 1..8 sources')
+    _require(max_rows >= 0 and capacity >= 0, 'accept_append: bad shape')
     ptrs = _vec(src_host, n_src, np.uint64)
     lds = _vec(ld_src_host, n_src, np.int64)
     wid = _vec(width_host, n_src, np.int64)
+    _require(all(ptrs) and all(wid >= 1) and all(lds >= wid), 'accept_append: bad source')
+    _require(int(wid.sum()) <= ld_dst, 'accept_append: ld_dst < total width')
+    if max_rows == 0:
+        return
+    n = int(_vec(n_acc, 1, np.int64)[0])
+    cnt = _vec(count, 1, np.int64)
     rows = min(n, max(0, capacity - int(cnt[0])))
     idx = _vec(acc_idx, max(n, 1), np.int32)[:rows] if _addr(acc_idx) else np.arange(rows)
     out = _mat(dst, capacity, ld_dst)
@@ -121,6 +129,10 @@ def accept_append_f64(ctx, acc_idx, n_acc, max_rows, n_src, src_host, ld_src_hos
 def rejection_batch_f64(ctx, S, ldS, B, D, obs, W, K, thr_host, thr_dev, d_out, acc_idx, n_acc, n_extra,
                         extra_host, ld_extra_host, width_extra_host, dst, ld_dst, capacity, count,
                         dropped, stream):
+    _require(all(_addr(p) for p in (acc_idx, n_acc, d_out)), 'rejection_batch: NULL argument')
+    _require(bool(_addr(thr_host)) != bool(_addr(thr_dev)),
+             'rejection_batch: thresholds on the host OR on the device')
+    _require(0 <= n_extra < 8, 'rejection_batch: 0..7 extra sources')
     thr = thr_host if _addr(thr_host) else thr_dev
     dist_euclid_thr_f64(ctx, S, ldS, B, D, obs, W, K, thr, d_out, acc_idx, n_acc, stream)
     ptrs = np.concatenate([[_addr(d_out)], _vec(extra_host, max(n_extra, 1), np.uint64)[:n_extra]]

@@ -7,18 +7,28 @@ import numpy as np
 import elfi_oracle as o
 
 
-def reference_merge(batches, thr, n):
-    """samplers.py:209-237 restated on the host: mask, copy to the tail, argsort over n + B."""
+def reference_merge(batches, thr, n, pad=np.inf):
+    """samplers.py:209-237 restated on the host: mask, copy to the tail, argsort over n + B.
+
+    Each batch maps output names to (B,) or (B, width) arrays; 'd' holds the K distance columns
+    and a row is accepted when every column is within its threshold (thr: a scalar or K values).
+    The rows are ranked by the LAST distance column, as the reference ranks nested distances.
+    The argsort is stable: the project promises that ties keep their append order (merge_topn,
+    argsort, CandidateBuffer.best), while the reference's own np.argsort is a quicksort, whose
+    order among ties is unspecified.  The distances of the rows not yet filled start at `pad`:
+    the reference's +inf, or NaN, which ranks after an accepted +inf distance (the reference
+    ranks its padding first among such ties).  Returns the first n rows of every output."""
     B = len(batches[0]['d'])
-    state = {k: np.zeros(n + B) for k in batches[0]}
-    state['d'][:] = np.inf
+    state = {k: np.zeros((n + B,) + np.shape(v)[1:]) for k, v in batches[0].items()}
+    state['d'][:] = pad
     for b in batches:
-        acc = b['d'] <= thr
+        d = np.asarray(b['d']).reshape(B, -1)
+        acc = np.all(d <= np.atleast_1d(thr), axis=1)
         k = int(acc.sum())
         if k:
             for name in state:
                 state[name][-k:] = b[name][acc]
-        order = np.argsort(state['d'], kind='stable')
+        order = np.argsort(state['d'].reshape(n + B, -1)[:, -1], kind='stable')
         for name in state:
             state[name][:] = state[name][order]
     return {k: v[:n] for k, v in state.items()}
