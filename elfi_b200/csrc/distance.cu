@@ -599,6 +599,103 @@ metric_direct_kernel<METRIC_SEUCLIDEAN>(const double* __restrict__ S, int64_t ld
     });
 }
 
+// 'mahalanobis' (cdist(..., 'mahalanobis', VI=VI)): with u = S_i - obs, t_r = TS_c(VI[r, c] u_c)
+// over ROW r of VI, q = TS_r(u_r t_r), d = sqrt(q), TS being the two-sum order of 'seuclidean'
+// above and every product and sum rounded on its own -- bit-identical to SciPy 1.18's loop, for
+// any VI (tests/test_mahalanobis_host.py replays the order against cdist).
+// One thread per row.  About 2 D^2 fp64 operations per 8 D bytes read, so beyond small D the
+// fp64 pipe bounds it, not HBM.  Shared memory: each thread's u in a strip of D | 1 doubles (odd:
+// the 16 threads of a half-warp read u_c from 16 different bank pairs) and a tile of MH_RB rows of
+// VI stored column-major, [c][k] for row r0 + k, so that the MH_RB values of a column are four
+// LDS.128 broadcasts.  A thread keeps 2 MH_RB running sums of the tile's t_r in registers and
+// folds each finished t_r into q in ascending r.  Tile rows past D are zero and never folded.
+constexpr int MH_THREADS = 128;
+constexpr int MH_RB = 8;
+
+constexpr size_t mahalanobis_smem_bytes(int64_t D) {
+    return (size_t(MH_THREADS) * size_t(D | 1) + size_t(D) * MH_RB) * sizeof(double);
+}
+static_assert(mahalanobis_smem_bytes(ELFI_B200_MAHALANOBIS_D_MAX) <= 227 * 1024,
+              "the widest Mahalanobis CTA must fit sm_90's 227 KB of opt-in shared memory");
+
+__device__ __forceinline__ void ts_add(double& even, double& odd, double& last, int j, int j_last,
+                                       double term) {
+    if (j == j_last) last = term;
+    else if (j & 1) odd = __dadd_rn(odd, term);
+    else even = __dadd_rn(even, term);
+}
+
+__global__ void __launch_bounds__(MH_THREADS)
+mahalanobis_kernel(const double* __restrict__ S, int64_t ld, int64_t B, int D,
+                   const double* __restrict__ VI, DistParams p) {
+    extern __shared__ double mh_smem[];
+    const int st = D | 1;
+    const int tid = threadIdx.x;
+    const int64_t row0 = int64_t(blockIdx.x) * MH_THREADS;
+    const int64_t row = row0 + tid;
+    const int rows = int(B - row0 < MH_THREADS ? B - row0 : MH_THREADS);
+    double* u = mh_smem + tid * st;
+    double* vt = mh_smem + MH_THREADS * st;
+    // the CTA's rows of S, coalesced, as u = S - obs into the strips
+    for (int e = tid; e < rows * D; e += MH_THREADS) {
+        const int r = e / D, c = e - r * D;
+        mh_smem[r * st + c] = __dsub_rn(__ldg(S + (row0 + r) * ld + c), __ldg(p.obs + c));
+    }
+    const int pairs = D - (D & 1);
+    const int j_last = (D & 1) ? D - 1 : -1;
+    double qe = 0.0, qo = 0.0, ql = 0.0;
+    for (int r0 = 0; r0 < D; r0 += MH_RB) {
+        __syncthreads();   // the strips are written / the previous tile is consumed
+        for (int e = tid; e < D * MH_RB; e += MH_THREADS) {
+            const int k = e / D, c = e - k * D;
+            vt[c * MH_RB + k] = r0 + k < D ? __ldg(VI + size_t(r0 + k) * D + c) : 0.0;
+        }
+        __syncthreads();
+        double te[MH_RB], to[MH_RB];
+#pragma unroll
+        for (int k = 0; k < MH_RB; ++k) te[k] = to[k] = 0.0;
+        if (row < B) {
+            for (int c = 0; c < pairs; c += 2) {
+                const double u0 = u[c], u1 = u[c + 1];
+                const double2* v0 = reinterpret_cast<const double2*>(vt + c * MH_RB);
+                const double2* v1 = reinterpret_cast<const double2*>(vt + (c + 1) * MH_RB);
+#pragma unroll
+                for (int h = 0; h < MH_RB / 2; ++h) {
+                    const double2 a = v0[h], b = v1[h];
+                    te[2 * h] = __dadd_rn(te[2 * h], __dmul_rn(a.x, u0));
+                    te[2 * h + 1] = __dadd_rn(te[2 * h + 1], __dmul_rn(a.y, u0));
+                    to[2 * h] = __dadd_rn(to[2 * h], __dmul_rn(b.x, u1));
+                    to[2 * h + 1] = __dadd_rn(to[2 * h + 1], __dmul_rn(b.y, u1));
+                }
+            }
+#pragma unroll
+            for (int k = 0; k < MH_RB; ++k) {
+                if (r0 + k < D) {
+                    double t = __dadd_rn(te[k], to[k]);
+                    if (j_last >= 0) t = __dadd_rn(t, __dmul_rn(vt[j_last * MH_RB + k], u[j_last]));
+                    ts_add(qe, qo, ql, r0 + k, j_last, __dmul_rn(u[r0 + k], t));
+                }
+            }
+        }
+    }
+    dist_record<false, 1>(p, 1, row, B, tid & 31, [&](int) {
+        const double s = __dadd_rn(qe, qo);
+        return sqrt(j_last >= 0 ? __dadd_rn(s, ql) : s);
+    });
+}
+
+static int launch_mahalanobis(const double* S, int64_t ldS, int64_t B, int64_t D,
+                              const double* VI, const DistParams& p, cudaStream_t stream) {
+    if (B == 0) return ELFI_B200_OK;
+    const size_t smem = mahalanobis_smem_bytes(D);
+    ELFI_CUDA_OK(cudaFuncSetAttribute(mahalanobis_kernel,
+                                      cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    mahalanobis_kernel<<<unsigned((B + MH_THREADS - 1) / MH_THREADS), MH_THREADS, smem, stream>>>(
+        S, ldS, B, int(D), VI, p);
+    ELFI_CUDA_OK(cudaGetLastError());
+    return ELFI_B200_OK;
+}
+
 // One column of any metric: the row stream when the matrix takes it, else a thread per row.
 template <int METRIC>
 static int launch_metric_t(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B, int64_t D,
@@ -966,6 +1063,21 @@ int elfi_b200_dist_seuclidean_thr_f64(elfi_b200_ctx* ctx, const double* S, int64
                      d_out, acc_idx, n_acc, stream_, [&](const DistParams& p, cudaStream_t stream) {
                          return launch_metric(ctx, METRIC_SEUCLIDEAN, S, ldS, B, D,
                                               MetricParams{p, 0.0, V}, stream);
+                     });
+}
+
+int elfi_b200_dist_mahalanobis_thr_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
+                                       int64_t D, const double* obs, const double* VI,
+                                       const double* thr_host, double* d_out, int32_t* acc_idx,
+                                       int64_t* n_acc, void* stream_) {
+    using namespace elfi;
+    ELFI_REQUIRE(ctx != nullptr, "dist_mahalanobis: ctx is NULL");
+    ELFI_REQUIRE(VI != nullptr, "dist_mahalanobis: VI is NULL");
+    ELFI_REQUIRE(D <= ELFI_B200_MAHALANOBIS_D_MAX, "dist_mahalanobis: D=%lld above %d",
+                 (long long)D, ELFI_B200_MAHALANOBIS_D_MAX);
+    return dist_call("dist_mahalanobis", ctx, S, ldS, B, D, obs, nullptr, 1, thr_host, nullptr,
+                     d_out, acc_idx, n_acc, stream_, [&](const DistParams& p, cudaStream_t stream) {
+                         return launch_mahalanobis(S, ldS, B, D, VI, p, stream);
                      });
 }
 

@@ -836,11 +836,23 @@ def device_seuclidean_discrepancy(*summaries, observed, V, accept=None):
     return AcceptedOutput(d, idx) if accept is not None else d
 
 
+def device_mahalanobis_discrepancy(*summaries, observed, VI, accept=None):
+    """distance_as_discrepancy for cdist's 'mahalanobis' (VI = inverse covariance matrix)."""
+    X = _stack_summaries(summaries)
+    if _stack_observed(observed).shape[0] != 1:
+        raise ValueError('observed summaries must form a single row')
+    thr = None if accept is None else np.atleast_1d(dev.to_host(accept))
+    d, idx = ops.dist_mahalanobis(X, _observed_on_device(observed), _device_constant(VI),
+                                  threshold=thr)
+    return AcceptedOutput(d, idx) if accept is not None else d
+
+
 def host_distance_as_discrepancy(dist, *summaries, observed):
     """Generic path for metrics without a CUDA kernel: explicit error, never a silent fallback."""
     raise NotImplementedError(
         "elfi_b200.Distance implements the Euclidean family on the device "
-        "('euclidean' with or without w=, 'seuclidean' with V=) and 'sqeuclidean', 'cityblock', "
+        "('euclidean' with or without w=, 'seuclidean' with V=), 'mahalanobis' with VI= and "
+        "'sqeuclidean', 'cityblock', "
         "'chebyshev', 'minkowski' (p=) unweighted. Metric {!r} with these keywords has no "
         "CUDA kernel; use elfi_b200.Discrepancy with your own callable.".format(dist))
 
@@ -856,6 +868,9 @@ def _device_metric_operation(metric, kw):
         return partial(device_euclidean_discrepancy, w=kw.get('w'))
     if metric == 'seuclidean' and given == {'V'}:
         return partial(device_seuclidean_discrepancy, V=np.asarray(kw['V'], dtype=np.float64))
+    if metric == 'mahalanobis' and given == {'VI'}:
+        return partial(device_mahalanobis_discrepancy,
+                       VI=np.asarray(kw['VI'], dtype=np.float64))
     if metric == 'minkowski' and given <= {'p'}:
         return partial(device_metric_discrepancy, metric, p=kw.get('p', 2.0))
     if metric in DEVICE_METRICS and not given:

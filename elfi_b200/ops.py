@@ -250,6 +250,29 @@ def dist_seuclidean(S, obs, V, threshold=None, want_indices=True):
     return d.reshape(B), _dist_accepted(acc_idx, n_acc, want_indices)
 
 
+MAHALANOBIS_D_MAX = _lib.CONSTANTS['MAHALANOBIS_D_MAX']
+
+
+def dist_mahalanobis(S, obs, VI, threshold=None, want_indices=True):
+    """cdist(S, obs, 'mahalanobis', VI=VI) + acceptance on the device, bit-identical to SciPy for
+    any (D, D) VI (t = VI u by rows of VI, then u . t, both in SciPy's two-sum order;
+    elfi/model/elfi_model.py:1016-1037 forwards the metric string and VI to cdist).  D is at most
+    MAHALANOBIS_D_MAX.  Returns (d (B,), acc_idx or None)."""
+    S, obs_t, thr, d, acc_idx, n_acc = _dist_prepare(S, obs, threshold, 1, want_indices)
+    B, D = S.shape
+    if D > MAHALANOBIS_D_MAX:
+        raise ValueError('dist_mahalanobis: D={} is above MAHALANOBIS_D_MAX = {}'.format(
+            D, MAHALANOBIS_D_MAX))
+    VI_t = dev.to_device(VI)
+    if tuple(VI_t.shape) != (D, D):
+        raise ValueError('VI must be a ({0}, {0}) matrix for summaries of dimension {0}, got shape '
+                         '{1}'.format(D, tuple(VI_t.shape)))
+    _lib.call('elfi_b200_dist_mahalanobis_thr_f64', dev.context(), dev.ptr(S), _ld(S), B, D,
+              dev.ptr(obs_t), dev.ptr(VI_t), dev.ptr(thr), dev.ptr(d), dev.ptr(acc_idx),
+              dev.ptr(n_acc), dev.stream_ptr())
+    return d.reshape(B), _dist_accepted(acc_idx, n_acc, want_indices)
+
+
 def dist_euclid_host(S, obs, w=None, thresholds=None, return_distances=True):
     """Host-buffer variant (elfi_b200_dist_euclid_thr_f64_host): numpy in, numpy out."""
     S = np.asarray(S, dtype=np.float64)

@@ -151,6 +151,23 @@ int elfi_b200_dist_seuclidean_thr_f64(elfi_b200_ctx* ctx, const double* S, int64
                                       const double* thr_host, double* d_out, int32_t* acc_idx,
                                       int64_t* n_acc, void* stream);
 
+/* cdist(S, obs, 'mahalanobis', VI=VI) (elfi/model/elfi_model.py:1016-1037 with the VI keyword of
+ * the Distance docstring): with u = S_i - obs,
+ *   t_r = TS_c(VI[r, c] * u_c)  over ROW r of VI,   q = TS_r(u_r * t_r),   d_i = sqrt(q),
+ * TS being the summation order of SciPy's compiled loop that elfi_b200_dist_seuclidean_thr_f64
+ * follows (two running sums over the even and the odd positions of the first D - D%2 terms, their
+ * sum, then the last term when D is odd), every product and sum rounded on its own: bit-identical
+ * to cdist for any VI, symmetric or not.  Non-finite inputs propagate; a VI that makes q < 0 gives
+ * NaN, which no threshold accepts.  VI (D, D) row-major device.  1 <= D <=
+ * ELFI_B200_MAHALANOBIS_D_MAX: each thread of a 128-thread CTA keeps its row of u in shared memory
+ * next to a tile of 8 rows of VI.  Other arguments, the scratch use (the acceptance mask) and the
+ * acceptance outputs as for elfi_b200_dist_metric_thr_f64. */
+#define ELFI_B200_MAHALANOBIS_D_MAX 192
+int elfi_b200_dist_mahalanobis_thr_f64(elfi_b200_ctx* ctx, const double* S, int64_t ldS, int64_t B,
+                                       int64_t D, const double* obs, const double* VI,
+                                       const double* thr_host, double* d_out, int32_t* acc_idx,
+                                       int64_t* n_acc, void* stream);
+
 /* ---- summary statistics ----------------------------------------------------------------
  * Row-wise summaries with NumPy's pairwise summation order (bit-identical results).
  *
