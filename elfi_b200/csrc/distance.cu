@@ -18,7 +18,6 @@
 // with a fused distance share) and dist_call() is the host skeleton of the entry
 // points over a device-resident matrix.  A metric adds its per-term arithmetic and its finish:
 // a consumer, a thread-per-row kernel and a case in launch_dist() or launch_metric().
-#include <cstdlib>
 
 #include "distrecord.cuh"
 #include "metric.cuh"
@@ -286,14 +285,12 @@ colmoments_flush_kernel(const double* __restrict__ S, const double* __restrict__
 // Warps per CTA of the fused kernel: 12 when the ring still gets >= 3 slots next to the per-warp
 // accumulators (two warps per scheduler leave the fp64 pipe half idle: long dependent chains of
 // K + 2 accumulators per lane), else 8; 16 warps (128 registers, 2-slot ring) gives the
-// 8-warp time back, and the plain nested kernels do not gain from either.  ELFI_B200_FUSED_WARPS=8 restores 8 (KMAX <= 8).
+// 8-warp time back, and the plain nested kernels do not gain from either.
 template <int KMAX>
 static int fused_moments_warps(elfi_b200_ctx* ctx, int64_t Dp, int64_t K) {
-    int warps = 12;
-    if (const char* e = getenv("ELFI_B200_FUSED_WARPS")) warps = atoi(e);
-    if (KMAX > 8 || warps != 12) return RS_WARPS;
-    const size_t aux = NestedMomentsConsumer<KMAX>::aux_bytes(Dp, K, warps);
-    return rs_pick_stages(ctx->smem_optin, aux, warps) >= 3 ? warps : RS_WARPS;
+    if (KMAX > 8) return RS_WARPS;
+    const size_t aux = NestedMomentsConsumer<KMAX>::aux_bytes(Dp, K, 12);
+    return rs_pick_stages(ctx->smem_optin, aux, 12) >= 3 ? 12 : RS_WARPS;
 }
 
 template <int KMAX>

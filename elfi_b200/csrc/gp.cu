@@ -17,7 +17,6 @@
 // Variance uses the explicit inverse factor W = L^-1 instead of a triangular solve per query
 // chunk:  v_i = k** - || W k_i ||^2.  The product is a GEMM with a triangular K-range (row a
 // of W is zero beyond column a), i.e. n^2 m / 2 FMAs = 0.4 TFLOP at n = 2000, m = 1e5.
-#include <cstdlib>
 
 #include "common.cuh"
 
@@ -25,6 +24,7 @@ namespace elfi {
 
 constexpr int GP_NB = 64;          // Cholesky panel width / base block of the inverse
 constexpr int GM_BM = 128, GM_BN = 128;
+constexpr int GM_SMALL_BELOW = 100;  // launch_gemm: fewer large tiles than this take the 64 x 64 tile
 // k-slab width BK (16 or 32); smem rows are padded to BK + 4 doubles: the 16 lanes of a half warp
 // (grp 0..3 x tig 0..3) then read 16 distinct 8-byte banks
 constexpr int GM_STAGES = 3;       // cp.async ring: two slabs in flight while one is consumed
@@ -269,25 +269,14 @@ static int launch_gemm_cfg(const GemmArgs& g, int64_t batch, cudaStream_t stream
 
 static int launch_gemm(const GemmArgs& g, int64_t batch, cudaStream_t stream) {
     if (g.M <= 0 || g.N <= 0 || batch <= 0) return ELFI_B200_OK;
-    static const int small_below = [] {
-        const char* v = getenv("ELFI_B200_GEMM_SMALL_BELOW");   // 0 = always the large tile
-        return v ? atoi(v) : 100;
-    }();
     int64_t tiles = ((g.M + GM_BM - 1) / GM_BM) * ((g.N + GM_BN - 1) / GM_BN) * batch;
     if (g.mode == 1) tiles = tiles / 2 + 1;
-    if (g.mode != 2 && tiles < small_below) return launch_gemm_cfg<64, 64, 2, 2, 16>(g, batch, stream);
+    if (g.mode != 2 && tiles < GM_SMALL_BELOW) return launch_gemm_cfg<64, 64, 2, 2, 16>(g, batch, stream);
     // 32-wide slabs halve the block barriers of the large tile (221 KB of shared memory, within
-    // the 227 KB a block may opt in to; 230 registers).  ELFI_B200_GEMM_BK32=0: 16.
-    static const bool wide_slab = [] {
-        const char* v = getenv("ELFI_B200_GEMM_BK32");
-        return !(v != nullptr && v[0] == '0');
-    }();
-    if (g.mode == 2 && g.tri_skip) {   // the guarded k-steps exist in these two instances only
-        if (wide_slab) return launch_gemm_cfg<GM_BM, GM_BN, 2, 4, 32, true>(g, batch, stream);
-        return launch_gemm_cfg<GM_BM, GM_BN, 2, 4, 16, true>(g, batch, stream);
-    }
-    if (wide_slab) return launch_gemm_cfg<GM_BM, GM_BN, 2, 4, 32>(g, batch, stream);
-    return launch_gemm_cfg<GM_BM, GM_BN, 2, 4, 16>(g, batch, stream);
+    // the 227 KB a block may opt in to; 230 registers).
+    if (g.mode == 2 && g.tri_skip)     // the guarded k-steps exist in this instance only
+        return launch_gemm_cfg<GM_BM, GM_BN, 2, 4, 32, true>(g, batch, stream);
+    return launch_gemm_cfg<GM_BM, GM_BN, 2, 4, 32>(g, batch, stream);
 }
 
 // ---- K10: Gram / cross-covariance ----------------------------------------------------------
@@ -592,6 +581,7 @@ static int launch_trimv(const double* M, int64_t ldm, int64_t n, const double* V
 }
 constexpr int64_t GP_FEW_CHUNK = 16;   // right-hand sides per launch
 constexpr int64_t GP_PREDICT_FEW = 160;// elfi_b200_gp_predict_f64: up to this many points go this way
+constexpr int64_t GP_PREDICT_CHUNK = 32768;   // elfi_b200_gp_predict_f64: most query rows per chunk
 
 // kq[q][j] = s2 exp(f |x_q - X_j|^2) + bias
 __global__ void __launch_bounds__(256)
@@ -738,14 +728,10 @@ int elfi_b200_gp_fit_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, const
     // caller's stream right away, the rest of the trailing matrix on the context's side stream,
     // where it overlaps with the next panel's latency-bound factorisation.  Ordering: the side
     // stream waits for the panel (ev_panel); the caller's stream waits for rest(p - 1) before it
-    // touches block column p + 1 again (ev_rest).  ELFI_B200_GP_LOOKAHEAD=0: one stream.
+    // touches block column p + 1 again (ev_rest).
     double* T = static_cast<double*>(ctx_scratch(ctx, size_t(n_pad) * n_pad * 8 + 256));
     if (!T) return ELFI_B200_ERR_NOMEM;
     double* Dblocks = T;     // (n_pad / 64) factored diagonal blocks, copied into L after the loop
-    static const bool lookahead = [] {
-        const char* v = getenv("ELFI_B200_GP_LOOKAHEAD");
-        return !(v != nullptr && v[0] == '0');
-    }();
     cudaStream_t side = ctx->copy_stream[0];
     cudaEvent_t ev_panel = ctx->copy_event[0], ev_rest = ctx->copy_event[1];
     bool rest_pending = false;
@@ -769,11 +755,6 @@ int elfi_b200_gp_fit_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, const
         }
         potrf_diag_panel_kernel<<<unsigned((below + 127) / 128), 128, 0, stream>>>(
             L, n_pad, k, n_pad, info, Dblocks + (k / GP_NB) * GP_NB * GP_NB);
-        if (!lookahead) {
-            int rc = syrk(k, k + GP_NB, below, below, 1, stream);
-            if (rc) return rc;
-            continue;
-        }
         ELFI_CUDA_OK(cudaEventRecord(ev_panel, stream));
         if (rest_pending) { ELFI_CUDA_OK(cudaStreamWaitEvent(stream, ev_rest, 0)); rest_pending = false; }
         int rc = syrk(k, k + GP_NB, below, GP_NB, 0, stream);          // next block column
@@ -878,14 +859,8 @@ int elfi_b200_gp_predict_f64(elfi_b200_ctx* ctx, const double* Xq, int64_t ldq, 
     // Query chunks: Ks (mc x n_pad) lives in scratch.  Every chunk boundary costs the tail wave of
     // its GEMM plus the K* / epilogue kernels' launch gaps, so chunks are as large as gridDim.y of
     // the K* kernel allows (32768 rows = 0.5 GB of scratch at n_pad = 2048, nothing on a 180 GB
-    // part) and equal in size (a short last chunk would be 1-2 ragged waves).  Round 2 ran 8192-row
-    // chunks; ELFI_B200_GP_PREDICT_CHUNK restores any other size.
-    static const int64_t mc_max = [] {
-        const char* v = getenv("ELFI_B200_GP_PREDICT_CHUNK");
-        const long c = v ? atol(v) : 32768;
-        return int64_t(c < 128 ? 128 : (c > 65408 ? 65408 : c));
-    }();
-    const int64_t nchunks = (m + mc_max - 1) / mc_max;
+    // part) and equal in size (a short last chunk would be 1-2 ragged waves).
+    const int64_t nchunks = (m + GP_PREDICT_CHUNK - 1) / GP_PREDICT_CHUNK;
     const int64_t mc = ((m + nchunks - 1) / nchunks + 127) / 128 * 128;
     // scratch: Ks (mc x n_pad), then the per-column-tile sums of squares (ntiles x mc)
     const int ntiles = int(n_pad / GM_BN);
@@ -905,13 +880,9 @@ int elfi_b200_gp_predict_f64(elfi_b200_ctx* ctx, const double* Xq, int64_t ldq, 
         g.C = nullptr; g.ldc = n_pad;          // V = K* W^T is consumed in the epilogue
         g.rowsq = rowsq; g.ld_rowsq = mc;
         g.M = rows; g.N = n_pad; g.K = n_pad; g.alpha = 1.0; g.beta = 0.0; g.mode = 2;
-        static const bool tri_skip = [] {
-            const char* v = getenv("ELFI_B200_GEMM_TRI_SKIP");
-            return !(v != nullptr && v[0] == '0');
-        }();
-        g.tri_skip = tri_skip ? 1 : 0;
+        g.tri_skip = 1;
         g.n_valid = n;
-        if (tri_skip) g.K = (n + 3) & ~int64_t(3);   // k >= n: zero columns of K*, identity rows of W
+        g.K = (n + 3) & ~int64_t(3);   // k >= n: zero columns of K*, identity rows of W
         int rc = launch_gemm(g, 1, stream);
         if (rc) return rc;
         predict_rows_sq_kernel<<<unsigned((rows + 7) / 8), 256, 0, stream>>>(

@@ -14,7 +14,6 @@
 // replayed (e.g. to materialise X for a test) and any sharding of rows gives the same particles.
 // oracle/streams.py replays every kernel's counter layout in NumPy; tests/test_streams_gpu.py
 // compares the kernels with it element by element.
-#include <cstdlib>
 
 #include "boxmuller.cuh"
 #include "gnkmath.cuh"
@@ -569,7 +568,7 @@ int elfi_b200_sim_ma2_f64(elfi_b200_ctx* ctx, const double* t1, const double* t2
     ELFI_REQUIRE((!X || ldX >= n_obs) && (!S || ldS >= 2), "sim_ma2: bad leading dimension");
     if (B == 0) return ELFI_B200_OK;
     const unsigned blocks = unsigned((B + 127) / 128);
-    const bool leaf = n_obs - 1 <= LEAF_MAX_TERMS && getenv("ELFI_B200_SIM_MA2_TREE") == nullptr;
+    const bool leaf = n_obs - 1 <= LEAF_MAX_TERMS;
     return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
 #define ELFI_SIM_MA2(WX, SM, LF) \
     sim_ma2_kernel<WX, SM, LF><<<blocks, 128, 0, stream>>>(t1, t2, B, int(n_obs), seed, offset, X, ldX, S, ldS)
@@ -724,7 +723,7 @@ int elfi_b200_sim_gauss_f64(elfi_b200_ctx* ctx, const double* mu, const double* 
     ELFI_REQUIRE((!Y || ldY >= n_obs) && (!S || ldS >= 2), "sim_gauss: bad leading dimension");
     if (B == 0) return ELFI_B200_OK;
     const unsigned blocks = unsigned((B + 127) / 128);
-    const bool leaf = n_obs <= LEAF_MAX_TERMS && getenv("ELFI_B200_SIM_GAUSS_TREE") == nullptr;
+    const bool leaf = n_obs <= LEAF_MAX_TERMS;
     return run_on_device(ctx, stream_, [&](cudaStream_t stream) {
 #define ELFI_SIM_GAUSS(WY, LF) \
     sim_gauss_kernel<WY, LF><<<blocks, 128, 0, stream>>>(mu, sigma, B, int(n_obs), seed, offset, Y, ldY, S, ldS)

@@ -12,7 +12,6 @@
 // 64-bit conversions, which run at quarter rate) and a degree-6 minimax polynomial: relative
 // error < 2e-9 per term, far inside the 1e-5 relative tolerance on the weights.  Accumulation
 // is fp64.
-#include <cstdlib>
 
 #include "common.cuh"
 #include "gmterm.cuh"
@@ -370,10 +369,6 @@ static int gm_logpdf_impl(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int6
         chunk_len = ((M / 64 + 511) / 512) * 512;
         if (chunk_len < 2048) chunk_len = 2048;
         if (chunk_len > 16384) chunk_len = 16384;
-        if (const char* e = getenv("ELFI_B200_GM_CHUNK")) {
-            const long v = atol(e);
-            if (v >= 512) chunk_len = (int64_t(v) / 512) * 512;
-        }
         chunks = (M + chunk_len - 1) / chunk_len;
         ELFI_REQUIRE(chunks <= 65535, "gm_logpdf: too many component chunks (%lld)", (long long)chunks);
     }
@@ -397,13 +392,7 @@ static int gm_logpdf_impl(elfi_b200_ctx* ctx, const double* x, int64_t ldx, int6
     const double lognorm = -0.5 * (double(p) * 1.8378770664093453 + logdet);  // log(2 pi)
     if (p <= 4) {
         dim3 grid(static_cast<unsigned>(xblocks), static_cast<unsigned>(chunks));
-        // ELFI_B200_GM_MODE = fp64 | mixed overrides the choice of the entry point (measurements)
-        static const int forced = [] {
-            const char* v = getenv("ELFI_B200_GM_MODE");
-            return v == nullptr ? 0 : (v[0] == 'm' ? 2 : (v[0] == 'f' ? 1 : 0));
-        }();
-        const bool mixed = forced == 2 || (forced == 0 && mixed_entry);
-        if (mixed) {
+        if (mixed_entry) {
             switch (p) {
                 case 1: gm_pdf_kernel<1, R, true><<<grid, 128, 0, stream>>>(xw, N, mw, M, chunk_len, partial); break;
                 case 2: gm_pdf_kernel<2, R, true><<<grid, 128, 0, stream>>>(xw, N, mw, M, chunk_len, partial); break;

@@ -1,8 +1,7 @@
 #!/usr/bin/env python
 """Round-2 kernel timings (CUDA events around batches of back-to-back launches, so the per-call
 Python overhead overlaps with the previous kernel; median of the batches).  One JSON line per
-kernel + bench_out/r2_kernels[_TAG].json.  Variants selected by environment variables are
-static per process: run the script once per variant (TAG names the output)."""
+kernel + bench_out/r2_kernels.json."""
 import json
 import os
 import sys
@@ -16,7 +15,6 @@ from elfi_b200 import ops  # noqa: E402
 
 HBM = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs'] \
     if os.path.exists(os.path.join(ROOT, 'MEASURED_PEAKS.json')) else 6650.0
-TAG = os.environ.get('TAG', 'default')
 out = []
 
 
@@ -37,7 +35,7 @@ def timeit(fn, per_batch=10, batches=7, warm=3):
 
 
 def rec(name, ms, best, nbytes, **kw):
-    e = dict(name=name, tag=TAG, ms_median=ms, ms_min=best, algorithmic_GB=nbytes / 1e9,
+    e = dict(name=name, ms_median=ms, ms_min=best, algorithmic_GB=nbytes / 1e9,
              GBps=nbytes / (ms * 1e-3) / 1e9, frac_hbm_measured=nbytes / (ms * 1e-3) / 1e9 / HBM, **kw)
     out.append(e)
     print(json.dumps(e), flush=True)
@@ -90,7 +88,7 @@ ms_f, best_f = timeit(lambda: ops.dist_euclid(Sg, og, w=W, thresholds=thr, sync=
 rec('nested_K5_plus_moments_fused_5e5x256', ms_f, best_f, nb + 2 * 256 * 8)
 ms_c, best_c = timeit(lambda: ops.colmoments(Sg))
 rec('colmoments_alone_5e5x256', ms_c, best_c, Sg.numel() * 8)
-out.append(dict(name='fused_vs_two_passes', tag=TAG, fused_ms=ms_f, two_passes_ms=ms + ms_c,
+out.append(dict(name='fused_vs_two_passes', fused_ms=ms_f, two_passes_ms=ms + ms_c,
                 speedup=(ms + ms_c) / ms_f))
 print(json.dumps(out[-1]), flush=True)
 W1 = torch.ones(1, 256, dtype=torch.float64, device='cuda')
@@ -107,14 +105,11 @@ for N in (125_000, 1_000_000):
     xs = randn(N, 2) * 0.3
     ms, best = timeit(lambda: ops.gm_logpdf(xs, means, cov, w, validate=False), per_batch=1,
                       batches=3, warm=1)
-    e = dict(name='gm_logpdf_N{}_M1e6'.format(N), tag=TAG, ms_median=ms, ms_min=best,
+    e = dict(name='gm_logpdf_N{}_M1e6'.format(N), ms_median=ms, ms_min=best,
              pairs_per_s=N * M / (ms * 1e-3), fp64_inst_per_pair=16,
              tflops_equiv=N * M * 16 / (ms * 1e-3) / 1e12)
     out.append(e)
     print(json.dumps(e), flush=True)
-    if N == 125_000:      # kept for an accuracy comparison between ELFI_B200_GM_MODE variants
-        np.save(os.path.join(ROOT, 'bench_out', 'gm_logq_{}.npy'.format(TAG)),
-                ops.gm_logpdf(xs, means, cov, w, validate=False).cpu().numpy())
 
-with open(os.path.join(ROOT, 'bench_out', 'r2_kernels_{}.json'.format(TAG)), 'w') as f:
+with open(os.path.join(ROOT, 'bench_out', 'r2_kernels.json'), 'w') as f:
     json.dump(out, f, indent=1)

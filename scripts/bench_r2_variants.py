@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""A/B timings of kernel variants that an environment variable selects per process: run once per
-variant, `TAG` names the line.  CUDA events around batches of back-to-back launches."""
+"""Timings of the row sort, the nested and fused distances and the standardised Euclidean distance
+(`WHAT` selects among them).  CUDA events around batches of back-to-back launches."""
 import json
 import os
 import sys
@@ -14,7 +14,6 @@ from elfi_b200 import ops  # noqa: E402
 
 HBM = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs'] \
     if os.path.exists(os.path.join(ROOT, 'MEASURED_PEAKS.json')) else 6650.0
-TAG = os.environ.get('TAG', 'default')
 WHAT = set(os.environ.get('WHAT', 'rowsort,fused,nested,seuclid').split(','))
 gen = torch.Generator(device='cuda').manual_seed(0)
 
@@ -40,7 +39,7 @@ def timeit(fn, per_batch=10, batches=7, warm=3):
 
 
 def rec(name, ms, best, nbytes):
-    print(json.dumps(dict(name=name, tag=TAG, ms_median=round(ms, 4), ms_min=round(best, 4),
+    print(json.dumps(dict(name=name, ms_median=round(ms, 4), ms_min=round(best, 4),
                           GBps=round(nbytes / ms / 1e6, 1),
                           frac_hbm_measured=round(nbytes / ms / 1e6 / HBM, 4))), flush=True)
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""CUDA-event time of one GP fit at n = 2000 (variants by environment, one process each)."""
+"""CUDA-event time of one GP fit at n = 2000 (`N` sets another size)."""
 import os
 import sys
 
@@ -15,19 +15,13 @@ rs = np.random.RandomState(0)
 X = rs.uniform([-2, -1], [2, 1], (n, 2))
 y = np.log(0.05 + np.sum((X - 0.3) ** 2, axis=1)) + 0.1 * rs.randn(n)
 gp = GPyRegression(['t1', 't2'], bounds={'t1': (-2, 2), 't2': (-1, 1)}, incremental=False)
-try:
-    gp.update(X, y)
-except Exception as e:      # variants that skip work produce a "bad pivot": timing only
-    print('update:', type(e).__name__)
+gp.update(X, y)
 ts = []
 for _ in range(12):
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     a.record()
-    try:
-        gp._fit()
-    except Exception:
-        pass
+    gp._fit()
     b.record()
     torch.cuda.synchronize()
     ts.append(a.elapsed_time(b))
-print(os.environ.get('TAG', ''), 'fit ms median %.3f min %.3f' % (np.median(ts[2:]), np.min(ts[2:])))
+print('fit ms median %.3f min %.3f' % (np.median(ts[2:]), np.min(ts[2:])))

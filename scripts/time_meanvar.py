@@ -1,20 +1,19 @@
 #!/usr/bin/env python
-"""mean/var timings for contiguous rows: the 1-D bulk row-group kernel (n = 2 mod 4) against the
-2-D tensor-map row-stream path (ELFI_B200_MEANVAR_ROWGROUP=0).  The switch is read once per
-process, so the script re-runs itself per variant.  --once: a single launch (for ncu)."""
+"""mean/var timings for contiguous rows: the 1-D bulk row-group kernel takes n = 2 mod 4, the 2-D
+tensor-map row-stream path the other row lengths.  --once: a single launch (for ncu)."""
 import json
 import os
-import subprocess
 import sys
+
+import numpy as np
+import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from elfi_b200 import ops  # noqa: E402
 
 
-def child(once):
-    import numpy as np
-    import torch
-    from elfi_b200 import ops
+def main(once):
     hbm = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs'] \
         if os.path.exists(os.path.join(ROOT, 'MEASURED_PEAKS.json')) else 6650.0
     gen = torch.Generator(device='cuda').manual_seed(0)
@@ -45,7 +44,6 @@ def child(once):
         exact = bool(np.array_equal(got[:, 0], ref.mean(axis=1)) and
                      np.array_equal(got[:, 1], ref.var(axis=1)))
         print(json.dumps(dict(name='meanvar_{}x{}'.format(B, n),
-                              rowgroup=os.environ.get('ELFI_B200_MEANVAR_ROWGROUP', '1'),
                               ms_median=ms, ms_min=float(min(ts)), GBps=nbytes / ms / 1e6,
                               frac_hbm_measured=nbytes / ms / 1e6 / hbm, bit_exact=exact)),
               flush=True)
@@ -53,9 +51,4 @@ def child(once):
 
 
 if __name__ == '__main__':
-    if '--child' in sys.argv or '--once' in sys.argv:
-        child('--once' in sys.argv)
-    else:
-        for flag in ('1', '0'):
-            env = dict(os.environ, ELFI_B200_MEANVAR_ROWGROUP=flag)
-            subprocess.check_call([sys.executable, os.path.abspath(__file__), '--child'], env=env)
+    main('--once' in sys.argv)

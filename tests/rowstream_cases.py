@@ -38,10 +38,6 @@ Mean / variance:
   else rowstream_ok -> MeanVarRegsConsumer<NBOX> (n <= 64), MeanVarBoxConsumer<LeafSum>
     (n <= 128), MeanVarBoxConsumer<TreeSum<6>> (n <= 7688); else summary_direct_kernel.
   NBOX = ceil(n / 16).
-The environment switches ELFI_B200_SUMM_TERMWISE=0 (AutocovConsumer, MeanVarConsumer),
-ELFI_B200_MEANVAR_TWO_SWEEPS, ELFI_B200_MEANVAR_ROWGROUP=0 and ELFI_B200_FUSED_WARPS are read once
-per process; their paths are listed in the registry (so that the source scan knows them) but have
-no cases.
 
 Layouts (the leading dimension and the base offset of the input, in doubles): contiguous; ld even
 and > D (TMA with a row gap); ld odd; base + 1 (never TMA); base + 2 with ld even (TMA with a
@@ -161,7 +157,7 @@ def first_at_least(values, K):
 # ---------------------------------------------------------------------------- registry
 class Path(types.SimpleNamespace):
     """name; kernel: the substring of the launched kernel's demangled name (whitespace and '(int)'
-    removed); consumer: the key the source scan finds; env: the switch that alone reaches it."""
+    removed); consumer: the key the source scan finds."""
 
 
 def _rs(consumer, warps=RS_WARPS):
@@ -171,8 +167,8 @@ def _rs(consumer, warps=RS_WARPS):
 def _registry():
     P = []
 
-    def add(name, kernel, consumer, env=None):
-        P.append(Path(name=name, kernel=kernel, consumer=consumer, env=env))
+    def add(name, kernel, consumer):
+        P.append(Path(name=name, kernel=kernel, consumer=consumer))
     add('dist:Euclid', _rs('EuclidConsumer'), 'EuclidConsumer')
     add('dist:Weighted', _rs('WeightedConsumer'), 'WeightedConsumer')
     for k in NESTED_KMAX:
@@ -198,9 +194,6 @@ def _registry():
             add('autocov:{}<{},{}>'.format(sname, la, lb),
                 _rs('AutocovBoxConsumer<{},{},{}>'.format(sk, la, lb)),
                 'AutocovBoxConsumer<{},{},{}>'.format(sname, la, lb))
-        add('autocov:TermGrouper<{},{}>'.format(la, lb),
-            _rs('AutocovConsumer<{},{}>'.format(la, lb)), 'AutocovConsumer<{},{}>'.format(la, lb),
-            env='ELFI_B200_SUMM_TERMWISE=0')
     add('summary:direct', 'elfi::summary_direct_kernel(', 'summary_direct_kernel')
     for nb in (1, 2, 3, 4):
         for w in (8, 6):
@@ -210,8 +203,6 @@ def _registry():
             'MeanVarRegsConsumer<{}>'.format(nb))
     add('meanvar:BoxLeaf', _rs('MeanVarBoxConsumer<elfi::LeafSum>'), 'MeanVarBoxConsumer<Leaf>')
     add('meanvar:BoxTree', _rs('MeanVarBoxConsumer<elfi::TreeSum<6>>'), 'MeanVarBoxConsumer<Tree>')
-    add('meanvar:TermGrouper', _rs('MeanVarConsumer'), 'MeanVarConsumer',
-        env='ELFI_B200_SUMM_TERMWISE=0')
     return {p.name: p for p in P}
 
 
@@ -219,13 +210,11 @@ REGISTRY = _registry()
 
 
 def reachable(optin):
-    """Registry paths some input selects at this shared-memory opt-in (no environment switch).  The
-    row-group kernel's warp count depends on n and optin alone: at 227 KiB only NBOX = 4 (n = 58,
-    62) needs 6 warps."""
+    """Registry paths some input selects at this shared-memory opt-in.  The row-group kernel's
+    warp count depends on n and optin alone: at 227 KiB only NBOX = 4 (n = 58, 62) needs 6 warps."""
     rg = {'meanvar:rowgroup<{},{}>'.format(-(-n // 16), rowgroup_warps(optin, n))
           for n in range(2, 65, 4) if rowgroup_ok(optin, True, n, n)}
-    return sorted(n for n, p in REGISTRY.items()
-                  if p.env is None and (not n.startswith('meanvar:rowgroup') or n in rg))
+    return sorted(n for n in REGISTRY if not n.startswith('meanvar:rowgroup') or n in rg)
 
 
 def normalize_kernel_name(name):
@@ -508,9 +497,12 @@ def uncovered(sm, optin):
 def scan_sources(distance_cu, summaries_cu):
     """Consumer / kernel keys that distance.cu and summaries.cu launch: every consumer passed to
     rowstream_launch<...> (template arguments kept when they are literals; the typedef of
-    launch_metric_t resolved), every *_direct_kernel<<<, every meanvar_rowgroup_kernel instance."""
+    launch_metric_t resolved), every *_direct_kernel<<<, every meanvar_rowgroup_kernel instance,
+    and 'colmoments' for a call of the stand-alone column moments."""
     keys = set()
     for text in (distance_cu, summaries_cu):
+        if re.search(r'\belfi_b200_colmoments_f64\(', text):
+            keys.add('colmoments')
         typedefs = dict((b, a) for a, b in re.findall(r'typedef\s+(\w+)<[^;]*>\s+(\w+);', text))
         for name, args in re.findall(r'rowstream_launch<\s*(\w+)\s*(<[^<>]*(?:<[^<>]*>[^<>]*)*>)?', text):
             name = typedefs.get(name, name)
@@ -528,13 +520,17 @@ def scan_sources(distance_cu, summaries_cu):
     return keys
 
 
+def names(key, consumer):
+    """Does a scanned key name a registry consumer (by instance, or by template name)?"""
+    return key == consumer or ('<' not in key and consumer.split('<')[0] == key)
+
+
 def registry_has(key):
-    """Does a scanned key name a registry entry (by instance, or by template name)?"""
-    for p in REGISTRY.values():
-        c = p.consumer
-        if key == c or (('<' not in key) and c.split('<')[0] == key):
-            return True
-    return False
+    return any(names(key, p.consumer) for p in REGISTRY.values())
+
+
+def launched(keys, consumer):
+    return any(names(k, consumer) for k in keys)
 
 
 # ---------------------------------------------------------------------------- data

@@ -89,3 +89,12 @@ def test_product_never_imports_oracle():
                 if re.search(r'^\s*(import|from)\s+(elfi_oracle|oracle|ref_shim|streams)\b', src, re.M):
                     bad.append(os.path.join(dirpath, f))
     assert not bad, bad
+
+
+def test_native_code_reads_no_environment():
+    """Every kernel choice follows from the inputs and the device: no source of the library reads
+    an environment variable, so a variable set in a user's shell cannot change what runs."""
+    csrc = os.path.join(ROOT, 'elfi_b200', 'csrc')
+    bad = sorted(f for f in os.listdir(csrc)
+                 if re.search(r'getenv\s*\(', open(os.path.join(csrc, f)).read()))
+    assert not bad, bad

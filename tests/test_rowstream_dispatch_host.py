@@ -1,6 +1,7 @@
 """The row-stream case table against the kernels it is meant to cover, without a GPU: every
-reachable registry path has cases on both H100 variants, and every consumer, thread-per-row kernel
-and row-group instance that distance.cu and summaries.cu launch has a registry entry."""
+reachable registry path has cases on both H100 variants, every consumer, thread-per-row kernel
+and row-group instance that distance.cu and summaries.cu launch has a registry entry, and every
+registry entry is launched there."""
 import os
 
 import numpy as np
@@ -70,6 +71,14 @@ def test_source_scan_finds_only_registered_kernels():
             'summary_direct_kernel'} <= keys
     missing = sorted(k for k in keys if not cases.registry_has(k))
     assert not missing, 'launched but not in the registry: {}'.format(missing)
+
+
+def test_source_scan_finds_every_registered_kernel():
+    keys = cases.scan_sources(_read('distance.cu'), _read('summaries.cu'))
+    # a template name does not stand for another template it is a substring of
+    assert not cases.launched(keys, 'AutocovConsumer<1,2>')
+    stale = sorted(p.name for p in cases.REGISTRY.values() if not cases.launched(keys, p.consumer))
+    assert not stale, 'in the registry but never launched: {}'.format(stale)
 
 
 def test_source_scan_flags_an_unregistered_consumer():
