@@ -57,13 +57,9 @@ struct elfi_b200_ctx {
     elfi::tensor_map_encode_fn encode_tiled;
     void* scratch;
     size_t scratch_bytes;
-    // pinned staging + copy streams for the *_host entry points
-    void* pinned;
-    size_t pinned_bytes;
-    void* dev_stage;
-    size_t dev_stage_bytes;
-    cudaStream_t copy_stream[2];
-    cudaEvent_t copy_event[4];
+    // the GP Cholesky look-ahead's second stream and its two ordering events (gp.cu)
+    cudaStream_t side_stream;
+    cudaEvent_t side_event[2];
 };
 
 namespace elfi {

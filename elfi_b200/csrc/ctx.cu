@@ -97,10 +97,9 @@ int elfi_b200_ctx_create(int device, elfi_b200_ctx** out) {
         return ELFI_B200_ERR_CUDA;
     }
     ctx->encode_tiled = reinterpret_cast<elfi::tensor_map_encode_fn>(fn);
+    ELFI_CUDA_OK(cudaStreamCreateWithFlags(&ctx->side_stream, cudaStreamNonBlocking));
     for (int i = 0; i < 2; ++i)
-        ELFI_CUDA_OK(cudaStreamCreateWithFlags(&ctx->copy_stream[i], cudaStreamNonBlocking));
-    for (int i = 0; i < 4; ++i)
-        ELFI_CUDA_OK(cudaEventCreateWithFlags(&ctx->copy_event[i], cudaEventDisableTiming));
+        ELFI_CUDA_OK(cudaEventCreateWithFlags(&ctx->side_event[i], cudaEventDisableTiming));
     *out = ctx;
     return ELFI_B200_OK;
 }
@@ -110,78 +109,13 @@ int elfi_b200_ctx_destroy(elfi_b200_ctx* ctx) {
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
     if (ctx->scratch) cudaFree(ctx->scratch);
-    if (ctx->dev_stage) cudaFree(ctx->dev_stage);
-    if (ctx->pinned) cudaFreeHost(ctx->pinned);
+    if (ctx->side_stream) cudaStreamDestroy(ctx->side_stream);
     for (int i = 0; i < 2; ++i)
-        if (ctx->copy_stream[i]) cudaStreamDestroy(ctx->copy_stream[i]);
-    for (int i = 0; i < 4; ++i)
-        if (ctx->copy_event[i]) cudaEventDestroy(ctx->copy_event[i]);
+        if (ctx->side_event[i]) cudaEventDestroy(ctx->side_event[i]);
     delete ctx;
     return ELFI_B200_OK;
 }
 
 int elfi_b200_ctx_sm_count(const elfi_b200_ctx* ctx) { return ctx ? ctx->sm_count : 0; }
-
-// Single-process multi-GPU exchange of accepted particles (SURVEY.md section 8b/8e): one context
-// per GPU; GPU g contributes send[g] (rows x width doubles in its memory) and receives the
-// context-ordered concatenation in recv[g].  Peer copies (cudaMemcpyPeerAsync, NVLink when peer
-// access can be enabled) ordered by events: a destination stream waits until every source has
-// produced its block; every source stream waits until all destinations have read it, so the
-// caller may overwrite send[g] with later work on streams[g].
-int elfi_b200_allgather_particles(elfi_b200_ctx* const* ctxs, int64_t n_ctx, const double* const* send,
-                                  int64_t rows, int64_t width, double* const* recv,
-                                  void* const* streams) {
-    ELFI_REQUIRE(ctxs && send && recv && streams && n_ctx >= 1 && n_ctx <= 64,
-                 "allgather_particles: bad argument");
-    ELFI_REQUIRE(rows >= 0 && width >= 1, "allgather_particles: bad shape");
-    for (int64_t g = 0; g < n_ctx; ++g)
-        ELFI_REQUIRE(ctxs[g] && (rows == 0 || (send[g] && recv[g])), "allgather_particles: NULL entry %lld",
-                     (long long)g);
-    if (rows == 0) return ELFI_B200_OK;
-    const size_t bytes = size_t(rows) * size_t(width) * 8;
-    int caller_device = 0;
-    ELFI_CUDA_OK(cudaGetDevice(&caller_device));
-    struct Restore {
-        int d;
-        ~Restore() { cudaSetDevice(d); }
-    } restore{caller_device};   // the calling thread keeps its current device
-    // peer access (once per ordered pair; "already enabled" is not an error)
-    for (int64_t d = 0; d < n_ctx; ++d) {
-        ELFI_CUDA_OK(cudaSetDevice(ctxs[d]->device));
-        for (int64_t s = 0; s < n_ctx; ++s) {
-            if (ctxs[s]->device == ctxs[d]->device) continue;
-            int can = 0;
-            ELFI_CUDA_OK(cudaDeviceCanAccessPeer(&can, ctxs[d]->device, ctxs[s]->device));
-            if (can) {
-                cudaError_t e = cudaDeviceEnablePeerAccess(ctxs[s]->device, 0);
-                if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) ELFI_CUDA_OK(e);
-                cudaGetLastError();
-            }
-        }
-    }
-    // ready[g]: send[g] is complete on its stream
-    for (int64_t g = 0; g < n_ctx; ++g) {
-        ELFI_CUDA_OK(cudaSetDevice(ctxs[g]->device));
-        ELFI_CUDA_OK(cudaEventRecord(ctxs[g]->copy_event[2], static_cast<cudaStream_t>(streams[g])));
-    }
-    for (int64_t d = 0; d < n_ctx; ++d) {
-        ELFI_CUDA_OK(cudaSetDevice(ctxs[d]->device));
-        cudaStream_t sd = static_cast<cudaStream_t>(streams[d]);
-        for (int64_t s = 0; s < n_ctx; ++s) {
-            if (s != d) ELFI_CUDA_OK(cudaStreamWaitEvent(sd, ctxs[s]->copy_event[2], 0));
-            ELFI_CUDA_OK(cudaMemcpyPeerAsync(recv[d] + size_t(s) * rows * width, ctxs[d]->device, send[s],
-                                             ctxs[s]->device, bytes, sd));
-        }
-        ELFI_CUDA_OK(cudaEventRecord(ctxs[d]->copy_event[3], sd));   // done[d]: d has read every block
-    }
-    for (int64_t s = 0; s < n_ctx; ++s) {
-        ELFI_CUDA_OK(cudaSetDevice(ctxs[s]->device));
-        for (int64_t d = 0; d < n_ctx; ++d)
-            if (d != s)
-                ELFI_CUDA_OK(cudaStreamWaitEvent(static_cast<cudaStream_t>(streams[s]),
-                                                 ctxs[d]->copy_event[3], 0));
-    }
-    return ELFI_B200_OK;
-}
 
 }  // extern "C"

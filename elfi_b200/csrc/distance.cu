@@ -940,98 +940,6 @@ int elfi_b200_dist_euclid_mom_f64(elfi_b200_ctx* ctx, const double* S, int64_t l
     return fused ? ELFI_B200_OK : elfi_b200_colmoments_f64(ctx, S, ldS, B, D, moments, stream_);
 }
 
-int elfi_b200_dist_euclid_thr_f64_host(elfi_b200_ctx* ctx, const double* S_host, int64_t ldS,
-                                       int64_t B, int64_t D, const double* obs_host,
-                                       const double* W_host, int64_t K, const double* thr_host,
-                                       double* d_out_host, int32_t* acc_idx_host,
-                                       int64_t* n_acc_host) {
-    using namespace elfi;
-    ELFI_REQUIRE(ctx != nullptr, "dist_host: ctx is NULL");
-    int rc = check_dist_args(S_host, ldS, B, D, obs_host, W_host, K, thr_host, acc_idx_host);
-    if (rc) return rc;
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-
-    // Device staging: two row chunks (ping-pong), obs, W, distances, mask, indices, count.
-    const int64_t row_bytes = D * 8;
-    int64_t chunk_rows = (int64_t(32) << 20) / row_bytes;
-    chunk_rows = (chunk_rows / 32) * 32;
-    if (chunk_rows < 32) chunk_rows = 32;
-    if (chunk_rows > B) chunk_rows = ((B + 31) / 32) * 32;
-    const size_t chunk_bytes = size_t(chunk_rows) * row_bytes;
-    const size_t nwords = size_t((B + 31) / 32);
-    auto align = [](size_t v) { return (v + 255) & ~size_t(255); };
-    const size_t off_chunk1 = align(chunk_bytes);
-    const size_t off_obs = off_chunk1 + align(chunk_bytes);
-    const size_t off_w = off_obs + align(size_t(D) * 8);
-    const size_t off_d = off_w + align(size_t(K) * D * 8);
-    const size_t off_mask = off_d + align(size_t(B) * K * 8);
-    const size_t off_idx = off_mask + align(nwords * 4 + 4);
-    const size_t off_n = off_idx + align(size_t(B) * 4 + 4);
-    const size_t total = off_n + 256;
-    if (total > ctx->dev_stage_bytes) {
-        ELFI_CUDA_OK(cudaDeviceSynchronize());
-        if (ctx->dev_stage) ELFI_CUDA_OK(cudaFree(ctx->dev_stage));
-        ctx->dev_stage = nullptr;
-        ctx->dev_stage_bytes = 0;
-        ELFI_CUDA_OK(cudaMalloc(&ctx->dev_stage, total));
-        ctx->dev_stage_bytes = total;
-    }
-    uint8_t* base = static_cast<uint8_t*>(ctx->dev_stage);
-    double* chunk[2] = {reinterpret_cast<double*>(base), reinterpret_cast<double*>(base + off_chunk1)};
-    double* obs_d = reinterpret_cast<double*>(base + off_obs);
-    double* w_d = W_host ? reinterpret_cast<double*>(base + off_w) : nullptr;
-    double* d_d = reinterpret_cast<double*>(base + off_d);
-    uint32_t* mask_d = thr_host ? reinterpret_cast<uint32_t*>(base + off_mask) : nullptr;
-    int32_t* idx_d = reinterpret_cast<int32_t*>(base + off_idx);
-    int64_t* n_d = reinterpret_cast<int64_t*>(base + off_n);
-
-    cudaStream_t s0 = ctx->copy_stream[0], s1 = ctx->copy_stream[1];
-    ELFI_CUDA_OK(cudaMemcpyAsync(obs_d, obs_host, size_t(D) * 8, cudaMemcpyHostToDevice, s0));
-    if (W_host)
-        ELFI_CUDA_OK(cudaMemcpyAsync(w_d, W_host, size_t(K) * D * 8, cudaMemcpyHostToDevice, s0));
-    ELFI_CUDA_OK(cudaEventRecord(ctx->copy_event[0], s0));
-    ELFI_CUDA_OK(cudaStreamWaitEvent(s1, ctx->copy_event[0], 0));
-
-    int which = 0;
-    for (int64_t r0 = 0; r0 < B; r0 += chunk_rows, which ^= 1) {
-        const int64_t rows = (B - r0) < chunk_rows ? (B - r0) : chunk_rows;
-        cudaStream_t st = which ? s1 : s0;
-        if (ldS == D) {
-            ELFI_CUDA_OK(cudaMemcpyAsync(chunk[which], S_host + r0 * ldS, size_t(rows) * row_bytes,
-                                         cudaMemcpyHostToDevice, st));
-        } else {
-            ELFI_CUDA_OK(cudaMemcpy2DAsync(chunk[which], size_t(row_bytes), S_host + r0 * ldS,
-                                           size_t(ldS) * 8, size_t(row_bytes), size_t(rows),
-                                           cudaMemcpyHostToDevice, st));
-        }
-        rc = launch_dist(ctx, chunk[which], D, rows, D,
-                         dist_params(obs_d, w_d, K, thr_host, nullptr, d_d + r0 * K,
-                                     mask_d ? mask_d + r0 / 32 : nullptr), st);
-        if (rc) return rc;
-    }
-    // join s1 into s0, compact, copy back
-    ELFI_CUDA_OK(cudaEventRecord(ctx->copy_event[1], s1));
-    ELFI_CUDA_OK(cudaStreamWaitEvent(s0, ctx->copy_event[1], 0));
-    ELFI_CUDA_OK(cudaEventRecord(ctx->copy_event[2], s0));
-    ELFI_CUDA_OK(cudaStreamWaitEvent(s1, ctx->copy_event[2], 0));
-    if (d_out_host && B > 0)
-        ELFI_CUDA_OK(cudaMemcpyAsync(d_out_host, d_d, size_t(B) * K * 8, cudaMemcpyDeviceToHost, s1));
-    int64_t n_acc = 0;
-    if (thr_host != nullptr) {
-        rc = launch_compact_mask(mask_d, B, acc_idx_host ? idx_d : nullptr, n_d, s0);
-        if (rc) return rc;
-        ELFI_CUDA_OK(cudaMemcpyAsync(&n_acc, n_d, 8, cudaMemcpyDeviceToHost, s0));
-        ELFI_CUDA_OK(cudaStreamSynchronize(s0));
-        if (acc_idx_host && n_acc > 0)
-            ELFI_CUDA_OK(cudaMemcpyAsync(acc_idx_host, idx_d, size_t(n_acc) * 4,
-                                         cudaMemcpyDeviceToHost, s0));
-        if (n_acc_host) *n_acc_host = n_acc;
-    }
-    ELFI_CUDA_OK(cudaStreamSynchronize(s0));
-    ELFI_CUDA_OK(cudaStreamSynchronize(s1));
-    return ELFI_B200_OK;
-}
-
 int elfi_b200_dist_metric_thr_f64(elfi_b200_ctx* ctx, int32_t metric, double pexp, const double* S,
                                   int64_t ldS, int64_t B, int64_t D, const double* obs,
                                   const double* thr_host, double* d_out, int32_t* acc_idx,

@@ -732,8 +732,8 @@ int elfi_b200_gp_fit_f64(elfi_b200_ctx* ctx, const double* X, int64_t ldX, const
     double* T = static_cast<double*>(ctx_scratch(ctx, size_t(n_pad) * n_pad * 8 + 256));
     if (!T) return ELFI_B200_ERR_NOMEM;
     double* Dblocks = T;     // (n_pad / 64) factored diagonal blocks, copied into L after the loop
-    cudaStream_t side = ctx->copy_stream[0];
-    cudaEvent_t ev_panel = ctx->copy_event[0], ev_rest = ctx->copy_event[1];
+    cudaStream_t side = ctx->side_stream;
+    cudaEvent_t ev_panel = ctx->side_event[0], ev_rest = ctx->side_event[1];
     bool rest_pending = false;
     auto syrk = [&](int64_t k, int64_t c0, int64_t rows, int64_t cols, int mode, cudaStream_t st) {
         // C[c0.., c0..(c0 + cols)) -= P P^T with P = L[.., k .. k + 64): rows x cols block at (c0, c0)

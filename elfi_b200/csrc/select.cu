@@ -757,25 +757,6 @@ int elfi_b200_gather_rows_f64(elfi_b200_ctx* ctx, const double* src, int64_t ld_
     return ELFI_B200_OK;
 }
 
-int elfi_b200_gather2_rows_f64(elfi_b200_ctx* ctx, const double* A, int64_t ldA, int64_t nA,
-                               const double* Bm, int64_t ldB, const int32_t* mapB,
-                               const int32_t* perm, int64_t n, int64_t width, double* dst,
-                               int64_t ld_dst, void* stream_) {
-    using namespace elfi;
-    ELFI_REQUIRE(ctx != nullptr, "gather2: ctx is NULL");
-    ELFI_REQUIRE(n >= 0 && nA >= 0 && width >= 1 && ld_dst >= width, "gather2: bad shape");
-    if (n == 0) return ELFI_B200_OK;
-    ELFI_REQUIRE(dst != nullptr && (nA == 0 || A != nullptr), "gather2: NULL argument");
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    ELFI_CUDA_OK(cudaSetDevice(ctx->device));
-    int64_t blocks = (n * width + 255) / 256;
-    if (blocks > int64_t(ctx->sm_count) * 16) blocks = int64_t(ctx->sm_count) * 16;
-    gather2_rows_kernel<<<unsigned(blocks), 256, 0, stream>>>(A, ldA, nA, Bm, ldB, mapB, perm, n,
-                                                             width, dst, ld_dst);
-    ELFI_CUDA_OK(cudaGetLastError());
-    return ELFI_B200_OK;
-}
-
 int elfi_b200_topn_merge_f64(elfi_b200_ctx* ctx, const double* keysA, int64_t ld_keysA, int64_t nA,
                              const double* keysB, int64_t ld_keysB, const int32_t* mapB, int64_t nB,
                              int64_t n_keep, int64_t n_out, const double* const* A_host,

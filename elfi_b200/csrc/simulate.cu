@@ -657,23 +657,6 @@ int elfi_b200_gm_rvs_cdf_f64(elfi_b200_ctx* ctx, const double* means, int64_t ld
     });
 }
 
-int elfi_b200_gm_rvs_f64(elfi_b200_ctx* ctx, const double* means, int64_t ldm, const double* weights,
-                         int64_t N, int64_t p, const double* Lchol_host, int64_t B, uint64_t seed,
-                         uint64_t offset, int32_t support, const double* box_host, double* out,
-                         int64_t ldo, void* stream_) {
-    using namespace elfi;
-    ELFI_REQUIRE(ctx && N >= 1, "gm_rvs: bad argument");
-    if (B == 0) return ELFI_B200_OK;
-    return run_on_device(ctx, stream_, [&](cudaStream_t) {
-        double* cumw = static_cast<double*>(ctx_scratch(ctx, size_t(N) * 8 + 256));
-        if (!cumw) return ELFI_B200_ERR_NOMEM;
-        int rc = elfi_b200_gm_cdf_f64(ctx, weights, N, cumw, stream_);
-        if (rc != ELFI_B200_OK) return rc;
-        return elfi_b200_gm_rvs_cdf_f64(ctx, means, ldm, cumw, N, p, Lchol_host, B, seed, offset,
-                                        support, box_host, out, ldo, stream_);
-    });
-}
-
 static elfi::GaussPrior make_gauss_prior(const double* prm) {
     elfi::GaussPrior g;
     g.mu_lo = prm[0]; g.mu_w = prm[1]; g.a = prm[2]; g.b = prm[3];

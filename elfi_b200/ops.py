@@ -273,34 +273,6 @@ def dist_mahalanobis(S, obs, VI, threshold=None, want_indices=True):
     return d.reshape(B), _dist_accepted(acc_idx, n_acc, want_indices)
 
 
-def dist_euclid_host(S, obs, w=None, thresholds=None, return_distances=True):
-    """Host-buffer variant (elfi_b200_dist_euclid_thr_f64_host): numpy in, numpy out."""
-    S = np.asarray(S, dtype=np.float64)
-    if S.ndim == 1:
-        S = S[:, None]
-    if S.strides[1] != 8:
-        S = np.ascontiguousarray(S)
-    B, D = S.shape
-    ld = S.strides[0] // 8 if B > 1 else D
-    obs = np.ascontiguousarray(obs, dtype=np.float64).reshape(-1)
-    K = 1
-    W = None
-    if w is not None:
-        W = np.ascontiguousarray(np.atleast_2d(w), dtype=np.float64)
-        K = W.shape[0]
-    thr = None if thresholds is None else np.ascontiguousarray(np.atleast_1d(thresholds),
-                                                               dtype=np.float64)
-    d = np.empty((B, K)) if return_distances else None
-    idx = np.empty(max(B, 1), dtype=np.int32) if thr is not None else None
-    n = ctypes.c_int64(0)
-    _lib.call('elfi_b200_dist_euclid_thr_f64_host', dev.context(), dev.ptr(S), ld, B, D,
-              dev.ptr(obs), dev.ptr(W), K, dev.ptr(thr), dev.ptr(d), dev.ptr(idx),
-              ctypes.byref(n) if thr is not None else None)
-    if d is not None and K == 1 and (w is None or np.ndim(w) == 1):
-        d = d.reshape(B)
-    return d, (idx[:n.value] if idx is not None else None)
-
-
 def autocov(x, lags=(1,), out=None):
     """MA2 autocovariance summaries (elfi/examples/ma2.py:40-59) for one or more lags.
 
@@ -369,22 +341,6 @@ def take_rows(src, idx):
         _lib.call('elfi_b200_gather_rows_f64', dev.context(), dev.ptr(s2), _ld(s2), dev.ptr(idx),
                   n, width, dev.ptr(dst), width, dev.stream_ptr())
     return dst.reshape((n,) + tuple(shape[1:]))
-
-
-def take_rows2(a, b, perm, n_out, map_b=None):
-    """Rows perm[:n_out] of the virtual concatenation [a; b[map_b]] (top-n merge gather)."""
-    shape = a.shape if a is not None else b.shape
-    a2 = _as_2d(a) if a is not None else None
-    b2 = _as_2d(b) if b is not None else None
-    width = (a2 if a2 is not None else b2).shape[1]
-    n_a = a2.shape[0] if a2 is not None else 0
-    dst = dev.empty((n_out, width))
-    if n_out and width:
-        _lib.call('elfi_b200_gather2_rows_f64', dev.context(), dev.ptr(a2),
-                  _ld(a2) if a2 is not None else width, n_a, dev.ptr(b2),
-                  _ld(b2) if b2 is not None else width, dev.ptr(map_b), dev.ptr(perm), n_out,
-                  width, dev.ptr(dst), width, dev.stream_ptr())
-    return dst.reshape((n_out,) + tuple(shape[1:]))
 
 
 def merge_topn(state, batch, key_state, key_batch, map_b, n_keep):
@@ -612,32 +568,6 @@ class CandidateBuffer:
         keys = self.rows[:count, key_col].contiguous()
         perm = argsort(keys)
         return take_rows(self.rows, perm[:min(n, count)]), count, dropped
-
-
-def allgather_particles(blocks):
-    """Single-process multi-GPU all-gather (elfi_b200_allgather_particles): `blocks` = one
-    (rows, width) fp64 CUDA tensor per GPU (equal shapes, each on its own device); returns one
-    (len(blocks) * rows, width) tensor per GPU holding the blocks in list order.  The copies are
-    enqueued on each device's current stream."""
-    n = len(blocks)
-    blocks = [b.contiguous() for b in blocks]
-    rows = blocks[0].shape[0]
-    width = int(np.prod(blocks[0].shape[1:])) if blocks[0].dim() > 1 else 1
-    if any(tuple(b.shape) != tuple(blocks[0].shape) or b.dtype != torch.float64 for b in blocks):
-        raise ValueError('blocks must be fp64 tensors of equal shape')
-    outs, streams, ctxs = [], [], []
-    for b in blocks:
-        with torch.cuda.device(b.device):
-            outs.append(torch.empty((n * rows,) + tuple(b.shape[1:]), dtype=torch.float64,
-                                    device=b.device))
-            streams.append(torch.cuda.current_stream(b.device).cuda_stream)
-            ctxs.append(dev.context(b.device).value)
-    arr = ctypes.c_void_p * n
-    _lib.call('elfi_b200_allgather_particles', ctypes.cast(arr(*ctxs), ctypes.c_void_p), n,
-              ctypes.cast(arr(*[b.data_ptr() for b in blocks]), ctypes.c_void_p), rows, width,
-              ctypes.cast(arr(*[o.data_ptr() for o in outs]), ctypes.c_void_p),
-              ctypes.cast(arr(*streams), ctypes.c_void_p))
-    return outs
 
 
 def weighted_sample_quantile(x, alpha, weights=None):

@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define ELFI_B200_VERSION 100
+#define ELFI_B200_VERSION 101
 
 #define ELFI_B200_OK 0
 #define ELFI_B200_ERR_ARG (-1)     /* invalid argument (shape, alignment, NULL) */
@@ -49,20 +49,6 @@ int elfi_b200_ctx_create(int device, elfi_b200_ctx** out);
 int elfi_b200_ctx_destroy(elfi_b200_ctx* ctx);
 /* Number of SMs of the context's device (grid sizing is a multiple of this). */
 int elfi_b200_ctx_sm_count(const elfi_b200_ctx* ctx);
-
-/* ---- single-process multi-GPU exchange ----------------------------------------------------
- * The per-generation all-gather of accepted particles / weights (SURVEY.md section 8e; the
- * reference merges the batches of its workers in the master, samplers.py:140-237) for a process
- * that drives several GPUs itself (one context per GPU, e.g. the thread-per-GPU client): GPU g
- * contributes send[g] (rows x width doubles in ITS memory) and receives the context-ordered
- * concatenation (n_ctx * rows x width) in recv[g].  ctxs / send / recv / streams are HOST arrays
- * of n_ctx entries; streams[g] is the stream of GPU g on which send[g] was produced and on which
- * recv[g] is consumed afterwards (the call only enqueues copies and event waits).  Copies are
- * peer-to-peer (NVLink when peer access can be enabled, otherwise staged by the driver).
- * One-process-per-GPU runs use torch.distributed / NCCL instead (DESIGN.md section 5). */
-int elfi_b200_allgather_particles(elfi_b200_ctx* const* ctxs, int64_t n_ctx,
-                                  const double* const* send, int64_t rows, int64_t width,
-                                  double* const* recv, void* const* streams);
 
 /* ---- distance + acceptance ------------------------------------------------------------
  * Replaces, for the Euclidean family, the body of
@@ -114,16 +100,6 @@ int elfi_b200_dist_euclid_mom_f64(elfi_b200_ctx* ctx, const double* S, int64_t l
                                   int64_t D, const double* obs, const double* W, int64_t K,
                                   const double* thr_host, const double* thr_dev, double* d_out,
                                   int32_t* acc_idx, int64_t* n_acc, double* moments, void* stream);
-
-/* Same computation with HOST buffers (pageable or pinned): rows are streamed to the device
- * in chunks on two copy streams overlapped with the kernel; distances, accepted indices
- * and the count are copied back.  Blocks until the results are in host memory.
- * d_out_host may be NULL (then only accepted indices / count come back). */
-int elfi_b200_dist_euclid_thr_f64_host(elfi_b200_ctx* ctx, const double* S_host, int64_t ldS,
-                                       int64_t B, int64_t D, const double* obs_host,
-                                       const double* W_host, int64_t K, const double* thr_host,
-                                       double* d_out_host, int32_t* acc_idx_host,
-                                       int64_t* n_acc_host);
 
 /* Other cdist metrics that elfi.Distance forwards to SciPy (elfi/model/elfi_model.py:1016-1037):
  *   SQEUCLIDEAN  sum_j (S_ij - obs_j)^2          CITYBLOCK  sum_j |S_ij - obs_j|
@@ -198,11 +174,6 @@ int elfi_b200_summary_meanvar_f64(elfi_b200_ctx* ctx, const double* X, int64_t l
  * elfi_b200_gather_rows_f64: dst[i, 0:width] = src[idx[i], 0:width] -- the fancy-index
  * permutation `v[:] = v[sort_mask]` / `batch[node][accepted]` (samplers.py:228-237).
  *
- * elfi_b200_gather2_rows_f64: same from the virtual concatenation [A (nA rows); B], where B
- * rows may be indirected through mapB (the accepted indices of the new batch): the running
- * top-n merge without materialising the (n + batch) buffers of samplers.py:196-205.
- * perm == NULL means the identity.
- *
  * elfi_b200_accept_append_f64: `v[-num_accepted:] = batch[node][accepted]` for every output node
  * (samplers.py:228-230) with the counts read ON THE DEVICE, so a threshold-mode batch needs no
  * host round trip between the distance kernel and the merge: rows acc_idx[0 .. *n_acc) (acc_idx
@@ -237,10 +208,6 @@ int elfi_b200_rejection_batch_f64(elfi_b200_ctx* ctx, const double* S, int64_t l
                                   const double* const* extra_host, const int64_t* ld_extra_host,
                                   const int64_t* width_extra_host, double* dst, int64_t ld_dst,
                                   int64_t capacity, int64_t* count, int64_t* dropped, void* stream);
-int elfi_b200_gather2_rows_f64(elfi_b200_ctx* ctx, const double* A, int64_t ldA, int64_t nA,
-                               const double* B, int64_t ldB, const int32_t* mapB,
-                               const int32_t* perm, int64_t n, int64_t width, double* dst,
-                               int64_t ld_dst, void* stream);
 
 /* elfi_b200_topn_merge_f64: Rejection._merge_batch (samplers.py:226-237) in one call.  The
  * reference appends the accepted rows of a batch behind its best-n buffers, argsorts the distance
@@ -424,24 +391,23 @@ int elfi_b200_probe_fp64_f64(elfi_b200_ctx* ctx, double* tflops_host);
  *   elfi_b200_sim_ma2_f64       MA2 simulator (ma2.py:11-37); writes X (B, n_obs) and/or, fused,
  *                               the lag-1 / lag-2 autocovariances S (B, 2) (ma2.py:40-59, NumPy
  *                               pairwise order) so that X never has to touch HBM
- *   elfi_b200_gm_rvs_f64        GMDistribution.rvs (elfi/methods/utils.py:200-261): component by
- *                               weight, + MVN(0, Sigma) with Sigma = L L^T (Lchol_host, p <= 16),
- *                               redrawn until inside the support (0 = none, 1 = MA2 prior support
- *                               (p = 2), 2 = box: box_host = [lo_0..lo_{p-1}, hi_0..hi_{p-1}],
- *                               3 = prior: box_host = the 5p-word prior table of
- *                               elfi_b200_prior_logpdf_f64, a draw is kept iff its joint log
- *                               density is finite; 4 = the same with the 7p-word table of
- *                               conditional priors).  At most 1000 draws per row: when all of them
- *                               fall outside the support, the 1000th draw is returned as it is
- *                               (outside the support).  For p <= 4 with supports 0-2 the streams
- *                               are those of earlier versions; support 3 uses the same blocks, and
- *                               z_4 .. z_15 come from a stream of their own
  *   elfi_b200_gm_cdf_f64        inclusive running sum of the (unnormalised) component weights, the
  *                               table np.random.choice(p=weights) builds on every call
  *                               (utils.py:239); one per population, reused by every batch of it.
  *                               Nondecreasing whatever the weights (>= 0), so a zero-weight
  *                               component is never drawn; deterministic
- *   elfi_b200_gm_rvs_cdf_f64    gm_rvs with that table (`cumw`, device, N) instead of the weights
+ *   elfi_b200_gm_rvs_cdf_f64    GMDistribution.rvs (elfi/methods/utils.py:200-261) with that table
+ *                               (`cumw`, device, N): component by weight, + MVN(0, Sigma) with
+ *                               Sigma = L L^T (Lchol_host, p <= 16), redrawn until inside the
+ *                               support (0 = none, 1 = MA2 prior support (p = 2), 2 = box:
+ *                               box_host = [lo_0..lo_{p-1}, hi_0..hi_{p-1}], 3 = prior: box_host =
+ *                               the 5p-word prior table of elfi_b200_prior_logpdf_f64, a draw is
+ *                               kept iff its joint log density is finite; 4 = the same with the
+ *                               7p-word table of conditional priors).  At most 1000 draws per row:
+ *                               when all of them fall outside the support, the 1000th draw is
+ *                               returned as it is (outside the support).  For p <= 4 with supports
+ *                               0-2 the streams are those of earlier versions; support 3 uses the
+ *                               same blocks, and z_4 .. z_15 come from a stream of their own
  */
 int elfi_b200_prior_ma2_f64(elfi_b200_ctx* ctx, int64_t B, uint64_t seed, uint64_t offset,
                             int32_t mode, double* t1, double* t2, void* stream);
@@ -450,10 +416,6 @@ int elfi_b200_logprior_ma2_f64(elfi_b200_ctx* ctx, const double* x, int64_t ldx,
 int elfi_b200_sim_ma2_f64(elfi_b200_ctx* ctx, const double* t1, const double* t2, int64_t B,
                           int64_t n_obs, uint64_t seed, uint64_t offset, double* X, int64_t ldX,
                           double* S, int64_t ldS, void* stream);
-int elfi_b200_gm_rvs_f64(elfi_b200_ctx* ctx, const double* means, int64_t ldm, const double* weights,
-                         int64_t N, int64_t p, const double* Lchol_host, int64_t B, uint64_t seed,
-                         uint64_t offset, int32_t support, const double* box_host, double* out,
-                         int64_t ldo, void* stream);
 int elfi_b200_gm_cdf_f64(elfi_b200_ctx* ctx, const double* weights, int64_t N, double* cumw,
                          void* stream);
 int elfi_b200_gm_rvs_cdf_f64(elfi_b200_ctx* ctx, const double* means, int64_t ldm, const double* cumw,
@@ -500,7 +462,7 @@ int elfi_b200_gm_rvs_cdf_f64(elfi_b200_ctx* ctx, const double* means, int64_t ld
  *                                    of the same stream as elfi_b200_prior_rvs_f64 (which computes
  *                                    fma(scale, y_i, loc)); with both NULL the two are the same bits
  *   elfi_b200_prior_logpdf_cond_f64  prior_logpdf with the 7p-word table
- *   elfi_b200_gm_rvs(_cdf)_f64 with support = 4: box_host is the 7p-word table; the draws use the
+ *   elfi_b200_gm_rvs_cdf_f64 with support = 4: box_host is the 7p-word table; the draws use the
  *                                    blocks of support 3, so with every source -1 they are its bits
  */
 #define ELFI_B200_MAX_PRIOR_PARAMS 16       /* parameters p of one prior table */

@@ -144,20 +144,6 @@ def rejection_batch_f64(ctx, S, ldS, B, D, obs, W, K, thr_host, thr_dev, d_out, 
                       capacity, count, dropped, stream)
 
 
-def dist_euclid_thr_f64_host(ctx, S, ldS, B, D, obs, W, K, thr_host, d_out, acc_idx, n_acc):
-    Sm = _mat(S, B, D, ldS)
-    d = _distances(Sm, _vec(obs, D), _mat(W, K, D), K) if B else np.empty((0, K))
-    if _addr(d_out) and B:
-        _mat(d_out, B, K)[:] = d
-    thr = _vec(thr_host, K)
-    if thr is not None:
-        idx = o.accept_indices(d, thr) if B else np.empty(0, dtype=np.int32)
-        if _addr(acc_idx):
-            _vec(acc_idx, max(B, 1), np.int32)[:len(idx)] = idx
-        if n_acc is not None:
-            n_acc._obj.value = len(idx)   # ctypes.byref(c_int64)
-
-
 def dist_metric_thr_f64(ctx, metric, pexp, S, ldS, B, D, obs, thr_host, d_out, acc_idx, n_acc,
                         stream):
     name = {v: k for k, v in o.METRIC_CODES.items()}[metric]
@@ -229,21 +215,6 @@ def gather_rows_f64(ctx, src, ld_src, idx, n, width, dst, ld_dst, stream):
     idx = _vec(idx, n, np.int32)
     src = _mat(src, int(idx.max()) + 1, width, ld_src)
     _mat(dst, n, width, ld_dst)[:] = src[idx]
-
-
-def gather2_rows_f64(ctx, A, ldA, nA, B, ldB, mapB, perm, n, width, dst, ld_dst, stream):
-    if not (n and width):
-        return
-    sel = np.arange(n) if not _addr(perm) else _vec(perm, n, np.int32).astype(np.int64)
-    from_b = sel >= nA
-    rows_b = sel[from_b] - nA
-    if _addr(mapB) and rows_b.size:
-        rows_b = _vec(mapB, int(rows_b.max()) + 1, np.int32)[rows_b].astype(np.int64)
-    out = _mat(dst, n, width, ld_dst)
-    if (~from_b).any():
-        out[~from_b] = _mat(A, nA, width, ldA)[sel[~from_b]]
-    if from_b.any():
-        out[from_b] = _mat(B, int(rows_b.max()) + 1, width, ldB)[rows_b]
 
 
 def topn_merge_f64(ctx, keysA, ld_keysA, nA, keysB, ld_keysB, mapB, nB, n_keep, n_out, A_host, ldA_host,
@@ -552,18 +523,10 @@ def gm_cdf_f64(ctx, weights, N, cumw, stream):
 
 def gm_rvs_cdf_f64(ctx, means, ldm, cumw, N, p, Lchol_host, B, seed, offset, support, box_host, out,
                    ldo, stream):
-    c = _vec(cumw, N)
-    w = np.diff(np.concatenate([[0.0], c]))
-    gm_rvs_f64(ctx, means, ldm, ctypes.c_void_p(w.ctypes.data), N, p, Lchol_host, B, seed, offset,
-               support, box_host, out, ldo, stream)
-
-
-def gm_rvs_f64(ctx, means, ldm, weights, N, p, Lchol_host, B, seed, offset, support, box_host, out,
-               ldo, stream):
     from elfi_b200.examples import ma2 as ex
     rs = _rs(seed, offset, 3)
     mu = _mat(means, N, p, ldm)
-    w = np.ones(N) if not _addr(weights) else _vec(weights, N).copy()
+    w = np.diff(np.concatenate([[0.0], _vec(cumw, N)]))    # the weights back from their running sum
     L = _mat(Lchol_host, p, p)
     box = _vec(box_host, 2 * p) if support == 2 else None
     res = _mat(out, B, p, ldo)
@@ -626,11 +589,11 @@ def logprior_box_f64(ctx, x, ldx, B, p, box_host, out, stream):
 
 
 _TABLE = {'elfi_b200_' + f.__name__: f for f in (
-    dist_euclid_thr_f64, dist_euclid_thr_dev_f64, dist_euclid_mom_f64, accept_append_f64, rejection_batch_f64, dist_euclid_thr_f64_host, dist_metric_thr_f64, dist_seuclidean_thr_f64, topn_merge_f64, summary_autocov_f64, summary_meanvar_f64,
-    sort_pairs_f64, gather_rows_f64, gather2_rows_f64, wquantile_f64, colmoments_f64,
+    dist_euclid_thr_f64, dist_euclid_thr_dev_f64, dist_euclid_mom_f64, accept_append_f64, rejection_batch_f64, dist_metric_thr_f64, dist_seuclidean_thr_f64, topn_merge_f64, summary_autocov_f64, summary_meanvar_f64,
+    sort_pairs_f64, gather_rows_f64, wquantile_f64, colmoments_f64,
     weighted_stats_f64, gm_logpdf_f64, gm_logpdf_mixed_f64, smc_weights_f64, rowsort_f64, kliep_fit_f64, gp_fit_f64,
     gp_predict_f64, gp_predict_grad_f64, gp_whiten_f64, gp_apply_wt_f64, gp_cross_cov_f64, lcbsc_f64, prior_ma2_f64, logprior_ma2_f64, sim_ma2_f64,
-    gm_rvs_f64, gm_cdf_f64, gm_rvs_cdf_f64, prior_gauss_f64, logprior_gauss_f64, sim_gauss_f64, sim_gnk_f64, logprior_box_f64)}
+    gm_cdf_f64, gm_rvs_cdf_f64, prior_gauss_f64, logprior_gauss_f64, sim_gauss_f64, sim_gnk_f64, logprior_box_f64)}
 
 
 # ------------------------------------------------------------------------------ device.py side

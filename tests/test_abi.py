@@ -1,6 +1,7 @@
 """CPU-side checks of the drop-in boundary: the shared library loads and exports exactly
 the entry points include/elfi_b200.h declares (no compute calls: no GPU here)."""
 import ctypes
+import glob
 import os
 import re
 
@@ -53,7 +54,7 @@ def test_binding_covers_header():
     assert _lib.SIGNATURES['elfi_b200_dist_metric_thr_f64'][:5] == [
         ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_void_p, ctypes.c_int64]
     lib = _lib.load()
-    assert lib.elfi_b200_version() == _lib.CONSTANTS['VERSION'] == 100
+    assert lib.elfi_b200_version() == _lib.CONSTANTS['VERSION'] == 101
 
 
 def test_constants_cover_header_macros():
@@ -98,3 +99,13 @@ def test_native_code_reads_no_environment():
     bad = sorted(f for f in os.listdir(csrc)
                  if re.search(r'getenv\s*\(', open(os.path.join(csrc, f)).read()))
     assert not bad, bad
+
+
+def test_every_header_function_has_a_product_caller():
+    """Every function the header declares is named by product code (the package, integration/ or
+    bench.py), so the library exports no entry point that only tests reach."""
+    sources = glob.glob(os.path.join(ROOT, 'elfi_b200', '**', '*.py'), recursive=True)
+    sources += glob.glob(os.path.join(ROOT, 'integration', '*.py')) + [os.path.join(ROOT, 'bench.py')]
+    text = '\n'.join(open(f).read() for f in sources)
+    unused = [n for n in header_functions() if not re.search(r'\b' + n + r'\b', text)]
+    assert not unused, 'declared in include/elfi_b200.h but named by no product code: {}'.format(unused)

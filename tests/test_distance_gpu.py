@@ -8,7 +8,7 @@ from conftest import load_golden
 pytestmark = pytest.mark.gpu
 
 
-def _check(B, D, K=1, weighted=False, q=0.05, ld=None, seed=0, host=False):
+def _check(B, D, K=1, weighted=False, q=0.05, ld=None, seed=0):
     import torch
     from elfi_b200 import ops
     rs = np.random.RandomState(seed)
@@ -24,14 +24,10 @@ def _check(B, D, K=1, weighted=False, q=0.05, ld=None, seed=0, host=False):
         W = None
     thr = np.quantile(ref, q, axis=0) if B > 0 else np.zeros(K)
     ref_idx = o.accept_indices(ref, thr)
-    if host:
-        d, idx = ops.dist_euclid_host(S, obs, w=W, thresholds=thr)
-        d = np.asarray(d).reshape(B, K)
-    else:
-        St = torch.from_numpy(S_full).cuda()[:, :D]
-        d, idx = ops.dist_euclid(St, obs, w=W, thresholds=thr)
-        d = d.cpu().numpy().reshape(B, K)
-        idx = idx.cpu().numpy()
+    St = torch.from_numpy(S_full).cuda()[:, :D]
+    d, idx = ops.dist_euclid(St, obs, w=W, thresholds=thr)
+    d = d.cpu().numpy().reshape(B, K)
+    idx = idx.cpu().numpy()
     assert np.array_equal(d, ref), 'distances differ from the oracle'
     assert np.array_equal(idx, ref_idx), 'accepted index set differs'
     return len(idx)
@@ -97,12 +93,6 @@ def test_nan_rows_are_rejected():
     ref = o.cdist_euclid(S, obs)
     assert np.array_equal(d.cpu().numpy(), ref, equal_nan=True)
     assert np.array_equal(idx.cpu().numpy(), o.accept_indices(ref, 1e9))
-
-
-def test_host_buffer_entry_point():
-    _check(70000, 128, host=True, seed=3)
-    _check(70000, 128, host=True, ld=136, seed=4)
-    _check(5000, 256, K=3, host=True, q=0.5, seed=5)
 
 
 def test_golden_ma2_distance():

@@ -13,28 +13,3 @@ def test_device_thresholds_and_append():
 
 def test_topn_merge_matches_reference_merge():
     cases.case_topn_merge_matches_reference_merge()
-
-
-def test_allgather_particles_single_process():
-    """elfi_b200_allgather_particles: every GPU receives the context-ordered concatenation of all
-    blocks (two GPUs when the box has them; two blocks of one GPU otherwise -- same code path with
-    same-device peer copies); the caller's current device is left alone."""
-    import numpy as np
-    import torch
-    from elfi_b200 import ops
-    n_dev = min(2, torch.cuda.device_count())
-    devices = [0, 1] if n_dev == 2 else [0, 0]
-    rs = np.random.RandomState(3)
-    host = [rs.randn(5000, 3) for _ in devices]
-    blocks = [torch.from_numpy(h).to('cuda:{}'.format(d)) for h, d in zip(host, devices)]
-    before = torch.cuda.current_device()
-    outs = ops.allgather_particles(blocks)
-    for d in set(devices):
-        torch.cuda.synchronize(d)
-    assert torch.cuda.current_device() == before
-    want = np.concatenate(host)
-    for o, d in zip(outs, devices):
-        assert o.device.index == d and np.array_equal(o.cpu().numpy(), want)
-    one = ops.allgather_particles(blocks[:1])
-    torch.cuda.synchronize()
-    assert np.array_equal(one[0].cpu().numpy(), host[0])

@@ -44,20 +44,6 @@ def test_take_rows():
     assert np.array_equal(ops.take_rows(t3, idx[:50] % 100).cpu().numpy(), t3[idx[:50] % 100])
 
 
-def test_take_rows2_merge():
-    import torch
-    from elfi_b200 import ops
-    rs = np.random.RandomState(2)
-    a = rs.randn(50, 3)
-    b = rs.randn(400, 3)
-    mapb = np.sort(rs.choice(400, 120, replace=False)).astype(np.int32)
-    cat = np.vstack([a, b[mapb]])
-    perm = rs.permutation(len(cat)).astype(np.int32)
-    got = ops.take_rows2(torch.from_numpy(a).cuda(), torch.from_numpy(b).cuda(),
-                         torch.from_numpy(perm).cuda(), 60, torch.from_numpy(mapb).cuda())
-    assert np.array_equal(got.cpu().numpy(), cat[perm[:60]])
-
-
 def test_weighted_quantile_golden():
     from elfi_b200 import ops
     g = load_golden('weighted_quantile')
