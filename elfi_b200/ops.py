@@ -1704,6 +1704,113 @@ def sim_ar1(phi, n_obs=200, seed=0, offset=0, obs=None, thresholds=None, want_da
     return X, d, _dist_accepted(acc_idx, n_acc)
 
 
+# ---- n-D Gaussian mean model (elfi/examples/gauss.py, nd_mean=True) -------------------------------
+GAUSS_ND_D_MAX = _lib.CONSTANTS['GAUSS_ND_D_MAX']
+GAUSS_ND_NOBS_MAX = _lib.CONSTANTS['GAUSS_ND_NOBS_MAX']
+GAUSS_ND_SUMM_NOBS_MAX = _lib.CONSTANTS['GAUSS_ND_SUMM_NOBS_MAX']
+
+
+def gauss_nd_summaries(y, out=None):
+    """np.mean(y, axis=1) and np.var(y, axis=1) of (batch, n, D) data (elfi/examples/gauss.py:142-173)
+    as one (batch, 2 D) tensor [means | variances], bit for bit NumPy's on the C-contiguous array:
+    each coordinate's sum over the n observations is NumPy's pairwise sum for D = 1 and a left fold
+    for D >= 2.  Device float64 data is read in place, whatever its strides."""
+    y = _data(y, 'gauss_nd_summaries', ('batch', 'n', 'D'))
+    B, n, D = (int(v) for v in y.shape)
+    if not 1 <= n <= GAUSS_ND_SUMM_NOBS_MAX or D < 1:
+        raise ValueError('gauss_nd_summaries takes 1 <= n <= {} observations of D >= 1 coordinates, '
+                         'got shape {}'.format(GAUSS_ND_SUMM_NOBS_MAX, tuple(y.shape)))
+    out = _out(out, (B, 2 * D), 'gauss_nd_summaries')
+    _lib.call('elfi_b200_gauss_nd_summaries_f64', dev.context(), dev.ptr(y), y.stride(0),
+              y.stride(1), y.stride(2), B, n, D, dev.ptr(out), out.stride(0) if B > 1 else 2 * D,
+              dev.stream_ptr())
+    return out
+
+
+def gauss_nd_distance(S, obs):
+    """The reference's euclidean_multidim (elfi/examples/gauss.py:176-198) on the device:
+    sqrt(np.sum((S - obs)**2., axis=1)) of S (batch, D), any strides, and the observed row obs
+    (D values), bit for bit NumPy's (one pairwise sum per row).  Returns d (batch,)."""
+    S = _data(S, 'gauss_nd_distance', ('batch', 'D'))
+    B, D = (int(v) for v in S.shape)
+    if not 1 <= D <= GAUSS_ND_SUMM_NOBS_MAX:
+        raise ValueError('gauss_nd_distance takes 1 <= D <= {} columns, got shape {}'.format(
+            GAUSS_ND_SUMM_NOBS_MAX, tuple(S.shape)))
+    obs_t = _dist_obs(obs, D)
+    d = dev.empty((B,))
+    _lib.call('elfi_b200_gauss_nd_distance_f64', dev.context(), dev.ptr(S), S.stride(0),
+              S.stride(1), B, D, dev.ptr(obs_t), dev.ptr(d), dev.stream_ptr())
+    return d
+
+
+def gauss_nd_factor(cov_matrix, D):
+    """The (D, D) factor A = sqrt(s)[:, None] * vh of NumPy's RandomState.multivariate_normal for
+    the covariance SciPy's multivariate_normal makes of cov_matrix (None: the identity; a scalar:
+    that multiple of it; a vector: its diagonal), so that mean + z @ A has the reference's law.  A
+    covariance that is not symmetric positive semidefinite raises, as SciPy does."""
+    cov = np.asarray(1.0 if cov_matrix is None else cov_matrix, dtype=np.float64)
+    if cov.ndim == 0:
+        cov = cov * np.eye(D)
+    elif cov.ndim == 1:
+        cov = np.diag(cov)
+    if cov.shape != (D, D):
+        raise ValueError('the covariance of {} means must be ({}, {}), got shape {}'.format(
+            D, D, D, cov.shape))
+    if not np.all(np.isfinite(cov)):
+        raise ValueError('the covariance must be finite')
+    _, s, vh = np.linalg.svd(cov)
+    tol = 1e-8
+    if not np.allclose(np.dot(vh.T * s, vh), cov, rtol=tol, atol=tol):
+        raise ValueError('the covariance must be symmetric positive semidefinite')
+    return np.ascontiguousarray(np.sqrt(s)[:, None] * vh)
+
+
+def _gauss_nd_means(mu):
+    """(batch, D) device means: a matrix, or D device or host columns of one length."""
+    if dev.is_device_array(mu) and mu.dtype == torch.float64 and mu.dim() == 2:
+        return mu
+    if isinstance(mu, (list, tuple)):
+        cols = [dev.to_device(c).reshape(-1) for c in mu]
+        if len({int(c.shape[0]) for c in cols}) != 1:
+            raise ValueError('the mean columns must have one length, got {}'.format(
+                [int(c.shape[0]) for c in cols]))
+        return torch.stack(cols, 1)
+    return _data(mu, 'sim_gauss_nd', ('batch', 'D'))
+
+
+def sim_gauss_nd(mu, A, n_obs=15, seed=0, offset=0, want_data=False, want_summaries=True):
+    """The n-D Gaussian mean simulator on the device (elfi/examples/gauss.py:38-72): row i draws
+    n_obs observations y_t = mu_i + z_t @ A, z_t standard normal (Philox streams; statistical parity
+    with the reference's SciPy draws).  Row i is a pure function of (seed, offset + i).
+
+    mu : (batch, D) device matrix (any strides) or D columns, 1 <= D <= GAUSS_ND_D_MAX
+    A : (D, D) factor, gauss_nd_factor(cov_matrix, D)
+    Returns (Y, S), each None unless asked for: Y (batch, n_obs, D) the data, S (batch, 2 D) its
+    summaries [means | variances], computed without writing Y, bit for bit
+    :func:`gauss_nd_summaries` of Y.  1 <= n_obs <= GAUSS_ND_NOBS_MAX."""
+    M = _gauss_nd_means(mu)
+    B, D = (int(v) for v in M.shape)
+    if not 1 <= D <= GAUSS_ND_D_MAX:
+        raise ValueError('the device n-D Gaussian simulator takes 1 <= D <= {} means, got shape '
+                         '{}'.format(GAUSS_ND_D_MAX, tuple(M.shape)))
+    if int(n_obs) != n_obs or not 1 <= n_obs <= GAUSS_ND_NOBS_MAX:
+        raise ValueError('the device n-D Gaussian simulator takes an integer 1 <= n_obs <= {}, got '
+                         '{}'.format(GAUSS_ND_NOBS_MAX, n_obs))
+    n_obs = int(n_obs)
+    A = np.ascontiguousarray(dev.to_host(A) if dev.is_device_array(A) else A, dtype=np.float64)
+    if A.shape != (D, D):
+        raise ValueError('the factor of {} means must be ({}, {}), got shape {}'.format(
+            D, D, D, A.shape))
+    if not (want_data or want_summaries):
+        raise ValueError('sim_gauss_nd asked for neither the data nor the summaries')
+    Y = dev.empty((B, n_obs, D)) if want_data else None
+    S = dev.empty((B, 2 * D)) if want_summaries else None
+    _lib.call('elfi_b200_sim_gauss_nd_f64', dev.context(), dev.ptr(M), M.stride(0), M.stride(1),
+              B, D, dev.ptr(A), n_obs, int(seed), int(offset), dev.ptr(Y), n_obs * D, dev.ptr(S),
+              2 * D, dev.stream_ptr())
+    return Y, S
+
+
 # ---- M/G/1 queue (elfi/examples/mg1.py) ------------------------------------------------------------
 MG1_NOBS_MIN = _lib.CONSTANTS['MG1_NOBS_MIN']
 MG1_NOBS_MAX = _lib.CONSTANTS['MG1_NOBS_MAX']

@@ -819,6 +819,42 @@ int elfi_b200_sim_ar1_f64(elfi_b200_ctx* ctx, const double* phi, int64_t B, int6
                           const double* obs, const double* thr_host, const double* thr_dev,
                           double* d_out, int32_t* acc_idx, int64_t* n_acc, void* stream);
 
+/* n-D Gaussian mean model of elfi/examples/gauss.py (nd_mean=True); stream layout, thread layout
+ * and arithmetic in elfi_b200/csrc/gauss_nd.cu and gauss_nd.cuh.  Every sum below starts from 0.0,
+ * as NumPy's reductions do, and every operation is rounded on its own.
+ * gauss_nd_summaries: the (n, D) block of row b is X[b * ld_b + t * ld_t + j * ld_j], any strides;
+ *   out[b * ld_out + j] = np.mean(y, axis=1)[b, j] and out[b * ld_out + D + j] =
+ *   np.var(y, axis=1)[b, j] (ld_out >= 2 D), bit for bit NumPy's on the C-contiguous (B, n, D)
+ *   array: for D = 1 the sum over t is NumPy's pairwise sum, for D >= 2 a left fold
+ *   t = 0 .. n - 1; var = sum_t (y - m) * (y - m) / n in the same order, m = sum / n.
+ *   1 <= n <= ELFI_B200_GAUSS_ND_SUMM_NOBS_MAX, D >= 1, B * D < 2^62.
+ * gauss_nd_distance: d[b] = sqrt(sum_j (S[b * ld_b + j * ld_j] - obs[j])^2), the sum in NumPy's
+ *   pairwise order (np.sum(..., axis=1) of a contiguous (B, D) array), bit for bit the reference's
+ *   euclidean_multidim.  1 <= D <= ELFI_B200_GAUSS_ND_SUMM_NOBS_MAX.
+ * sim_gauss_nd (throughput mode, statistical parity): row i has the means
+ *   mu[i * ld_b + j * ld_j], j < D (1 <= D <= ELFI_B200_GAUSS_ND_D_MAX), and observations
+ *   y[t, j] = (sum_k z[t, k] A[k, j]) + mu_j, t < n_obs (1 <= n_obs <= ELFI_B200_GAUSS_ND_NOBS_MAX),
+ *   with A_host the D x D row-major factor sqrt(s)[:, None] * vh of the covariance (NumPy's
+ *   multivariate_normal), on the host.  The sum over k runs in ascending order as
+ *   z_0 A_0j, then fma(z_k, A_kj, s) (FMA is used).  z[t, k] is normal q = t D + k of the row:
+ *   block q / 2 of (seed, offset + i) gives normals 2 (q / 2) and 2 (q / 2) + 1, so the row is a
+ *   pure function of (seed, offset + i), whatever the launch.  Y[i * ldY + t D + j] (ldY >= n_obs D)
+ *   and S[i * ldS + 0 .. 2 D - 1] (ldS >= 2 D) may each be NULL, not both; S is computed without
+ *   writing Y and is bit for bit gauss_nd_summaries of the written Y. */
+#define ELFI_B200_GAUSS_ND_D_MAX 16                  /* the device priors take 16 parameters */
+#define ELFI_B200_GAUSS_ND_NOBS_MAX 7688             /* D = 1: a pairwise sum of depth 6 */
+#define ELFI_B200_GAUSS_ND_SUMM_NOBS_MAX 16777216    /* 2^24 */
+int elfi_b200_gauss_nd_summaries_f64(elfi_b200_ctx* ctx, const double* X, int64_t ld_b,
+                                     int64_t ld_t, int64_t ld_j, int64_t B, int64_t n, int64_t D,
+                                     double* out, int64_t ld_out, void* stream);
+int elfi_b200_gauss_nd_distance_f64(elfi_b200_ctx* ctx, const double* S, int64_t ld_b,
+                                    int64_t ld_j, int64_t B, int64_t D, const double* obs,
+                                    double* d, void* stream);
+int elfi_b200_sim_gauss_nd_f64(elfi_b200_ctx* ctx, const double* mu, int64_t ld_b, int64_t ld_j,
+                               int64_t B, int64_t D, const double* A_host, int64_t n_obs,
+                               uint64_t seed, uint64_t offset, double* Y, int64_t ldY, double* S,
+                               int64_t ldS, void* stream);
+
 /* M/G/1 queue of elfi/examples/mg1.py (throughput mode, statistical parity); stream layout, thread
  * layout and arithmetic in elfi_b200/csrc/mg1.cu and mg1.cuh.  Rows where the reference's NumPy
  * raises (1/t3 with its sign bit set, t2 - t1 not finite) give NaN data and NaN quantiles.
