@@ -60,6 +60,8 @@ struct elfi_b200_ctx {
     // the GP Cholesky look-ahead's second stream and its two ordering events (gp.cu)
     cudaStream_t side_stream;
     cudaEvent_t side_event[2];
+    // the simulators compiled by elfi_b200_usersim_compile, a list (usersim.cu)
+    elfi_b200_usersim* usersims;
 };
 
 namespace elfi {
@@ -67,6 +69,9 @@ namespace elfi {
 // Returns a device pointer to at least `bytes` of scratch (256-byte aligned), or nullptr
 // after set_error().  Growth synchronises the device: it only happens on the first calls.
 void* ctx_scratch(elfi_b200_ctx* ctx, size_t bytes);
+
+// Frees every simulator of elfi_b200_usersim_compile the context holds (usersim.cu).
+void usersim_free_all(elfi_b200_ctx* ctx);
 
 // Encodes a rank-2 fp64 tensor map over a row-major (rows, cols) matrix with leading
 // dimension `ld` (elements) and a (box_rows x 16) box, 128-byte swizzle.

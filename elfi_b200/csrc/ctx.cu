@@ -108,6 +108,7 @@ int elfi_b200_ctx_destroy(elfi_b200_ctx* ctx) {
     if (!ctx) return ELFI_B200_OK;
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
+    elfi::usersim_free_all(ctx);
     if (ctx->scratch) cudaFree(ctx->scratch);
     if (ctx->side_stream) cudaStreamDestroy(ctx->side_stream);
     for (int i = 0; i < 2; ++i)

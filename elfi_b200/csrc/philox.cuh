@@ -4,7 +4,9 @@
 // Random123 known-answer vectors and against the NumPy replay in oracle/streams.py).
 #pragma once
 
+#if !defined(__CUDACC_RTC__)   // NVRTC has no C headers: usersim_rt.cuh declares the types
 #include <stdint.h>
+#endif
 
 #include "hd.cuh"
 

@@ -2711,3 +2711,167 @@ def linear_adjust(S, theta, observed, tol=1e-6):
             fits[k] = dict(coef=coef[:, kk].copy(), intercept=float(intercept[kk]), rank=rank,
                            singular=singular.copy(), n_rows=n)
     return adjusted, fits
+
+
+# ---- user-written simulators, compiled at run time (csrc/usersim.cu, csrc/usersim_rt.cuh) ---------
+USERSIM_P_MAX = _lib.CONSTANTS['USERSIM_P_MAX']
+USERSIM_N_OUT_MAX = _lib.CONSTANTS['USERSIM_N_OUT_MAX']
+USERSIM_N_SUM_MAX = _lib.CONSTANTS['USERSIM_N_SUM_MAX']
+USERSIM_LOCAL_MAX = _lib.CONSTANTS['USERSIM_LOCAL_MAX']
+_USERSIM_LOG_CHARS = 1 << 16
+_usersim_refs = {}        # (device, handle address) -> references taken by usersim_compile
+_usersim_compiled = [0]   # NVRTC compilations run by usersim_compile
+
+
+class UserSimulator:
+    """A simulator compiled by :func:`usersim_compile` for one device: its library handle and the
+    shapes it was compiled for."""
+
+    def __init__(self, handle, device, n_params, n_out, n_summaries, salt):
+        self.handle = handle
+        self.device = device
+        self.n_params = n_params
+        self.n_out = n_out
+        self.n_summaries = n_summaries
+        self.salt = salt
+
+
+def _count(value, lo, hi, what):
+    if isinstance(value, (bool, np.bool_)) or int(value) != value or not lo <= value <= hi:
+        raise ValueError('a user simulator takes an integer {} <= {} <= {}, got {!r}'.format(
+            lo, what, hi, value))
+    return int(value)
+
+
+def usersim_shapes(n_params, n_out, n_summaries=0, salt=0):
+    """(n_params, n_out, n_summaries, salt) as ints, or ValueError when one is out of the range
+    elfi_b200.h gives it."""
+    return (_count(n_params, 1, USERSIM_P_MAX, 'n_params'),
+            _count(n_out, 1, USERSIM_N_OUT_MAX, 'n_out'),
+            _count(n_summaries, 0, USERSIM_N_SUM_MAX, 'n_summaries'),
+            _count(salt, 0, 2 ** 32 - 1, 'salt'))
+
+
+def usersim_compile(source, n_params, n_out, n_summaries=0, salt=0):
+    """Compile a user's CUDA simulator for the current device (NVRTC, sm_90a) and load it.
+
+    ``source`` defines ``__device__ void simulate(const double* theta, elfi::RowStream& rng,
+    double* y)``, which writes the n_out values of one row from its n_params parameters, and, when
+    n_summaries > 0, ``__device__ void summarise(const double* y, double* s)``, which writes a
+    row's n_summaries summaries; elfi_b200/csrc/usersim_rt.cuh states the contract.  ``salt`` is
+    the fourth counter word of the simulator's Philox blocks.  The context caches compiled sources:
+    the same (source, shapes, salt) again returns the same simulator without running NVRTC.
+
+    Returns a :class:`UserSimulator`.  Shapes are checked before anything is compiled (ValueError);
+    a source NVRTC refuses raises ElfiB200Error carrying NVRTC's log, whose line numbers are the
+    source's own."""
+    if not isinstance(source, str) or not source.strip():
+        raise ValueError('the simulator source must be a non-empty string')
+    n_params, n_out, n_summaries, salt = usersim_shapes(n_params, n_out, n_summaries, salt)
+    ctx = dev.context()
+    device = dev.current_device()
+    log = ctypes.create_string_buffer(_USERSIM_LOG_CHARS)
+    handle = ctypes.c_void_p()
+    try:
+        _lib.call('elfi_b200_usersim_compile', ctx, source.encode('utf-8'), n_params, n_out,
+                  n_summaries, salt, log, len(log), ctypes.byref(handle))
+    except _lib.ElfiB200Error as e:
+        text = log.value.decode('utf-8', 'replace')
+        if not text:
+            raise
+        hint = ''
+        if 'Unresolved extern function' in text:
+            hint = ('\nThe source must define __device__ void simulate(const double* theta, '
+                    'elfi::RowStream& rng, double* y){}.'.format(
+                        ' and __device__ void summarise(const double* y, double* s)'
+                        if n_summaries else ''))
+        raise _lib.ElfiB200Error('NVRTC could not compile the user simulator:\n{}{}'.format(
+            text, hint)) from e
+    key = (device, handle.value)
+    if key not in _usersim_refs:
+        _usersim_compiled[0] += 1
+    _usersim_refs[key] = _usersim_refs.get(key, 0) + 1
+    return UserSimulator(handle, device, n_params, n_out, n_summaries, salt)
+
+
+def usersim_compiles():
+    """How many times :func:`usersim_compile` has run NVRTC in this process (cache hits do not
+    count)."""
+    return _usersim_compiled[0]
+
+
+def usersim_release(sim):
+    """Give back the reference :func:`usersim_compile` took; the last one frees the simulator."""
+    key = (sim.device, sim.handle.value)
+    if _usersim_refs.get(key, 0) <= 0:
+        raise ValueError('this user simulator has been released already')
+    _lib.call('elfi_b200_usersim_release', dev.context(sim.device), sim.handle)
+    _usersim_refs[key] -= 1
+    if _usersim_refs[key] == 0:
+        del _usersim_refs[key]
+        sim.handle = ctypes.c_void_p()
+
+
+def _usersim_ctx(sim):
+    if (sim.device, sim.handle.value) not in _usersim_refs:
+        raise ValueError('this user simulator has been released')
+    if dev.current_device() != sim.device:
+        raise ValueError('the user simulator was compiled for cuda:{}, the current device is '
+                         'cuda:{}'.format(sim.device, dev.current_device()))
+    return dev.context(sim.device)
+
+
+def usersim_run(sim, params, seed=0, offset=0, want_data=False, want_summaries=True):
+    """Run a :class:`UserSimulator` on a batch: row i has parameters ``params[j][i]`` (n_params
+    columns of one length, device or host; or one (batch, n_params) matrix) and is row offset + i
+    of the Philox stream keyed by ``seed``, so a row does not depend on how a batch is split.
+
+    Returns (Y, S), each None unless asked for: Y (batch, n_out) the data and S (batch,
+    n_summaries) the summaries.  Summaries without the data are computed in the simulator's
+    kernel without writing the data when n_out <= USERSIM_LOCAL_MAX, bit for bit the summaries of
+    a run that writes it."""
+    if not (want_data or want_summaries):
+        raise ValueError('usersim_run asked for neither the data nor the summaries')
+    if want_summaries and sim.n_summaries == 0:
+        raise ValueError('the user simulator has no summaries (n_summaries = 0)')
+    if isinstance(params, (list, tuple)):
+        cols = [dev.to_device(c).reshape(-1).contiguous() for c in params]
+    else:
+        P = _matrix(params)
+        cols = [P[:, j].contiguous() for j in range(P.shape[1])]
+    if len(cols) != sim.n_params:
+        raise ValueError('the user simulator takes {} parameters, got {}'.format(
+            sim.n_params, len(cols)))
+    B = int(cols[0].numel())
+    if any(int(c.numel()) != B for c in cols):
+        raise ValueError('the parameter columns must have one length, got {}'.format(
+            [int(c.numel()) for c in cols]))
+    ctx = _usersim_ctx(sim)
+    fused = want_summaries and not want_data and sim.n_out <= USERSIM_LOCAL_MAX
+    Y = None if fused else dev.empty((B, sim.n_out))
+    S = dev.empty((B, sim.n_summaries)) if want_summaries else None
+    mode = 2 if fused else (1 if want_summaries else 0)
+    ptrs = (ctypes.c_void_p * len(cols))(*[c.data_ptr() for c in cols])
+    _lib.call('elfi_b200_usersim_launch', ctx, sim.handle, ptrs, B, int(seed), int(offset), mode,
+              dev.ptr(Y), sim.n_out, dev.ptr(S), max(1, sim.n_summaries), dev.stream_ptr())
+    return (Y if want_data else None), S
+
+
+def usersim_summarise(sim, y):
+    """The summaries a :class:`UserSimulator`'s ``summarise`` gives the rows of y (batch, n_out)
+    or the one row y (n_out,): observed data, say, or data kept in a sample.  Returns S (batch,
+    n_summaries)."""
+    y = y if dev.is_device_array(y) else np.asarray(y, dtype=np.float64)
+    if sim.n_summaries == 0:
+        raise ValueError('the user simulator has no summaries (n_summaries = 0)')
+    Y = _matrix(y.reshape(1, -1) if y.ndim == 1 else y)
+    if Y.shape[1] != sim.n_out:
+        raise ValueError('the user simulator summarises rows of {} values, got shape {}'.format(
+            sim.n_out, tuple(Y.shape)))
+    B = int(Y.shape[0])
+    ctx = _usersim_ctx(sim)
+    S = dev.empty((B, sim.n_summaries))
+    ptrs = (ctypes.c_void_p * 1)()
+    _lib.call('elfi_b200_usersim_launch', ctx, sim.handle, ptrs, B, 0, 0, 3, dev.ptr(Y),
+              _ld(Y), dev.ptr(S), sim.n_summaries, dev.stream_ptr())
+    return S

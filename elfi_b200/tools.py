@@ -1,15 +1,21 @@
 """Graph helpers (mirror of elfi/model/tools.py): ``vectorize`` turns a simulator written for one
 parameter set into one that takes a batch, by calling it once per row, and
 ``external_operation`` turns a command line (a shell script or an executable) into an operation
-that runs it on a subprocess."""
+that runs it on a subprocess.  ``cuda_simulator`` turns a CUDA function that simulates one row
+into a throughput-mode simulator, and ``fused_summary`` reads the summaries it computes."""
 import subprocess
 from functools import partial
 
 import numpy as np
 
+from . import device as dev
+from . import ops
 from .model import get_sub_seed
+from .throughput import LazySimulation, batch_columns, batch_key
 
-__all__ = ['vectorize', 'external_operation']
+__all__ = ['vectorize', 'external_operation', 'cuda_simulator', 'fused_summary']
+
+USERSIM_SALT = 0x55534552   # "USER": the default salt of cuda_simulator's streams
 
 
 def _is_array(x):
@@ -180,3 +186,85 @@ def external_operation(command, process_result=None, prepare_inputs=None, sep=' 
     return partial(run_external, command, process_result=process_result,
                    prepare_inputs=prepare_inputs, stdout=stdout,
                    subprocess_kwargs=subprocess_kwargs)
+
+
+def cuda_simulator(source, n_params, n_out, n_summaries=0, salt=USERSIM_SALT):
+    """A throughput-mode simulator from CUDA source that simulates one row.
+
+    ``source`` defines ``__device__ void simulate(const double* theta, elfi::RowStream& rng,
+    double* y)``, which writes the ``n_out`` values ``y[0 .. n_out)`` of one row from its
+    ``n_params`` parameters, and, when ``n_summaries`` > 0, ``__device__ void summarise(const
+    double* y, double* s)``, which writes that row's summaries.  ``rng`` is the row's Philox
+    stream: ``rng.normal2(m, n0, n1)`` / ``rng.uniform2(m, u0, u1)`` give the two normals /
+    uniforms of block m, ``rng.block(m)`` its raw words, and ``rng.next_normal()`` /
+    ``rng.next_uniform()`` draw blocks in order.  ``elfi::n_params``, ``elfi::n_out`` and
+    ``elfi::n_sum`` are the shapes.  elfi_b200/csrc/usersim_rt.cuh states the contract.
+
+    The source is compiled for the H100 (NVRTC, sm_90a) on the first call on a device, and the
+    compiled code is kept for the same source, shapes and salt.  A compile error raises
+    ElfiB200Error carrying NVRTC's log.
+
+    Returns ``simulator(*params, batch_size=1, random_state=None)``, whose output is a
+    LazySimulation of shape (batch_size, n_out): ``summaries()`` runs simulate and summarise in
+    one kernel without writing the data (when n_out <= ops.USERSIM_LOCAL_MAX), and
+    ``materialize()`` writes the data.  Each call draws its Philox key from ``random_state``, as
+    the built-in throughput-mode simulators do, so a run is a function of its seed.
+    ``simulator.summarise(y)`` gives the summaries of data such as the observed rows.
+
+    Example::
+
+        sim = elfi_b200.tools.cuda_simulator(MA2_SOURCE, 2, 100, n_summaries=2)
+        elfi_b200.Simulator(sim, m['t1'], m['t2'], observed=y_obs, name='MA2')
+        elfi_b200.Summary(elfi_b200.tools.fused_summary(0, sim), m['MA2'], name='S1')
+    """
+    if not isinstance(source, str) or not source.strip():
+        raise ValueError('the simulator source must be a non-empty string')
+    n_params, n_out, n_summaries, salt = ops.usersim_shapes(n_params, n_out, n_summaries, salt)
+    compiled = {}
+
+    def on_device():
+        device = dev.current_device()
+        if device not in compiled:
+            compiled[device] = ops.usersim_compile(source, n_params, n_out, n_summaries, salt)
+        return compiled[device]
+
+    def summaries(sim, cols, key, kind):
+        if n_summaries == 0:
+            raise ValueError('this CUDA simulator has no summaries (n_summaries = 0)')
+        return ops.usersim_run(sim, cols, seed=key)[1]
+
+    def simulator(*params, batch_size=1, random_state=None):
+        if len(params) != n_params:
+            raise ValueError('this CUDA simulator takes {} parameters, got {}'.format(
+                n_params, len(params)))
+        cols = batch_columns(params, batch_size)
+        key = batch_key(random_state)
+        sim = on_device()
+        return LazySimulation(
+            (int(cols[0].numel()), n_out), partial(summaries, sim, cols, key),
+            lambda: ops.usersim_run(sim, cols, seed=key, want_data=True, want_summaries=False)[0])
+
+    simulator.summarise = lambda y: ops.usersim_summarise(on_device(), y)
+    return simulator
+
+
+def fused_summary(columns, simulator=None):
+    """A summary operation that reads columns of the summaries a :func:`cuda_simulator` computes.
+
+    ``columns`` is one column index (the summary is (batch,)) or a list of them ((batch, k)).  The
+    summaries of a simulator output come from its kernel.  Data that did not come from the
+    simulator, such as the observed data, is summarised by ``simulator.summarise``, so pass the
+    simulator when the model has observed data; without it such data raises ValueError."""
+    index = int(columns) if np.ndim(columns) == 0 else [int(c) for c in columns]
+
+    def summary(x):
+        if isinstance(x, LazySimulation):
+            S = x.summaries()
+        elif simulator is not None:
+            S = simulator.summarise(x)
+        else:
+            raise ValueError('fused_summary reads the summaries of a cuda_simulator output; '
+                             'to summarise other data, such as the observed data, give it the '
+                             'simulator: fused_summary(columns, simulator)')
+        return S[:, index]
+    return summary

@@ -1286,6 +1286,54 @@ int elfi_b200_romc_posterior_unnorm_f64(elfi_b200_ctx* ctx, int64_t M, int64_t R
                                         const double* fvals, int64_t ld_f, double eps,
                                         const double* prior, double* out, void* stream);
 
+/* ---- user-written simulators, compiled at run time (throughput mode) ------------------------
+ * elfi_b200_usersim_compile: compiles a user's CUDA source for this context's device (sm_90a) with
+ * NVRTC and loads it.  The source defines
+ *   __device__ void simulate(const double* theta, elfi::RowStream& rng, double* y);
+ * (one row: p parameters in, n_out doubles out) and, when n_sum > 0,
+ *   __device__ void summarise(const double* y, double* s);
+ * (one row's n_sum summaries); elfi_b200/csrc/usersim_rt.cuh, which NVRTC compiles before the
+ * source, declares both, elfi::RowStream and the harness kernel, and is all the source sees.
+ * NVRTC runs with --gpu-architecture=sm_90a -std=c++17, the directory of usersim_rt.cuh (csrc/
+ * beside the library's lib/ directory) as include path, and the salt and shapes as macros that the
+ * source reads as elfi::n_params, elfi::n_out and elfi::n_sum.  Line numbers in the NVRTC log are
+ * the source's own.
+ *   salt     the fourth Philox counter word of every block of the simulator's stream (< 2^32).
+ *   log      (log_len chars, HOST, may be NULL): on a compile error, the NVRTC log, truncated and
+ *            NUL-terminated; "" otherwise.  A compile error returns ELFI_B200_ERR_ARG.
+ *   handle   out: the compiled simulator.  The context caches simulators by (source, p, n_out,
+ *            n_sum, salt): compiling a cached one again returns the same handle without running
+ *            NVRTC and counts one more reference.
+ * Limits: 1 <= p <= ELFI_B200_USERSIM_P_MAX, 1 <= n_out <= ELFI_B200_USERSIM_N_OUT_MAX,
+ * 0 <= n_sum <= ELFI_B200_USERSIM_N_SUM_MAX.  Synchronous; a first compile takes about 0.5 s.
+ *
+ * elfi_b200_usersim_launch: rows i < B of one call, one thread per row.  Row i uses parameter
+ * theta_cols_host[j][i] (p DEVICE pointers in a HOST array) and is row offset + i of the stream
+ * keyed by `key`, so a row does not depend on how a batch is split into calls.  Modes:
+ *   0  data: simulate into Y[i * ldY + 0 .. n_out)                               (S unused)
+ *   1  data and summaries: mode 0, then summarise that row into S[i * ldS + 0 .. n_sum)
+ *   2  fused summaries: simulate into a thread-local row and summarise it into S; the data is never
+ *      written (Y unused).  Needs n_out <= ELFI_B200_USERSIM_LOCAL_MAX.  Bit for bit mode 1's S.
+ *   3  summaries of given data: summarise Y's row i into S (no simulation, theta_cols_host unused)
+ * Modes 1-3 need n_sum > 0.  ldY >= n_out and ldS >= n_sum where used.  Asynchronous on `stream`;
+ * a fault inside the user's code is reported by the stream, as for any kernel.
+ *
+ * elfi_b200_usersim_release: drops one reference; the last frees the simulator (synchronises the
+ * device first).  Destroying the context frees every simulator it holds. */
+#define ELFI_B200_USERSIM_P_MAX 16          /* parameters of a row: the prior table's */
+#define ELFI_B200_USERSIM_N_OUT_MAX 16777216   /* 2^24: 64 n_out still fits an int */
+#define ELFI_B200_USERSIM_N_SUM_MAX 4096    /* summaries of a row; the distances read whole rows */
+#define ELFI_B200_USERSIM_LOCAL_MAX 1024    /* n_out of mode 2: the row in 8 KiB of local memory */
+typedef struct elfi_b200_usersim elfi_b200_usersim;
+int elfi_b200_usersim_compile(elfi_b200_ctx* ctx, const char* source, int64_t p, int64_t n_out,
+                              int64_t n_sum, uint64_t salt, char* log, int64_t log_len,
+                              elfi_b200_usersim** handle);
+int elfi_b200_usersim_launch(elfi_b200_ctx* ctx, const elfi_b200_usersim* handle,
+                             const double* const* theta_cols_host, int64_t B, uint64_t key,
+                             uint64_t offset, int32_t mode, double* Y, int64_t ldY, double* S,
+                             int64_t ldS, void* stream);
+int elfi_b200_usersim_release(elfi_b200_ctx* ctx, elfi_b200_usersim* handle);
+
 #ifdef __cplusplus
 }
 #endif
